@@ -42,34 +42,41 @@ if ROOT not in sys.path:
 METRIC = "net_forward images/sec @256x256"   # --size 512 reports the same metric name with the size in config
 X = 256
 PER_GPU_BATCH = 64
-NCU_TRAFFIC_CSV = os.path.join(ROOT, "profiles", "r02_ncu_full_batch64_forward.csv")
 
 
-def _ncu_traffic(batch, size):
-    """dram__bytes_read + dram__bytes_write per launch of the dominant kernel (mean over the 25 umma_conv launches of
-    the regression trunk), from the committed `ncu --set full` capture of this same workload at HEAD
-    (profiles/r02_ncu_full_batch64_forward.csv, written by tools/ncu_summary.py)."""
-    if batch != 64 or size != 256 or not os.path.isfile(NCU_TRAFFIC_CSV):
-        return None
-    import csv
-    rows = list(csv.reader(l for l in open(NCU_TRAFFIC_CSV) if not l.startswith("#")))
-    h = rows[0]
-    tot, n = 0.0, 0
-    for r in rows[1:]:
-        d = dict(zip(h, r))
-        if d["kernel"].startswith("umma_conv_kernel") and d["op"] != "class":
-            tot += (float(d["dram_read_MB"]) + float(d["dram_write_MB"])) * 1e6
-            n += 1
-    return tot / n if n else None
+H100_DATASHEET = {"tensor": 989.0, "tensor_burst": 989.0, "hbm": 3350.0}   # dense FP16 TFLOP/s, HBM3 GB/s (700 W SXM)
 
 
 def _peaks():
+    """Measured peaks from MEASURED_PEAKS.json where present; every value it lacks is the H100 SXM data sheet's."""
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.isfile(p):
         d = json.load(open(p))
-        return {"tensor": d.get("bf16_tflops_sustained", 1370.8), "tensor_burst": d.get("bf16_tflops", 1653.3),
-                "hbm": d.get("hbm_gbs", 6569.6), "src": "measured (MEASURED_PEAKS.json, sustained bf16 cuBLAS)"}
-    return {"tensor": 1400.0, "tensor_burst": 1590.0, "hbm": 6650.0, "src": "fallback (B200_PROFILING.md)"}
+        got = {"tensor": d.get("bf16_tflops_sustained"), "tensor_burst": d.get("bf16_tflops"), "hbm": d.get("hbm_gbs")}
+        out = {k: (v if v is not None else H100_DATASHEET[k]) for k, v in got.items()}
+        missing = sorted(k for k, v in got.items() if v is None)
+        out["src"] = "measured (MEASURED_PEAKS.json, sustained bf16 cuBLAS)" + (
+            "; H100 SXM data sheet for %s" % ", ".join(missing) if missing else "")
+        return out
+    return dict(H100_DATASHEET, src="H100 SXM data sheet (dense FP16 tensor, HBM3; 700 W card), not measured")
+
+
+DUMP_CAP_BYTES = 64 << 20
+
+
+def dump_ab(dirname, ab):
+    """Write what the timed path returned in its last step, the [N, 2, X, X] ab map, as DIR/ab.npy (float32).  Above
+    64 MB a fixed, seeded sample of whole images is written instead (sorted image indices in DIR/ab_images.npy), so two
+    builds run with the same arguments dump the same images."""
+    os.makedirs(dirname, exist_ok=True)
+    per_image = ab[0].size * 4
+    n = ab.shape[0]
+    if n * per_image > DUMP_CAP_BYTES:
+        keep = max(1, (DUMP_CAP_BYTES - 65536) // per_image)      # room for the .npy headers and the index file
+        idx = np.sort(np.random.RandomState(12345).choice(n, keep, replace=False))
+        np.save(os.path.join(dirname, "ab_images.npy"), idx.astype(np.int64))
+        ab = ab[idx]
+    np.save(os.path.join(dirname, "ab.npy"), np.ascontiguousarray(ab, dtype=np.float32))
 
 
 def workload_config(N, size, world):
@@ -79,7 +86,7 @@ def workload_config(N, size, world):
                         "regression head (ab map)" % ("3" if size == 256 else "4 (no global hints)", N, size, size),
             "per_gpu_batch": N, "global_batch": N * world,
             "parallelism": "dp%d (image sharding, no per-step collective)" % world,
-            "l2_policy": "per-step working set (~%.1f GB of activations) >> 126 MB L2; inputs are not re-used from L2"
+            "l2_policy": "per-step working set (~%.1f GB of activations) >> 50 MB L2; inputs are not re-used from L2"
                          % (N * 0.15 * (size / 256.0) ** 2)}
 
 
@@ -475,6 +482,8 @@ def run_ours(args):
     clocks = sampler.finish(t_region0, t_region1) if sampler else None
     ms_step = ms_total / args.steps
     value = world * N / (ms_step * 1e-3)
+    if args.dump_outputs and rank == 0:
+        dump_ab(args.dump_outputs, out.cpu().numpy())      # the whole map at the default 64 x 256^2 (32 MB)
 
     # ---- per-op device times: separate untimed pass (events between the launches, PDL off by construction) ----
     ctx.set_profiling(True)
@@ -523,11 +532,10 @@ def run_ours(args):
     achieved = conv_flops / (conv_ms * 1e-3) / 1e12 if conv_ms > 0 else 0.0
     n_launch = sum(1 for _ in conv)
     split = 1.0 if args.fast_fp16 else 3.0
-    roofline = {"bound": "tensor", "kernel": "umma_conv_kernel<BN,MT,CG,SPLIT,HALO> (tcgen05 implicit-GEMM conv, %d launches/step)" % n_launch,
+    roofline = {"bound": "tensor", "kernel": "umma_conv_kernel<BN,SPLIT> (wgmma implicit-GEMM conv, %d launches/step)" % n_launch,
                 "achieved": achieved, "peak": peaks["tensor"], "unit": "TFLOP/s", "frac": achieved / peaks["tensor"],
                 "issued_mma_frac": split * achieved / peaks["tensor"],
-                "peak_source": peaks["src"], "traffic": _ncu_traffic(N, X),
-                "traffic_note": "average DRAM bytes per umma_conv launch (ncu --set full at HEAD, profiles/%s)" % os.path.basename(NCU_TRAFFIC_CSV),
+                "peak_source": peaks["src"],
                 "algorithmic_flops_per_launch": conv_flops / max(n_launch, 1),
                 "avg_launch_ms": conv_ms / max(n_launch, 1),
                 "kernel_share_of_step": min(1.0, conv_ms / ms_step),
@@ -578,7 +586,12 @@ def main():
     ap.add_argument("--fast-fp16", action="store_true",
                     help="NOT the parity configuration: single-pass FP16 operands (1 MMA per product, ~6e-2 ab error)")
     ap.add_argument("--skip-e2e", action="store_true", help="profiling runs only: skip the e2e, config 4 and latency legs")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's ab map (rank 0) as DIR/ab.npy (float32; a "
+                         "seeded sample of images above 64 MB)")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs writes the GPU path's outputs; the reference arm has none to write")
     if args.impl == "reference":
         return run_reference(args)
     return run_ours(args)

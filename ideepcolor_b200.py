@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Headless front end of the B200 backend (SURVEY row f4).
+"""Headless front end of the H100 backend (SURVEY row f4).
 
 The reference's entry point (`ideepcolor.py:60-86`) builds a colour model + a distribution model and hands them
 to a PyQt window; its `Save` button writes a result folder (`ui/gui_draw.py:222-244`).  PyQt is not part of this
@@ -23,7 +23,7 @@ import numpy as np
 
 
 def parse_args(argv=None):
-    ap = argparse.ArgumentParser(description="iDeepColor on the B200 backend, headless")
+    ap = argparse.ArgumentParser(description="iDeepColor on the H100 backend, headless")
     ap.add_argument("--image_file", default="test_imgs/mortar_pestle.jpg", help="input image")
     ap.add_argument("--color_model", required=True, help="state_dict (.pth) of the reference PyTorch model")
     ap.add_argument("--hints", default="", help="JSON list of hints; empty = automatic colorization")

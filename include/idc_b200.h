@@ -1,5 +1,5 @@
 /*
- * idc_b200.h -- C ABI of the B200-native Local Hints Network forward
+ * idc_b200.h -- C ABI of the H100-native Local Hints Network forward
  * (interactive deep colorization hot path).
  *
  * The reference has NO native interface: its operator boundary for this path is the
@@ -44,14 +44,14 @@ enum {
   IDC_ERR_CUDA = -2,         /* a CUDA call or kernel failed                        */
   IDC_ERR_STATE = -3,        /* wrong call order (e.g. forward before finalize)     */
   IDC_ERR_KEY = -4,          /* unknown / missing state_dict key                    */
-  IDC_ERR_UNSUPPORTED = -5,  /* e.g. not an sm_100 device                           */
+  IDC_ERR_UNSUPPORTED = -5,  /* e.g. not an sm_90 device                            */
   IDC_ERR_WATCHDOG = -6      /* a device-side pipeline wait timed out               */
 };
 
 /* idc_create flags */
 enum {
   IDC_FLAG_DIST = 1u << 0,        /* also run model_class + softmax (model.py:159-160)           */
-  IDC_FLAG_ENGINE_SIMT = 1u << 1, /* FP32 CUDA-core engine (exact FP32, slow); default = tcgen05 */
+  IDC_FLAG_ENGINE_SIMT = 1u << 1, /* FP32 CUDA-core engine (exact FP32, slow); default = wgmma */
   IDC_FLAG_FAST_FP16 = 1u << 2,   /* single-pass FP16 operands (1 MMA / product, ~6e-2 ab error);
                                      default = 2-term split FP16 (3 MMAs / product, <=1e-3)      */
   IDC_FLAG_GLOBAL_HINTS = 1u << 3,/* global-hints branch (models/global_model/deploy_nodist.prototxt:38-172,501-527) */
@@ -63,7 +63,7 @@ enum {
 /* dtype codes for idc_load_tensor */
 enum { IDC_F32 = 0, IDC_F64 = 1, IDC_I64 = 2 };
 
-/* Library / build info: "idc_b200 <version> sm_100a ..." */
+/* Library / build info: "idc_b200 <version> sm_90a ..." */
 const char* idc_version(void);
 
 /* Replaces `model.SIGGRAPHGenerator(dist=dist)` + `.cuda()` + `.eval()`
@@ -74,17 +74,11 @@ int idc_create(int device, int max_n, int h, int w, unsigned flags, idc_ctx** ou
  * must not read process-global state).  Call between idc_create and idc_finalize_weights / idc_adopt_weights;
  * a later call re-plans the launches.  -1 = automatic where it applies.
  *   "halo"          0 / 1 / 3   halo-tile A operand (one TMA tile per 64 input channels serves all 9 taps)
- *   "pairs"         0 / 1 / 2   cta_group::2 CTA pairs: never / large launches / always
- *   "mt"            1 / 2       128-pixel M-tiles per CTA tile on the <= 128-column layers
- *   "chunk_kb"      >= 1        k-blocks summed in TMEM before the FP32 round-to-nearest add (accuracy vs speed)
+ *   "pairs"         0 / 1 / 2   clusters of two CTAs sharing each weight tile: never (default) / large launches / always
+ *   "mt"            1 / 2       128-pixel M-tiles per CTA tile (2 runs the layer with 64-column tiles)
+ *   "chunk_kb"      >= 1        k-blocks summed inside the tensor core before the FP32 round-to-nearest add
  *   "split_k"       >= 1        K slices per tile on launches that cannot fill the machine
- *   "split_pairs"   0 / 1       run the split-K (small batch) launches as CTA pairs
- *   "split_bn128"   0 / 1       128-column tiles on the split-K path (default 1: half the reduction traffic per CTA)
- *   "halo_split"    0 / 1       halo-tile A operand on that path (experiment, measured slower; default 0)
- *   "chain"         0 / 1       the consecutive split-K layers as ONE launch with a grid barrier (measured equal; default 0)
- *   "prologue_sync2" 0 / 1      cluster barrier in front of the CTA pair's TMEM allocation (default 1; 0 is racecheck-dirty)
  *   "conv1_1_umma"  0 / 1       model1.0 on the tensor cores (default 1); 0 = the exact-FP32 CUDA-core kernel
- *   "direct_stores" 0 / 1       per-lane 16-byte stores instead of the warp-transposed ones
  *   "host_pipe"     0 / 1       idc_forward_host: chunked copy/compute overlap for batches >= 8
  *   "pdl"           0 / 1       programmatic dependent launch between the kernels of one forward
  *   "side_dist"     0 / 1       batches <= 4: run the dist head (class + softmax) on a side stream / graph branch
@@ -101,7 +95,7 @@ int idc_load_tensor(idc_ctx* ctx, const char* key, const void* data, int dtype, 
                     const int64_t* dims);
 
 /* Packs every loaded tensor into the device-resident weight arena (K-major FP16 hi/lo
- * tiles for tcgen05, FP32 [K][Cout] for the SIMT engine; BatchNorm folded to scale/shift).
+ * tiles for wgmma, FP32 [K][Cout] for the SIMT engine; BatchNorm folded to scale/shift).
  * Fails with IDC_ERR_KEY if a required key is missing. */
 int idc_finalize_weights(idc_ctx* ctx);
 

@@ -1,4 +1,4 @@
-"""B200-native forward pass of the Interactive Deep Colorization Local Hints Network.
+"""H100-native forward pass of the Interactive Deep Colorization Local Hints Network.
 
 Public surface (drop-in for /root/reference/data/colorize_image.py and
 /root/reference/models/pytorch/model.py):
@@ -8,7 +8,7 @@ Public surface (drop-in for /root/reference/data/colorize_image.py and
     engine.LhnContext                                           batched / device-tensor API
     parallel.ShardedColorizer                                   one process per GPU, image sharding
 
-Everything numerical runs in lib/libidc_b200.so (hand-written sm_100a CUDA, csrc/); importing
+Everything numerical runs in lib/libidc_b200.so (hand-written sm_90a CUDA, csrc/); importing
 the package does not load it, the first network call does -- and raises if it is missing.
 """
 __version__ = "0.1.0"

@@ -9,7 +9,7 @@ import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libidc_b200.so")
-if os.environ.get("IDC_B200_LIB"):            # tools only: an instrumented build (make COUNTERS=1 OUT=...)
+if os.environ.get("IDC_B200_LIB"):            # tools only: a build elsewhere (make OUT=...)
     LIB_PATH = os.environ["IDC_B200_LIB"]
 
 IDC_OK = 0

@@ -1,4 +1,4 @@
-"""Host-side mirror of the reference wrapper classes, backed by the B200 engine.
+"""Host-side mirror of the reference wrapper classes, backed by the H100 engine.
 
 API kept verbatim from /root/reference/data/colorize_image.py so `ideepcolor.py:62-72`, the Qt
 GUI (`ui/gui_draw.py:109-113,258-286`) and the notebooks work unchanged:
@@ -163,7 +163,7 @@ class ColorizeImageBase(object):
 class ColorizeImageB200(ColorizeImageBase):
     """<-> ColorizeImageTorch (reference :201-276)."""
 
-    def __init__(self, Xd=256, maskcent=False, engine="tcgen05", fast_fp16=False, gpu_prepost=True):
+    def __init__(self, Xd=256, maskcent=False, engine="wgmma", fast_fp16=False, gpu_prepost=True):
         print('ColorizeImageB200 instantiated')
         self.gpu_prepost = gpu_prepost    # quantised output_ab and the full-res render on the GPU (row f1)
         ColorizeImageBase.__init__(self, Xd)
@@ -384,7 +384,7 @@ class _LazyUpsampledDist(object):
 class ColorizeImageB200Dist(ColorizeImageB200):
     """<-> ColorizeImageTorchDist (reference :279-372)."""
 
-    def __init__(self, Xd=256, maskcent=False, engine="tcgen05", fast_fp16=False, materialize_full=False):
+    def __init__(self, Xd=256, maskcent=False, engine="wgmma", fast_fp16=False, materialize_full=False):
         ColorizeImageB200.__init__(self, Xd, engine=engine, fast_fp16=fast_fp16)
         self.dist_ab_set = False
         self.pts_grid = np.array(np.meshgrid(np.arange(-110, 120, 10), np.arange(-110, 120, 10))).reshape((2, 529)).T
@@ -505,7 +505,7 @@ class ColorizeImageB200GlobDist(ColorizeImageB200):
     weights arrive as extra state_dict keys `glob.{0..3}.*` (include/idc_b200.h).  Spec-only: no reference
     weights or vectors exist for it offline."""
 
-    def __init__(self, Xd=256, maskcent=False, engine="tcgen05"):
+    def __init__(self, Xd=256, maskcent=False, engine="wgmma"):
         ColorizeImageB200.__init__(self, Xd, maskcent=maskcent, engine=engine)
         self.glob_mask_mult = 1.
 
@@ -542,7 +542,7 @@ class ColorizeImageB200GlobDist(ColorizeImageB200):
 # =============================================================================================
 # Caffe-named wrapper surface (reference :375-442, :445-463, :466-561).  The notebooks and ideepcolor.py:60-65
 # instantiate ColorizeImageCaffe / ColorizeImageCaffeDist / ColorizeImageCaffeGlobDist; these classes keep those
-# names' semantics on the B200 engine:
+# names' semantics on the H100 engine:
 #   * Caffe scaling (SURVEY q4): the deploy nets feed RAW L-50, raw ab and mask x 110 into conv1_1 and scale the
 #     regression head by 100 (deploy_nodist.prototxt:19-51, :812-822; `self.mask_mult = 110.`, :383), where the
 #     PyTorch model feeds L/100, ab/110, mask and scales by 110.  The engine normalises the PyTorch way inside
@@ -571,7 +571,7 @@ class ColorizeImageB200Caffe(ColorizeImageB200):
     _caffe313 = False
     _global_hints = False
 
-    def __init__(self, Xd=256, engine="tcgen05"):
+    def __init__(self, Xd=256, engine="wgmma"):
         ColorizeImageB200.__init__(self, Xd, maskcent=False, engine=engine)
         self.mask_mult = 110.                     # reference :383
         self.pred_ab_layer = 'pred_ab'
@@ -611,7 +611,7 @@ class ColorizeImageB200CaffeGlobDist(ColorizeImageB200Caffe):
     """<-> ColorizeImageCaffeGlobDist (reference :445-463): additional 313-bin global histogram input."""
     _global_hints = True
 
-    def __init__(self, Xd=256, engine="tcgen05"):
+    def __init__(self, Xd=256, engine="wgmma"):
         ColorizeImageB200Caffe.__init__(self, Xd, engine=engine)
         self.glob_mask_mult = 1.
         self.glob_layer = 'glob_ab_313_mask'
@@ -660,7 +660,7 @@ class ColorizeImageB200CaffeDist(ColorizeImageB200Caffe):
     mean of the 313-bin head (deploy_nopred.prototxt:827-850), `dist_ab` the S-softened distribution (:808-820)."""
     _caffe313 = True
 
-    def __init__(self, Xd=256, engine="tcgen05"):
+    def __init__(self, Xd=256, engine="wgmma"):
         ColorizeImageB200Caffe.__init__(self, Xd, engine=engine)
         self.dist_ab_set = False
         self.scale_S_layer = 'scale_S'

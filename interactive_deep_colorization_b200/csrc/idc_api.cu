@@ -1,7 +1,7 @@
 // C ABI of libidc_b200.so (include/idc_b200.h): context, layer plan, weight packing, forward.
 // The plan restates the wiring of SIGGRAPHGenerator.forward
 // (/root/reference/models/pytorch/model.py:134-175) as a list of gather-GEMM ops; both engines
-// (idc_simt.cu FP32 CUDA cores, idc_umma.cu tcgen05) execute the same list.
+// (idc_simt.cu FP32 CUDA cores, idc_umma.cu wgmma) execute the same list.
 #include <math.h>
 #include <stdarg.h>
 #include <stdio.h>
@@ -473,10 +473,6 @@ int plan_engines(Ctx* c) {
     CUDA_TRY(c, cudaMalloc(&c->splitk_ws, c->splitk_ws_floats * sizeof(float)));
     CUDA_TRY(c, cudaMalloc(&c->splitk_counters, sizeof(int) * 2 * (size_t)c->splitk_max_tiles));
     CUDA_TRY(c, cudaMemset(c->splitk_counters, 0, sizeof(int) * 2 * (size_t)c->splitk_max_tiles));
-    if (!c->chain_bar) {
-      CUDA_TRY(c, cudaMalloc(&c->chain_bar, 256));
-      CUDA_TRY(c, cudaMemset(c->chain_bar, 0, 256));
-    }
   }
   return IDC_OK;
 }
@@ -568,19 +564,8 @@ int run_forward(Ctx* c, int n, const float* L, const float* ab, const float* mas
   // 128-CTA launches of the main chain leave idle, instead of sitting between c8_3 and up9 on the critical path.
   const bool side_dist = c->opt.side_dist && !c->simt && out_dist && n <= 4 && !hp && !ev;
   bool forked = false;
-  // chained launches: not while per-op events are recorded, not on the chunked large-batch path
-  const bool use_chain = c->opt.chain && !c->simt && !ev && !hp && c->chain_bar;
   for (size_t oi = 0; oi < c->ops.size(); ++oi) {
     ConvOp& op = c->ops[oi];
-    if (use_chain && umma_op_chainable(c, op)) {
-      size_t oj = oi;
-      while (oj + 1 < c->ops.size() && oj + 1 - oi < 20 && umma_op_chainable(c, c->ops[oj + 1])) ++oj;
-      if (oj > oi) {
-        CUDA_TRY(c, umma_run_chain(c, (int)oi, (int)oj, n, st));
-        oi = oj;
-        continue;
-      }
-    }
     if (side_dist && op.kind == OP_CLASS && op.name == "class") {
       if (!c->s_side) {
         CUDA_TRY(c, cudaStreamCreateWithFlags(&c->s_side, cudaStreamNonBlocking));
@@ -630,8 +615,8 @@ int run_forward(Ctx* c, int n, const float* L, const float* ab, const float* mas
       }
     } else {
       // announced click: the suggestion kernel (8 CTAs of 1024 threads, a whole SM each) runs on the side branch next
-      // to decoder levels 9-10; a 148-CTA launch would queue behind it on 8 SMs and finish that much later.  Leaving 8
-      // SMs free costs nothing: 512 tiles are 4 rounds on 148 and on 140 CTAs alike.
+      // to decoder levels 9-10; a full-width launch would queue behind it on 8 SMs and finish that much later.  Leaving 8
+      // SMs free costs little: 512 tiles are 4 rounds on 132 and on 124 CTAs alike.
       const int cap = (forked && c->click_mode && c->d_clickout) ? side_branch_cap(c) : 0;
       CUDA_TRY(c, umma_run_op(c, op, n, op.fuse_out_head ? out_ab : nullptr, (float)c->opt.tanh_scale, st, 0, cap));
     }
@@ -674,7 +659,7 @@ int check_forward_args(Ctx* c, int n, int h, int w, const void* L, const void* a
 // =============================================================================================
 extern "C" {
 
-const char* idc_version(void) { return "idc_b200 0.1 sm_100a (tcgen05 split-fp16 + fp32 simt engines)"; }
+const char* idc_version(void) { return "idc_b200 0.2 sm_90a (wgmma split-fp16 + fp32 simt engines)"; }
 
 int idc_create(int device, int max_n, int h, int w, unsigned flags, idc_ctx** out) {
   if (!out) return IDC_ERR_ARG;
@@ -684,7 +669,7 @@ int idc_create(int device, int max_n, int h, int w, unsigned flags, idc_ctx** ou
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || device < 0 || device >= ndev) return IDC_ERR_CUDA;
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return IDC_ERR_CUDA;
-  if (prop.major != 10) return IDC_ERR_UNSUPPORTED;  // sm_100a cubins only; no fallback
+  if (prop.major != 9 || prop.minor != 0) return IDC_ERR_UNSUPPORTED;  // sm_90a cubins only; no fallback
   if (cudaSetDevice(device) != cudaSuccess) return IDC_ERR_CUDA;
   idc_ctx* c = new idc_ctx();
   c->dev = device; c->max_n = max_n; c->H = h; c->W = w; c->flags = flags;
@@ -708,10 +693,10 @@ int idc_create(int device, int max_n, int h, int w, unsigned flags, idc_ctx** ou
 int idc_set_option(idc_ctx* c, const char* name, int value) {
   if (!c || !name) return IDC_ERR_ARG;
   struct { const char* n; int* v; } tab[] = {
-      {"halo", &c->opt.halo}, {"pairs", &c->opt.pairs}, {"mt", &c->opt.mt}, {"chunk_kb", &c->opt.chunk_kb},
-      {"split_k", &c->opt.split_k}, {"direct_stores", &c->opt.direct_stores}, {"host_pipe", &c->opt.host_pipe},
-      {"pdl", &c->opt.pdl}, {"split_pairs", &c->opt.split_pairs}, {"tanh_scale", &c->opt.tanh_scale},
-      {"side_dist", &c->opt.side_dist}, {"split_bn128", &c->opt.split_bn128}, {"halo_split", &c->opt.halo_split}, {"prologue_sync2", &c->opt.prologue_sync2}, {"chain", &c->opt.chain}, {"conv1_1_umma", &c->opt.conv1_1_umma}};
+      {"halo", &c->opt.halo}, {"pairs", &c->opt.pairs}, {"mt", &c->opt.mt},
+      {"chunk_kb", &c->opt.chunk_kb}, {"split_k", &c->opt.split_k}, {"host_pipe", &c->opt.host_pipe},
+      {"pdl", &c->opt.pdl}, {"tanh_scale", &c->opt.tanh_scale}, {"side_dist", &c->opt.side_dist},
+      {"conv1_1_umma", &c->opt.conv1_1_umma}};
   for (auto& t : tab)
     if (!strcmp(t.n, name)) {
       *t.v = value;
@@ -1391,23 +1376,6 @@ double idc_op_flops(idc_ctx* c, int i) {
   return (c && i >= 0 && i < (int)c->ops.size()) ? c->ops[i].flops_per_image : 0.0;
 }
 
-// experiments (tools/): per-CTA cycle counters of the LAST tcgen05 launch; out[148*16] long long (read + clear)
-extern "C" int idc_debug_counters(idc_ctx* c, int enable, long long* out_host) {
-  if (!c) return IDC_ERR_ARG;
-  CUDA_TRY(c, cudaSetDevice(c->dev));
-  if (enable && !c->dbgbuf) {
-    CUDA_TRY(c, cudaMalloc(&c->dbgbuf, 256 * 16 * sizeof(long long)));
-    CUDA_TRY(c, cudaMemset(c->dbgbuf, 0, 256 * 16 * sizeof(long long)));
-  }
-  if (out_host && c->dbgbuf) {
-    CUDA_TRY(c, cudaDeviceSynchronize());
-    CUDA_TRY(c, cudaMemcpy(out_host, c->dbgbuf, 148 * 16 * sizeof(long long), cudaMemcpyDeviceToHost));
-    CUDA_TRY(c, cudaMemset(c->dbgbuf, 0, 256 * 16 * sizeof(long long)));
-  }
-  if (!enable && c->dbgbuf) { cudaFree(c->dbgbuf); c->dbgbuf = nullptr; }
-  return IDC_OK;
-}
-
 // experiments (tools/click_breakdown.py): device time of the click graph (copy nodes included), measured with two
 // events around the graph launch.  enable = 1 / 0; returns the last span in *ms when non-null.
 extern "C" int idc_debug_graph_timing(idc_ctx* c, int enable, float* ms) {
@@ -1452,7 +1420,6 @@ int idc_destroy(idc_ctx* c) {
   if (c->pts313) cudaFree(c->pts313);
   if (c->splitk_ws) cudaFree(c->splitk_ws);
   if (c->splitk_counters) cudaFree(c->splitk_counters);
-  if (c->chain_bar) cudaFree(c->chain_bar);
   if (c->w11_umma) cudaFree(c->w11_umma);
   if (c->d_reccs) cudaFree(c->d_reccs);
   if (c->gvec) cudaFree(c->gvec);

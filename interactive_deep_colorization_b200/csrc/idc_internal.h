@@ -21,10 +21,10 @@ constexpr int kMaxCls = 4;    // output parity classes of a stride-2 transposed 
 
 enum Act { ACT_NONE = 0, ACT_RELU = 1, ACT_LEAKY02 = 2 };
 
-// tcgen05 engine: activations are stored as FP16 hi/lo planes of (value * 2^kActScaleLog2).
-// Measured on B200 (round 1): the tensor core treats FP16 *subnormal* operands as zero, so an
-// unscaled lo plane loses the low half of every activation below 0.125 (ab error 1.2e-2 instead
-// of 1e-4).  Scaling by 64 keeps lo normal down to |a| = 0.002; FP16 range then covers |a| < 1023.
+// wgmma engine: activations are stored as FP16 hi/lo planes of (value * 2^kActScaleLog2).
+// The scale keeps the lo plane out of the FP16 subnormal range (tensor cores may flush subnormal
+// operands to zero, which would drop the low half of every small activation): scaling by 64 keeps
+// lo normal down to |a| = 0.002; FP16 range then covers |a| < 1023.
 constexpr int kActScaleLog2 = 6;
 constexpr float kActScale = 64.0f;
 constexpr float kActInvScale = 1.0f / 64.0f;
@@ -38,7 +38,7 @@ struct Tap {
   int ty, tx;
 };
 
-// Activation buffer.  SIMT engine: p0 = float [N,H,W,C].  tcgen05 engine: p0/p1 = __half
+// Activation buffer.  SIMT engine: p0 = float [N,H,W,C].  wgmma engine: p0/p1 = __half
 // hi/lo planes, each [N,H,W,C]; value = hi + lo.
 struct ActBuf {
   std::string name;
@@ -49,7 +49,7 @@ struct ActBuf {
 
 // Per-output-channel epilogue vectors (device, fp32[cout_pad]).
 //   v = act(acc + bias) * scale + shift (+ gadd[n][c])
-// tcgen05 engine: weights are pre-scaled per output channel by a power of two 2^e (so the FP16 lo
+// wgmma engine: weights are pre-scaled per output channel by a power of two 2^e (so the FP16 lo
 // term stays normal); bias is stored as bias*2^e and scale as scale*2^-e, which is exact and leaves
 // the formula unchanged because ReLU / LeakyReLU are positively homogeneous.
 struct Epilogue {
@@ -87,14 +87,14 @@ struct ConvOp {
   int cout = 0, cout_pad = 0;
   int K = 0;                     // sum over taps of cin(src)
   Epilogue epi;
-  bool fuse_out_head = false;    // tcgen05 engine: model_out (128->2, tanh*110) in the epilogue
+  bool fuse_out_head = false;    // wgmma engine: model_out (128->2, tanh*110) in the epilogue
   bool out_f32 = false;          // store FP32 [M][cout_pad] instead of an activation (class logits)
   float* out_f32_ptr = nullptr;  // where (ctx->logits or ctx->logits313)
   // packed weights
   float* w_simt = nullptr;       // [ncls][K][cout_pad] fp32
   __half* w_hi = nullptr;        // [ncls*cout_pad][K] fp16 (x wscale)
   __half* w_lo = nullptr;
-  // tcgen05 launch plan (filled by umma_plan_op)
+  // wgmma launch plan (filled by umma_plan_op)
   int bn_tile = 0, hbox = 0, wbox = 0;
   void* umma_plan = nullptr;
   double flops_per_image = 0;
@@ -110,20 +110,14 @@ struct Conv11Weights {
 // round 1: a C ABI that is embedded in someone else's process must not read process-global state.
 struct Options {
   int halo = 1;           // halo-tile A operand: 0 off, 1 = 128-column stride-1 3x3 layers that fill the machine, 3 = every eligible op
-  int pairs = 1;          // cta_group::2: 0 never, 1 = launches that give every SM pair >= 2 tiles, 2 = always
-  int mt = -1;            // M-tiles per CTA tile on the <= 128-column layers (1 / 2)
-  int chunk_kb = -1;      // k-blocks summed in TMEM before the FP32 round-to-nearest add
+  int pairs = 0;          // clusters of 2 CTAs sharing the weight tile: 0 never (default: measured slower), 1 = launches that
+                          // give every SM >= 2 tiles, 2 = always
+  int mt = -1;            // M-tiles per CTA tile (1 / 2; 2 runs with 64-column tiles)
+  int chunk_kb = -1;      // k-blocks summed inside the tensor core before the FP32 round-to-nearest add
   int split_k = -1;       // K slices per tile on launches that cannot fill the machine
-  int direct_stores = 0;  // 1 = per-lane 16-byte stores instead of the warp-transposed ones
   int host_pipe = 1;      // idc_forward_host: chunked copy/compute overlap for batches >= 8
   int pdl = 1;            // programmatic dependent launch between the kernels of a forward
-  int split_pairs = 1;    // cta_group::2 on the split-K (small batch) path
-  int split_bn128 = 1;    // 128-column tiles on the split-K path (halves the partial-tile traffic of the reduction)
   int conv1_1_umma = 1;   // model1.0 on the tensor cores (one padded k-block); 0 = the FP32 CUDA-core kernel
-  int chain = 0;          // run consecutive same-shaped split-K layers as ONE launch with a grid barrier between layers
-  int prologue_sync2 = 1; // pairs: cluster barrier between barrier init and the cta_group::2 TMEM allocation (0: -3 us per click,
-                          // bit-identical results, but compute-sanitizer racecheck flags the allocation -> kept on)
-  int halo_split = 0;     // halo-tile A operand on the 128-column split-K path (stride-1 3x3 layers; experiment)
   int side_dist = 1;      // batch <= 4: run the dist head (class + softmax) on a side stream next to levels 9-10
   int tanh_scale = 110;   // regression head: tanh * 110 (model.py:175); the Caffe deploy nets use 100 (SURVEY q4)
 };
@@ -166,11 +160,9 @@ struct Ctx {
   float* logits313 = nullptr;  // Caffe-spec head: [max_n*(H/4)*(W/4)][320]
   bool caffe313 = false;
   float* pts313 = nullptr;     // [313][2] ab bin centres (device)
-  // split-K workspace of the tcgen05 engine (sized by umma_plan_op, allocated after planning)
+  // split-K workspace of the wgmma engine (sized by umma_plan_op, allocated after planning)
   float* splitk_ws = nullptr; size_t splitk_ws_floats = 0;
   int* splitk_counters = nullptr; int splitk_max_tiles = 0;
-  int* chain_bar = nullptr;      // grid-wide arrive counter of the chained launches (self-resetting)
-  long long* dbgbuf = nullptr;   // experiments: per-CTA cycle counters of the last tcgen05 launch
   bool dbg_graph_timing = false; // experiments: events around the click graph launch (idc_debug_graph_timing)
   cudaEvent_t dbg_ev[2] = {nullptr, nullptr};
   float dbg_graph_ms = 0.f;
@@ -224,8 +216,6 @@ void umma_free_op(ConvOp& op);
 cudaError_t umma_run_op(Ctx* c, ConvOp& op, int n, float* out_ab_fused, float out_mult, cudaStream_t st, int img0 = 0,
                         int max_ctas = 0);   // max_ctas > 0: cap the persistent grid (side-branch launches)
 bool umma_op_uses_split_k(const ConvOp& op);
-bool umma_op_chainable(const Ctx* c, const ConvOp& op);   // may run inside a chained launch (see conv_body<..., CHAIN>)
-cudaError_t umma_run_chain(Ctx* c, int first, int last, int n, cudaStream_t st);   // ops[first..last] in ONE launch
 
 cudaError_t launch_conv1_1(Ctx* c, int n, const float* L, const float* ab, const float* mask,
                            float maskcent, cudaStream_t st, int img0 = 0);   // L/ab/mask: full arrays; images img0..img0+n

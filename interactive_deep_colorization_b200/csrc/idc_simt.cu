@@ -1,7 +1,7 @@
 // FP32 CUDA-core engine: generic gather-GEMM convolution (3x3 / dilated / decimated-input /
 // transposed-conv parity classes + fused shortcut) with the fused epilogue
 //     v = act(acc + bias) * bn_scale + bn_shift (+ global-hints vector).
-// Exact-FP32 reference engine of the product (IDC_FLAG_ENGINE_SIMT); the tcgen05 engine in
+// Exact-FP32 reference engine of the product (IDC_FLAG_ENGINE_SIMT); the wgmma engine in
 // idc_umma.cu computes the same ops from the same tap tables.
 // Reference semantics: nn.Conv2d / nn.ConvTranspose2d / nn.BatchNorm2d(eval) / ReLU as wired in
 // /root/reference/models/pytorch/model.py:13-102,149-165.

@@ -15,21 +15,22 @@ def _np_ptr(a):
 
 
 class LhnContext(object):
-    """Local Hints Network forward context (the B200 stand-in for
+    """Local Hints Network forward context (the H100 stand-in for
     `SIGGRAPHGenerator(...).cuda().eval()`, /root/reference/data/colorize_image.py:221-232)."""
 
-    def __init__(self, device=0, max_n=1, H=256, W=256, dist=False, engine="tcgen05", fast_fp16=False,
+    def __init__(self, device=0, max_n=1, H=256, W=256, dist=False, engine="wgmma", fast_fp16=False,
                  global_hints=False, use_graph=True, keep_conv10=False, caffe313=False, options=None):
-        """options: {name: int} plan-time switches, see include/idc_b200.h: idc_set_option
-        (halo, pairs, mt, chunk_kb, split_k, split_pairs, direct_stores, host_pipe, pdl)."""
+        """engine: "wgmma" (tensor cores; "tcgen05" is accepted as the name earlier releases used) or "simt"
+        (exact FP32 CUDA cores).  options: {name: int} plan-time switches, see include/idc_b200.h: idc_set_option
+        (halo, pairs, mt, chunk_kb, split_k, host_pipe, pdl, side_dist, conv1_1_umma, tanh_scale)."""
         self.lib = _lib.load()
         flags = 0
         if dist:
             flags |= _lib.FLAG_DIST
         if engine == "simt":
             flags |= _lib.FLAG_ENGINE_SIMT
-        elif engine != "tcgen05":
-            raise ValueError("engine must be 'tcgen05' or 'simt'")
+        elif engine not in ("wgmma", "tcgen05"):
+            raise ValueError("engine must be 'wgmma' or 'simt'")
         if fast_fp16:
             flags |= _lib.FLAG_FAST_FP16
         if global_hints:
@@ -45,7 +46,7 @@ class LhnContext(object):
         h = ctypes.c_void_p()
         rc = self.lib.idc_create(self.device, self.max_n, self.H, self.W, flags, ctypes.byref(h))
         if rc != _lib.IDC_OK:
-            raise _lib.IdcError(rc, "idc_create(device=%d, max_n=%d, %dx%d) failed -- a CUDA sm_100 device is "
+            raise _lib.IdcError(rc, "idc_create(device=%d, max_n=%d, %dx%d) failed -- a CUDA sm_90 (H100) device is "
                                     "required; there is no CPU fallback" % (device, max_n, H, W))
         self.h = h
         self.ready = False

@@ -1,4 +1,4 @@
-"""`ideepcolor.py` with a B200 backend (SURVEY row f4).
+"""`ideepcolor.py` with an H100 backend (SURVEY row f4).
 
     python -m interactive_deep_colorization_b200.launcher --backend b200 --reference_root /path/to/ideepcolor \\
         --color_model caffemodel.pth [--pytorch_maskcent] [--image_file ...] [--win_size 512] [--gpu 0]
@@ -23,7 +23,7 @@ BACKENDS = ("b200", "b200-caffe")
 
 
 def parse_args(argv=None):
-    p = argparse.ArgumentParser(description='iDeepColor: deep interactive colorization (B200 backend)')
+    p = argparse.ArgumentParser(description='iDeepColor: deep interactive colorization (H100 backend)')
     # same names / defaults as ideepcolor.py:13-46
     p.add_argument('--win_size', dest='win_size', help='the size of the main window', type=int, default=512)
     p.add_argument('--image_file', dest='image_file', help='input image', type=str, default='test_imgs/mortar_pestle.jpg')
@@ -49,7 +49,7 @@ def parse_args(argv=None):
 
 
 def build_models(args):
-    """ideepcolor.py:60-74 for the B200 backends -> (colorModel, distModel)."""
+    """ideepcolor.py:60-74 for the H100 backends -> (colorModel, distModel)."""
     from . import colorize_image as CI
     if args.backend == 'b200':
         # "PyTorch (same model used for both)" (ideepcolor.py:34-38): one checkpoint, so one trunk -- the distribution
@@ -140,7 +140,7 @@ def main(argv=None):
     app = QApplication(sys.argv)
     window = gui_design.GUIDesign(color_model=colorModel, dist_model=distModel, img_file=args.image_file,
                                   load_size=args.load_size, win_size=args.win_size)
-    window.setWindowTitle('iColor (B200)')
+    window.setWindowTitle('iColor (H100)')
     window.show()
     app.exec_()
 

@@ -46,7 +46,7 @@ def _param_tree(mod):
 
 
 class SIGGRAPHGeneratorB200(nn.Module):
-    def __init__(self, dist=False, device=0, engine="tcgen05", fast_fp16=False, ref_quirks=True, max_batch=1):
+    def __init__(self, dist=False, device=0, engine="wgmma", fast_fp16=False, ref_quirks=True, max_batch=1):
         super(SIGGRAPHGeneratorB200, self).__init__()
         self.dist = dist
         self.b200_device = device

@@ -15,7 +15,7 @@ def _torch():
     with gpu_prepost=False uses the host numpy path by explicit choice, nothing switches silently)."""
     import torch
     if not torch.cuda.is_available():
-        raise _lib.IdcError(-5, "no CUDA device: the GPU pre/post-processing path (row f1) needs an sm_100 GPU")
+        raise _lib.IdcError(-5, "no CUDA device: the GPU pre/post-processing path (row f1) needs an sm_90 GPU")
     return torch
 
 

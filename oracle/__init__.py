@@ -8,7 +8,7 @@ package (``interactive_deep_colorization_b200``).  Allowed importers: ``tests/``
 Parity pin status (see DESIGN.md "Oracle"):
   * network trunk + regression head + 529-bin dist head (rows a3..a9, a12, a13 of
     SURVEY.md section 8a): PINNED against the unmodified reference
-    ``/root/reference/models/pytorch/model.py`` run in the build container; golden
+    ``models/pytorch/model.py`` (outputs stored as golden
     vectors + generating script live in ``tests/golden/``.
   * Lab<->RGB (rows a10, a11): restatement of scikit-image 0.13 ``color.rgb2lab /
     lab2rgb`` (absent from the image, not vendored by the reference): PARITY UNPINNED

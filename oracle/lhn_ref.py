@@ -2,8 +2,8 @@
 Network forward, /root/reference/models/pytorch/model.py:134-175, batched.
 
 Test infrastructure only -- see oracle/__init__.py.  Pinned against the unmodified
-reference module by tests/test_oracle.py (when /root/reference is present) and by the
-golden vectors in tests/golden/ (always).
+reference module through golden vectors generated from it (tests/golden/make_golden.py,
+tests/golden/make_ref_forward_golden.py) and checked by tests/test_oracle.py.
 """
 import numpy as np
 import torch

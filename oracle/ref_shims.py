@@ -1,9 +1,9 @@
-"""Import the UNMODIFIED reference (/root/reference) in the build container.
+"""Import the UNMODIFIED reference (a checkout named by IDC_REFERENCE_ROOT, or the staged copy).
 
 The reference wrapper needs matplotlib and scikit-image, both absent here
 (data/colorize_image.py:3-4).  We inject a stub ``matplotlib`` and a ``skimage.color``
 backed by oracle/color_ref.py into sys.modules, then import the reference modules as
-they are.  /root/reference does not exist on the GPU box: callers must check
+they are.  Where no checkout exists, callers must check
 ``reference_available()`` and skip.
 
 Test infrastructure only -- see oracle/__init__.py.
@@ -34,13 +34,13 @@ def reference_available():
 
 
 def full_reference_available():
-    """The whole tree (test images, colour-bin fixtures), i.e. the build container -- not the staged subset."""
+    """The whole tree (test images, colour-bin fixtures) -- not the staged subset."""
     return os.path.isfile(os.path.join(REF_ROOT, "test_imgs", "mortar_pestle.jpg"))
 
 
 def stage_reference(src="/root/reference"):
-    """Build-container step (called by __graft_entry__.build()): copy the reference's own network + wrapper files,
-    byte for byte, into the git-ignored oracle/_ref/ so that the GPU box (where /root/reference does not exist) can
+    """Build step (called by __graft_entry__.build()): copy the reference's own network + wrapper files,
+    byte for byte, into the git-ignored oracle/_ref/ so that a machine without the checkout can
     time the UNMODIFIED reference CPU path in `bench.py --impl reference`.  Nothing staged is product or test source:
     oracle/_ref/ is listed in .gitignore (never committed) and only bench.py's CPU arm reads it."""
     import shutil

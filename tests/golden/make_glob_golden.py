@@ -3,9 +3,9 @@
 
 The Caffe net `models/global_model/global_stats.prototxt` cannot run here (no Caffe), but its Python layer
 `NNEncLayer` (caffe_files/caffe_traininglayers.py:161-196) only wraps `NNEncode(NN=1, sigma=5)`
-(caffe_files/color_quantization.py:6-38), which needs numpy + scikit-learn and runs in the build container.
-This script imports THAT class unmodified from /root/reference, feeds it the 4x4-pooled ab map of the
-golden test image (and a random image), and stores the inputs + its encodings.  Run in the BUILD container:
+(caffe_files/color_quantization.py:6-38), which needs numpy + scikit-learn and runs on the CPU.
+This script imports THAT class unmodified from the reference checkout, feeds it the 4x4-pooled ab map of the
+golden test image (and a random image), and stores the inputs + its encodings.  Run where the reference checkout is available:
 
     python tests/golden/make_glob_golden.py        -> tests/golden/glob_nnenc.npz
 """

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Generate the golden vectors in tests/golden/ by running the UNMODIFIED reference
-(/root/reference, imported read-only through oracle/ref_shims.py) with the seeded
-synthetic state_dict of oracle/synth.py.  Run in the BUILD container only:
+(a checkout imported read-only through oracle/ref_shims.py) with the seeded
+synthetic state_dict of oracle/synth.py.  Run where the reference checkout is available:
 
     python tests/golden/make_golden.py
 
@@ -9,6 +9,10 @@ Outputs (committed):
     lhn_256.npz     configs 1-2 + notebook KAT on test_imgs/mortar_pestle.jpg @256
     lhn_dist_256.npz  ColorizeImageTorchDist sample (config 5 semantics)
     lhn_64.npz      small synthetic case incl. per-layer checksums (fast CPU check)
+
+Every file stays below 1 MB: the 256x256 outputs of lhn_256.npz are stored at a fixed, seeded sample of
+PIX_COUNT pixels (flat indices in `pix_idx`; inputs img_rgb / img_l_mc stay whole), and the 529-bin distributions of
+lhn_64.npz at a seeded sample of DIST_BINS bins (`dist16_bins`).
 """
 import os
 import sys
@@ -24,6 +28,31 @@ sys.path.insert(0, ROOT)
 from oracle import synth, ref_shims  # noqa: E402
 
 SEED = 1234
+PIX_COUNT = 16384                # of the 65536 pixels of a 256x256 output: every output-parity class is represented
+DIST_BINS = 64                   # of the 529 distribution bins
+
+
+def pix_idx():
+    return np.sort(np.random.RandomState(256).choice(256 * 256, PIX_COUNT, replace=False)).astype(np.int32)
+
+
+def dist_bins():
+    return np.sort(np.random.RandomState(529).choice(529, DIST_BINS, replace=False)).astype(np.int32)
+
+
+def sample_256(key, a, idx):
+    """[C, 256, 256] -> [C, PIX_COUNT]; [256, 256, 3] (RGB) -> [PIX_COUNT, 3]; anything else unchanged."""
+    if key in ("img_rgb", "img_l_mc") or a.ndim != 3:
+        return a
+    if a.shape[:2] == (256, 256):
+        return a.reshape(256 * 256, a.shape[2])[idx]
+    if a.shape[1:] == (256, 256):
+        return a.reshape(a.shape[0], 256 * 256)[:, idx]
+    return a
+
+
+def sample_64(key, a, bins):
+    return a[bins] if key.startswith("dist16_") and key != "dist16_bins" else a
 
 
 def main():
@@ -66,6 +95,9 @@ def main():
                 out["%s_%s_output_ab" % (tag, name)] = cm.output_ab.astype(np.float32)
             if tag == "mc0" and name == "kat":
                 out["kat_fullres_rgb_small"] = cm.get_img_fullres()[::8, ::8].copy()
+    idx = pix_idx()
+    out = {k: sample_256(k, v, idx) for k, v in out.items()}
+    out["pix_idx"] = idx
     np.savez_compressed(os.path.join(HERE, "lhn_256.npz"), **out)
     print("lhn_256.npz", {k: v.shape for k, v in out.items()})
 
@@ -108,6 +140,9 @@ def main():
             small["%s_%d_absmax" % (n, i)] = np.abs(t).max(axis=(1, 2))
     for h in hooks:
         h.remove()
+    bins = dist_bins()
+    small = {k: sample_64(k, v, bins) for k, v in small.items()}
+    small["dist16_bins"] = bins
     np.savez_compressed(os.path.join(HERE, "lhn_64.npz"), **small)
     print("lhn_64.npz", {k: v.shape for k, v in small.items()})
 

@@ -25,7 +25,7 @@ def test_library_exports_every_declared_symbol():
     for n in names:
         assert hasattr(lib, n), "libidc_b200.so does not export %s" % n
     assert sorted(s[0] for s in _lib.SYMBOLS) == names, "ctypes table and header disagree"
-    assert b"sm_100a" in lib.idc_version()
+    assert b"sm_90a" in lib.idc_version()
 
 
 def test_argument_validation_without_gpu():
@@ -57,13 +57,13 @@ def test_no_cpu_fallback():
         cm.net_forward(np.zeros((2, 64, 64)), np.zeros((1, 64, 64)))
 
 
-def test_sass_is_blackwell_native():
-    """The shipped cubin must contain tcgen05 MMA / TMA / TMEM-load instructions."""
+def test_sass_is_hopper_native():
+    """The shipped cubin must contain warpgroup MMA (wgmma) and TMA instructions."""
     import shutil
     import subprocess
     if not shutil.which("cuobjdump"):
         pytest.skip("cuobjdump not on PATH")
     sass = subprocess.run(["cuobjdump", "-sass", _lib.LIB_PATH], capture_output=True, text=True).stdout
-    for mnem in ("UTCHMMA", "UTMALDG", "LDTM"):
+    for mnem in ("HGMMA", "UTMALDG"):
         assert mnem in sass, mnem
-    assert "sm_100a" in subprocess.run(["cuobjdump", "-lelf", _lib.LIB_PATH], capture_output=True, text=True).stdout
+    assert "sm_90a" in subprocess.run(["cuobjdump", "-lelf", _lib.LIB_PATH], capture_output=True, text=True).stdout

@@ -138,9 +138,9 @@ def test_fast_fp16_forward_host_large_batch(synth_sd):
 
 
 def test_plan_options_agree(synth_sd):
-    """PDL on/off and the side-stream dist head on/off must be bit-identical (same kernels, same order of arithmetic); CTA pairs on the split-K path and
-    the halo-tile operand change the summation order only: each variant within tolerance of the oracle and within
-    3e-4 of each other.  256^2, batch 1 (the interactive plan: split-K everywhere) and batch 4."""
+    """PDL on/off and the side-stream dist head on/off must be bit-identical (same kernels, same order of arithmetic); the
+    FP32 conv1_1 kernel, other split-K / chunk settings and the halo-tile operand change the summation order only: each variant within tolerance
+    of the oracle and within 3e-4 of each other.  256^2, batch 1 (the interactive plan: split-K everywhere) and batch 4."""
     g = util.golden("lhn_256.npz")
     L1 = g["img_l_mc"].astype(np.float32)[None]
     a1, m1 = synth.synthetic_hints(256, 5, 0)
@@ -148,24 +148,23 @@ def test_plan_options_agree(synth_sd):
     ref = g["mc1_rand5_ab_raw"]
     outs = {}
     for name, opts in (("default", {}), ("no_pdl", {"pdl": 0}), ("no_side_dist", {"side_dist": 0}),
-                       ("chain", {"chain": 1}), ("prologue_sync1", {"prologue_sync2": 0}),
                        ("conv1_1_fp32", {"conv1_1_umma": 0}),
-                       ("no_split_pairs", {"split_pairs": 0}), ("split_bn256", {"split_bn128": 0}),
+                       ("no_split_k", {"split_k": 1}), ("chunk1", {"chunk_kb": 1}),
                        ("no_halo", {"halo": 0}), ("halo_all", {"halo": 3})):
         ctx = util.make_ctx(synth_sd, 256, 256, max_n=1, dist=True, options=opts)
         r = ctx.forward_host(L1, a1, m1, 0.5, want_dist=True, want_rgb=True)
         r2 = ctx.forward_host(L1, a1, m1, 0.5, want_dist=True, want_rgb=True)      # graph replay
         assert np.array_equal(r["ab"], r2["ab"]) and np.array_equal(r["dist"], r2["dist"])
-        err = util.maxabs(r["ab"][0], ref)
+        err = util.maxabs(util.at_pix(g, r["ab"][0]), ref)
         print("options %-15s max|d ab| vs reference golden = %.3e" % (name, err))
         assert err <= TOL_AB, (name, err)
         outs[name] = r
         ctx.close()
-    for k in ("no_pdl", "no_side_dist", "chain", "prologue_sync1"):    # scheduling only: bit-identical
+    for k in ("no_pdl", "no_side_dist"):    # scheduling only: bit-identical
         assert np.array_equal(outs["default"]["ab"], outs[k]["ab"]), k
         assert np.array_equal(outs["default"]["dist"], outs[k]["dist"]), k
         assert np.array_equal(outs["default"]["rgb"], outs[k]["rgb"]), k
-    for k in ("no_split_pairs", "split_bn256", "no_halo", "halo_all", "conv1_1_fp32"):
+    for k in ("no_split_k", "chunk1", "no_halo", "halo_all", "conv1_1_fp32"):
         assert util.maxabs(outs[k]["ab"], outs["default"]["ab"]) < 3e-4, k
     # batch 4 on a max_n = 4 context (halo + pairs plans differ from the batch-1 context)
     L, ab, m = synth.synthetic_batch(4, 256, seed=77, max_hints=6)
@@ -213,7 +212,6 @@ def test_wrapper_fused_quantised_ab_and_globdist_fullres(synth_sd):
     assert cm.output_ab.dtype == np.float64 and cm.output_ab.shape == (2, 256, 256)
     assert np.max(np.abs(cm.output_ab - ref_q[1:])) < 1e-9
     assert np.max(np.abs(cm.output_lab - ref_q)) < 1e-9                # lazily derived, same values
-    assert np.max(np.abs(cm.output_ab - g["mc0_kat_output_ab"] * 0 - ref_q[1:])) < 1e-9
     sd, _ = _glob_sd(synth_sd)
     cid = CI.ColorizeImageB200GlobDist(Xd=256)
     cid.prep_net(state_dict=sd)

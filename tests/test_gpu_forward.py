@@ -1,4 +1,4 @@
-"""GPU: the tcgen05 engine end to end -- the parity tests proper.  Everything goes through
+"""GPU: the wgmma engine end to end -- the parity tests proper.  Everything goes through
 the C ABI (engine.LhnContext -> libidc_b200.so)."""
 import numpy as np
 import pytest
@@ -36,12 +36,12 @@ def test_golden_256(ctx256, case, mc):
     ab, m = _hints(case)
     r = ctx256.forward_host(L, ab[None].astype(np.float32), m[None].astype(np.float32), mc, want_rgb=True)
     ref = g["mc%d_%s_ab_raw" % (1 if mc else 0, case)]
-    err = util.maxabs(r["ab"][0], ref)
+    err = util.maxabs(util.at_pix(g, r["ab"][0]), ref)
     print("golden %s mc=%s max|dab| = %.3e" % (case, mc, err))
     assert err <= TOL_AB, err
     if not mc:
         rgb_ref = g["mc0_%s_rgb" % case]
-        d = np.abs(r["rgb"][0].astype(int) - rgb_ref.astype(int))
+        d = np.abs(util.at_pix_hwc(g, r["rgb"][0]).astype(int) - rgb_ref.astype(int))
         assert d.max() <= 1 and (d > 0).mean() < 2e-3, (d.max(), (d > 0).mean())
 
 
@@ -109,10 +109,10 @@ def test_wrapper_api_end_to_end(synth_sd):
     CI.put_point(ab, m, [100, 160], 3, [0, 0])
     rgb = cm.net_forward(ab, m)
     assert rgb.shape == (256, 256, 3) and rgb.dtype == np.uint8
-    assert util.maxabs(cm.output_ab_raw, g["mc0_kat_ab_raw"]) <= TOL_AB
-    d = np.abs(rgb.astype(int) - g["mc0_kat_rgb"].astype(int))
+    assert util.maxabs(util.at_pix(g, cm.output_ab_raw), g["mc0_kat_ab_raw"]) <= TOL_AB
+    d = np.abs(util.at_pix_hwc(g, rgb).astype(int) - g["mc0_kat_rgb"].astype(int))
     assert d.max() <= 1 and (d > 0).mean() < 2e-3
-    assert np.max(np.abs(cm.output_ab - g["mc0_kat_output_ab"])) < 1.5     # 1 uint8 step in ab units
+    assert np.max(np.abs(util.at_pix(g, cm.output_ab) - g["mc0_kat_output_ab"])) < 1.5     # 1 uint8 step in ab units
     full = cm.get_img_fullres()                      # GPU zoom + Lab->RGB (row f1)
     assert full.shape == (256, 256, 3)
     d = np.abs(full.astype(int) - color_ref.lab2rgb_transpose(cm.img_l_fullres, cm.output_ab).astype(int))
@@ -172,7 +172,7 @@ def test_global_hints_branch(synth_sd):
     ref, inter = util.oracle_forward(synth_sd, L, ab, m, 0.5, glob_add=gvec, intermediates=True)
     ref_noglob = util.oracle_forward(synth_sd, L, ab, m, 0.5)
     assert util.maxabs(ref, ref_noglob) > 0.5                      # the branch actually matters
-    for engine in ("simt", "tcgen05"):
+    for engine in ("simt", "wgmma"):
         ctx = util.make_ctx(sd, 64, 64, max_n=3, engine=engine, global_hints=True)
         r = ctx.forward_device(util.dev(L), util.dev(ab), util.dev(m), 0.5, glob=util.dev(glob))
         torch.cuda.synchronize()
@@ -199,7 +199,7 @@ def test_caffe313_head(synth_sd):
         pred64, _, logits64, _ = caffe_spec.caffe313_head(csd, inter, return_logits=True, dtype=torch.float64)
     assert float(pred_ref.abs().max()) > 5.0
     ref32_vs_64 = util.maxabs(pred_ref, pred64)            # how far an FP32 evaluation of the spec is from exact arithmetic
-    for engine in ("simt", "tcgen05"):
+    for engine in ("simt", "wgmma"):
         ctx = util.make_ctx(sd, 64, 64, max_n=2, engine=engine, caffe313=True)
         ctx.forward_device(util.dev(L), util.dev(ab), util.dev(m), 0.5)
         torch.cuda.synchronize()

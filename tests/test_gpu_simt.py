@@ -34,6 +34,6 @@ def test_simt_golden_256(synth_sd):
     ab, m = synth.synthetic_hints(256, 5, 0)
     ctx = util.make_ctx(synth_sd, 256, 256, engine="simt")
     r = ctx.forward_host(L, ab[None].astype(np.float32), m[None].astype(np.float32), 0.5)
-    err = util.maxabs(r["ab"][0], g["mc1_rand5_ab_raw"])
+    err = util.maxabs(util.at_pix(g, r["ab"][0]), g["mc1_rand5_ab_raw"])
     assert err < 1e-3, err
     ctx.close()

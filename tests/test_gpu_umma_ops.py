@@ -1,4 +1,4 @@
-"""GPU: every tcgen05 op in isolation -- oracle activations are injected as the op's inputs,
+"""GPU: every wgmma op in isolation -- oracle activations are injected as the op's inputs,
 ONE op runs, and its output is compared with the oracle's activation.  Localises a bug to
 a layer / tap table / tensor map instead of letting it smear through the network."""
 import numpy as np
@@ -14,12 +14,12 @@ pytestmark = pytest.mark.gpu
                 ids=["mt1", "mt2", "pairs", "pairs_mt2", "halo", "halo_pairs"])
 def setup(request, synth_sd):
     """The plan-time options (mt, pairs, halo) are applied when the launch plan is built: the 128-pixel tiles, the 256-pixel
-    tiles, the cta_group::2 pair path (forced, incl. the odd-tile-count dummy tile) and the halo-tile
-    A operand (one TMA tile per 64 input channels + pixel-shifted UMMA descriptors, stride-1 3x3 layers with
-    <= 128 output columns) are exercised on every op that supports them."""
+    tiles, the pair path (clusters of two CTAs sharing a multicast weight tile; forced, incl. the odd-tile-count dummy
+    tile) and the halo-tile A operand (one TMA tile per 64 input channels + pixel-shifted wgmma descriptors, stride-1
+    3x3 layers with <= 128 output columns) are exercised on every op that supports them."""
     L, ab, m = util.small_batch(3, 64, seed=300)
     _, inter = util.oracle_forward(synth_sd, L, ab, m, 0.5, dist=False, intermediates=True)
-    ctx = util.make_ctx(synth_sd, 64, 64, max_n=3, engine="tcgen05", keep_conv10=True, use_graph=False,
+    ctx = util.make_ctx(synth_sd, 64, 64, max_n=3, engine="wgmma", keep_conv10=True, use_graph=False,
                         options={"mt": request.param[0], "pairs": request.param[1], "halo": request.param[2]})
     yield ctx, inter
     ctx.close()

@@ -25,10 +25,12 @@ def test_image_prep_matches_reference_golden():
     assert cm.img_l.shape == (1, 256, 256) and cm.img_ab.shape == (2, 256, 256)
     assert cm.get_img_gray().shape == (256, 256, 3)
     # quantised output_ab path (reference :196-198)
-    cm.output_rgb = g["mc0_kat_rgb"]
+    cm.output_rgb = g["mc0_kat_rgb"][None]            # the stored pixels as a 1 x K image (the conversion is per pixel)
     cm._set_out_ab_()
-    assert np.max(np.abs(cm.output_ab - g["mc0_kat_output_ab"])) < 1e-4
-    # full-res rendering: img_rgb_fullres == img_rgb here, so zoom factor is 1
+    assert np.max(np.abs(cm.output_ab[:, 0] - g["mc0_kat_output_ab"])) < 1e-4
+    # full-res rendering: img_rgb_fullres == img_rgb here, so zoom factor is 1 (any full-size output will do)
+    cm.output_rgb = g["img_rgb"]
+    cm._set_out_ab_()
     assert np.array_equal(cm.get_img_fullres(), color_ref.lab2rgb_transpose(cm.img_l, cm.output_ab))
 
 

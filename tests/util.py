@@ -27,6 +27,18 @@ def golden(name):
     return np.load(os.path.join(GOLDEN, name))
 
 
+def at_pix(g, a):
+    """[..., 256, 256] -> [..., K]: the pixels a golden file stores its 256x256 outputs at (g["pix_idx"])."""
+    a = a.detach().cpu().numpy() if hasattr(a, "detach") else np.asarray(a)
+    return a.reshape(a.shape[:-2] + (-1,))[..., g["pix_idx"]]
+
+
+def at_pix_hwc(g, a):
+    """[256, 256, C] (an RGB image) -> [K, C] at the same pixels."""
+    a = np.asarray(a)
+    return a.reshape(-1, a.shape[-1])[g["pix_idx"]]
+
+
 def oracle_forward(sd, L, ab, mask, maskcent=0.0, dist=False, glob_add=None, intermediates=False):
     torch.set_num_threads(max(1, os.cpu_count() or 1))
     with torch.no_grad():

@@ -3,7 +3,7 @@
 per-op device time (CUDA events between the launches, PDL off by construction), the wall-clock p50 of the
 graph-replayed idc_forward_host_q (the click), and the same through the ColorizeImageB200 wrapper.
 
-    python tools/latency_profile.py [name=opt:val,opt:val ...]      e.g.  base=pdl:0,split_pairs:0 new=
+    python tools/latency_profile.py [name=opt:val,opt:val ...]      e.g.  base=pdl:0 new=
 """
 import os
 import sys
@@ -68,7 +68,7 @@ def run(tag, options, per_op=True):
 
 
 if __name__ == "__main__":
-    specs = sys.argv[1:] or ["base=pdl:0,split_pairs:0", "pdl=split_pairs:0", "pairs=pdl:0", "new="]
+    specs = sys.argv[1:] or ["no_pdl=pdl:0", "no_split_k=split_k:1", "new="]
     for spec in specs:
         name, _, body = spec.partition("=")
         opts = {kv.split(":")[0]: int(kv.split(":")[1]) for kv in body.split(",") if kv}

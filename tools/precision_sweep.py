@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""GPU tool: ab error and time of the tcgen05 engine as a function of the chunk_kb option (k-blocks summed
-inside the tensor core before the FP32 round-to-nearest add).  Writes a small table for profiles/."""
+"""GPU tool: ab error and time of the wgmma engine as a function of the chunk_kb option (k-blocks summed
+inside the tensor core before the FP32 round-to-nearest add).  Prints a small table."""
 import os
 import sys
 import time

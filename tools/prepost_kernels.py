@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """GPU tool for ncu: ONE launch of every bandwidth-bound kernel either side of the conv trunk at a realistic size
-(rows a10-a14, f1, f3), so that `ncu --set full` yields one row per kernel for profiles/.
+(rows a10-a14, f1, f3), so that a profiler yields one row per kernel.
 
     rgb2lab_kernel          18 MP photo (3456 x 5184, bird_gray.jpg's size), uint8 -> float64 Lab
     resize_linear_u8_kernel 3456 x 5184 -> 256 x 256

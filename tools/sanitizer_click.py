@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """GPU tool for compute-sanitizer: a few clicks through the whole interactive path (resident image, announced click,
-tensor-core conv1_1, 128-column split-K pairs, chained launch on the second context) at 64x64 -- small enough for
-memcheck / racecheck to finish in minutes.
+tensor-core conv1_1, split-K on the first context; forced pairs and halo tiles on the second) at 64x64 -- small enough
+for memcheck / racecheck to finish in minutes.
 
     compute-sanitizer --tool memcheck python tools/sanitizer_click.py [size] [opt:val,...]
 """
@@ -22,7 +22,7 @@ sd = synth.torch_state_dict(1234)
 L, ab, m = synth.synthetic_batch(1, X, seed=0, max_hints=0)
 ab, m = ab.copy(), m.copy()
 outs = []
-for opts in ({}, {"chain": 1}):
+for opts in ({}, {"pairs": 2, "halo": 3}):
     opts = dict(opts, **EXTRA)
     ctx = util.make_ctx(sd, X, X, max_n=1, dist=True, options=opts)
     ctx.set_dist_resident(True)
@@ -43,5 +43,8 @@ for opts in ({}, {"chain": 1}):
         cen, conf, it = ctx.ab_reccs(0, y4, x4, K=5)
     outs.append((r["ab"].copy(), pmf.copy(), cen.copy()))
     ctx.close()
-assert np.array_equal(outs[0][0], outs[1][0]) and np.array_equal(outs[0][1], outs[1][1]) and np.array_equal(outs[0][2], outs[1][2])
-print("sanitizer_click: %dx%d, 2 contexts x 3 clicks done; chain == per-layer launches: True; pmf sum %.6f" % (X, X, float(outs[0][1].sum())))
+# the two plans sum in different orders: equal within the parity tolerance, not bit for bit
+d_ab = float(np.abs(outs[0][0] - outs[1][0]).max())
+assert d_ab < 3e-4, d_ab
+print("sanitizer_click: %dx%d, 2 contexts x 3 clicks done; max|d ab| between the plans %.2e; pmf sum %.6f"
+      % (X, X, d_ab, float(outs[0][1].sum())))

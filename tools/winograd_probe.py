@@ -9,7 +9,7 @@ layer (stride-1 3x3, incl. the dilation-2 ones via their 4 parity sub-grids): in
 then rounded to 22 bits, weights transformed G g G^T in FP64 then rounded, 16 element-wise GEMMs, output transform
 A^T m A in FP32.  Both are compared with the plain FP32 oracle (the parity target) and an FP64 evaluation.
 
-    python tools/winograd_probe.py            -> table for profiles/r02_precision_winograd.txt
+    python tools/winograd_probe.py            -> prints the table
 """
 import os
 import sys

@@ -64,19 +64,19 @@ def main(argv=None):
         dist_model = CI.ColorizeImageB200Dist(Xd=X, maskcent=args.pytorch_maskcent)
         dist_model.share_trunk(color_model)             # before the forward: it then carries the distribution head
 
-    im_ab, im_mask = np.zeros((2, X, X)), np.zeros((1, X, X))
     hints = json.load(open(args.hints)) if args.hints else []
-    for h in hints:
-        CI.put_point(im_ab, im_mask, [int(h["loc"][0]), int(h["loc"][1])], int(h.get("size", 3)), hint_ab(h))
-    result = color_model.net_forward(im_ab, im_mask)
+    # the notebook's put_point calls as a rectangle list: the engine rasterises it on the device
+    rects = CI.hints_from_points([([int(h["loc"][0]), int(h["loc"][1])], int(h.get("size", 3)), hint_ab(h)) for h in hints], X)
+    result = color_model.net_forward_hints(rects)
     if isinstance(result, int):
         print("net_forward failed")
         return 1
+    im_ab, im_mask = color_model.input_ab, color_model.input_mask      # the planes put_point would have painted
 
     suggestions = None
     if args.suggest > 0 and hints:
         dist_model.set_image(color_model.img_rgb)
-        dist_model.net_forward(im_ab, im_mask)          # answered from the colour model's forward above
+        dist_model.net_forward_hints(rects)             # answered from the colour model's forward above
         suggestions = []
         for h in hints:
             centers, conf = dist_model.get_ab_reccs(int(h["loc"][0]), int(h["loc"][1]), K=args.suggest, return_conf=True)

@@ -146,6 +146,22 @@ int idc_forward_host_q(idc_ctx* ctx, int n, int h, int w, const float* L_mc, con
  * n = 0 or L_mc = NULL forgets the image. */
 int idc_set_image(idc_ctx* ctx, int n, int h, int w, const float* L_mc);
 
+/* Hint lists: the GUI's and the notebook's hint IS a rectangle painted with one colour (ui/ui_control.py:52-63
+ * PointEdit.updateInput, DemoInteractiveColorization.ipynb put_point), so a click can send the list instead of the
+ * dense ab + mask planes.  Raster semantics: pixel (y, x) of image i takes the LAST hint in list order with img == i,
+ * y0 <= y <= y1 and x0 <= x <= x1 -> ab = (a, b), mask = 1; no hint -> ab = 0, mask = 0.  Rectangles are inclusive,
+ * are clipped to the image, and are empty when y1 < y0 or x1 < x0.  a, b are in the units of the `ab` plane of
+ * idc_forward_host, the mask value 1 is what the `mask` plane would hold.
+ * idc_set_hints copies the list (HOST memory, 0 <= count <= IDC_MAX_HINTS) into a pinned block of the ctx;
+ * idc_forward_host(_q) with ab == NULL && mask == NULL then rasterises that list on the device (hint mode) instead of
+ * uploading planes.  Hint mode combines with L_mc == NULL (resident image): a click uploads only the hint block.
+ * Errors: IDC_ERR_STATE when idc_set_hints was never called, IDC_ERR_ARG when only one of ab / mask is NULL or a hint's
+ * img is outside [0, n) of the forward.  Changing the list never re-captures the click graph (the count travels in the
+ * block).  The device-pointer idc_forward has no hint mode. */
+typedef struct { int32_t img, y0, x0, y1, x1; float a, b; } idc_hint;
+#define IDC_MAX_HINTS 1024
+int idc_set_hints(idc_ctx* ctx, int count, const idc_hint* hints);
+
 /* Page-locked host memory for the zero-copy click path: when every buffer handed to idc_forward_host(_q) with
  * n <= 4 comes from idc_host_alloc (or is otherwise pinned), the copy nodes of the click graph read / write the caller's
  * memory directly (no staging copy by the CPU); buffers laid out back to back -- [L | ab | mask (| glob)] and
@@ -228,6 +244,13 @@ int idc_resize_u8_linear(int device, int h_src, int w_src, const uint8_t* src, i
  * with the window-size L [h,w] float64, skimage lab2rgb, clip, x255, truncating cast -> uint8 [h,w,3].  DEVICE ptrs. */
 int idc_cubic_lab2rgb_u8(int device, int h_in, int w_in, const double* ab, int h, int w, const double* L, uint8_t* rgb,
                          void* stream);
+/* The GUI's gamut map (data/lab_gamut.py:66-78, abGrid(gamut_size, D).update_gamut(L), called on every colour change
+ * by ui/gui_gamut.py): for the A x B grid a = -gamut_size + i*D (row i), b = -gamut_size + j*D (column j),
+ * A = B = len(np.arange(-gamut_size, gamut_size + D, D)):
+ *   rgb  = trunc(255 * clip(lab2rgb(L, a, b), 0, 1))  (uint8)
+ *   mask = |(L, a, b) - rgb2lab(rgb)|_2 < 1            (uint8 0 / 1)
+ * and rgb = 255 where mask is 0 (`masked_rgb`).  float64 like the reference; rgb [A][B][3], mask [A][B] DEVICE ptrs. */
+int idc_gamut_ab(int device, double L, int gamut_size, int D, uint8_t* rgb, uint8_t* mask, void* stream);
 
 /* ---- introspection / test hooks (used by tests/, never by the product path) ---- */
 /* Copy a named activation ("conv1_2", "a8_1", ... see DESIGN.md) of the LAST forward to
@@ -250,6 +273,8 @@ int idc_get_profile(idc_ctx* ctx, float* ms, int max_slots);
 double idc_op_flops(idc_ctx* ctx, int i);
 /* kernels launched by the last forward (gpu_launches in bench.py) */
 int idc_last_launch_count(idc_ctx* ctx);
+/* click-graph instantiations of this ctx so far (a hint-list click must not add one) */
+int idc_graph_captures(idc_ctx* ctx);
 /* FLOPs (2*MACs, conv+deconv) of one image at the ctx geometry; includes model_class iff DIST */
 double idc_flops_per_image(idc_ctx* ctx);
 

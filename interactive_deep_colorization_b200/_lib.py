@@ -7,6 +7,8 @@ memory / streams only; nothing in here touches torch.
 import ctypes
 import os
 
+import numpy as np
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libidc_b200.so")
 if os.environ.get("IDC_B200_LIB"):            # tools only: a build elsewhere (make OUT=...)
@@ -21,6 +23,10 @@ FLAG_NO_GRAPH = 1 << 4
 FLAG_KEEP_CONV10 = 1 << 5
 FLAG_CAFFE313 = 1 << 6
 F32, F64, I64 = 0, 1, 2
+MAX_HINTS = 1024                      # IDC_MAX_HINTS
+# idc_hint: inclusive pixel rectangle of image `img` painted with one ab colour (28 bytes, no padding)
+HINT_DTYPE = np.dtype([("img", "<i4"), ("y0", "<i4"), ("x0", "<i4"), ("y1", "<i4"), ("x1", "<i4"),
+                       ("a", "<f4"), ("b", "<f4")])
 
 # every symbol include/idc_b200.h declares: (name, restype, argtypes)
 _c = ctypes
@@ -38,6 +44,9 @@ SYMBOLS = [
     ("idc_forward_host_q", _c.c_int, [_P, _c.c_int, _c.c_int, _c.c_int, _P, _P, _P, _c.c_float, _P, _P, _P, _P, _P]),
     ("idc_set_option", _c.c_int, [_P, _c.c_char_p, _c.c_int]),
     ("idc_set_image", _c.c_int, [_P, _c.c_int, _c.c_int, _c.c_int, _P]),
+    ("idc_set_hints", _c.c_int, [_P, _c.c_int, _P]),
+    ("idc_gamut_ab", _c.c_int, [_c.c_int, _c.c_double, _c.c_int, _c.c_int, _P, _P, _P]),
+    ("idc_graph_captures", _c.c_int, [_P]),
     ("idc_host_alloc", _P, [_c.c_size_t]),
     ("idc_host_free", _c.c_int, [_P]),
     ("idc_set_dist_resident", _c.c_int, [_P, _c.c_int]),

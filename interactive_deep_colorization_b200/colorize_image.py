@@ -14,7 +14,7 @@ and the Lab->RGB post-process run in libidc_b200.so.  There is no CPU fallback.
 """
 import numpy as np
 
-from . import color
+from . import color, engine
 from .color import lab2rgb_transpose, rgb2lab_transpose  # noqa: F401  (re-exported like the reference)
 
 
@@ -23,6 +23,61 @@ def put_point(input_ab, mask, loc, p, val):
     input_ab[:, loc[0] - p:loc[0] + p + 1, loc[1] - p:loc[1] + p + 1] = np.array(val)[:, np.newaxis, np.newaxis]
     mask[:, loc[0] - p:loc[0] + p + 1, loc[1] - p:loc[1] + p + 1] = 1
     return (input_ab, mask)
+
+
+# A hint list on the wrapper side: the fields of the C ABI's idc_hint (engine.as_hints), with a / b kept in float64 so
+# that the host planes rasterised from it equal the planes put_point paints.  The engine rounds a / b to float32, as it
+# rounds the dense ab plane.
+HINT_LIST_DTYPE = np.dtype([("img", "<i4"), ("y0", "<i4"), ("x0", "<i4"), ("y1", "<i4"), ("x1", "<i4"),
+                            ("a", "<f8"), ("b", "<f8")])
+
+
+def hints_from_points(points, X, img=0):
+    """put_point(input_ab, mask, loc, p, val) calls on X x X planes -> the equivalent hint list (HINT_LIST_DTYPE), in
+    call order.  Row / column ranges follow numpy's slice semantics exactly (`slice(loc - p, loc + p + 1).indices(X)`):
+    a negative start wraps around and, as in put_point, usually leaves the slice empty.  points: (loc, p, val) each."""
+    out = np.zeros(len(points), HINT_LIST_DTYPE)
+    for i, (loc, p, val) in enumerate(points):
+        y0, y1, _ = slice(int(loc[0]) - int(p), int(loc[0]) + int(p) + 1).indices(X)
+        x0, x1, _ = slice(int(loc[1]) - int(p), int(loc[1]) + int(p) + 1).indices(X)
+        out[i] = (img, y0, x0, y1 - 1, x1 - 1, float(val[0]), float(val[1]))
+    return out
+
+
+def raster_hints(rects, X, img=0):
+    """Host raster of a hint list (the idc_set_hints semantics) -> (ab [2,X,X], mask [1,X,X]) float64, the planes a
+    dense net_forward would have received."""
+    ab, mask = np.zeros((2, X, X)), np.zeros((1, X, X))
+    for h in rects:
+        if int(h["img"]) != img:
+            continue
+        y0, x0 = max(int(h["y0"]), 0), max(int(h["x0"]), 0)
+        y1, x1 = min(int(h["y1"]), X - 1), min(int(h["x1"]), X - 1)
+        if y1 >= y0 and x1 >= x0:
+            ab[0, y0:y1 + 1, x0:x1 + 1] = h["a"]
+            ab[1, y0:y1 + 1, x0:x1 + 1] = h["b"]
+            mask[:, y0:y1 + 1, x0:x1 + 1] = 1
+    return ab, mask
+
+
+def _lazy_hint_plane(name):
+    """input_ab / input_mask / input_ab_mc / input_mask_mult: plain attributes after a dense net_forward; after
+    net_forward_hints they are rasterised on the host on first read (a click itself never needs them)."""
+    key = "_" + name
+
+    def get(self):
+        d = self.__dict__
+        if key not in d and d.get("_hint_rects") is not None:
+            self._rasterise_hints()
+        if key not in d:
+            raise AttributeError(name)
+        return d[key]
+
+    def set(self, v):
+        self.__dict__[key] = v
+        self.__dict__["_hint_rects"] = None      # dense planes given: no hint list behind them
+
+    return property(get, set)
 
 
 def _zoom(a, factors, order):
@@ -62,18 +117,49 @@ class ColorizeImageBase(object):
     def set_image(self, input_image):
         self._ingest(input_image.copy(), input_image)
 
+    input_ab = _lazy_hint_plane("input_ab")
+    input_mask = _lazy_hint_plane("input_mask")
+    input_ab_mc = _lazy_hint_plane("input_ab_mc")
+    input_mask_mult = _lazy_hint_plane("input_mask_mult")
+
     # ----- forward preconditions + hint normalisation: reference :79-96 -----
     def net_forward(self, input_ab, input_mask):
+        hints = self.__dict__.pop("_hints_next", None)      # set by net_forward_hints for this one call
         for ok, what in ((self.img_l_set, 'an image'), (self.net_set, 'a net')):
             if not ok:
                 print('I need to have %s!' % what)
                 return -1
+        if hints is not None:
+            for k in ("_input_ab", "_input_mask", "_input_ab_mc", "_input_mask_mult"):
+                self.__dict__.pop(k, None)
+            self._hint_rects = hints                          # the four planes now derive from the list, lazily
+            return 0
         self.input_ab, self.input_mask = input_ab, input_mask
         # reference :92-93.  With the PyTorch constants (ab_mean 0, ab_norm 1, mask_mult 1) both statements are exact
         # identities; skipping the two float64 temporaries (2.5 MB of numpy traffic) is worth ~0.1 ms per click
         self.input_ab_mc = input_ab if (self.ab_mean == 0 and self.ab_norm == 1) else (input_ab - self.ab_mean) / self.ab_norm
         self.input_mask_mult = input_mask if self.mask_mult == 1 else input_mask * self.mask_mult
         return 0
+
+    def net_forward_hints(self, rects, glob_dist=-1):
+        """net_forward with the hints given as a list of rectangles (HINT_LIST_DTYPE, e.g. from hints_from_points)
+        instead of dense ab / mask planes.  The result equals net_forward(*raster_hints(rects, Xd)); where the engine's
+        click path runs, the list itself travels to the device and is rasterised there.  input_ab / input_mask /
+        input_ab_mc / input_mask_mult read as the dense call would have set them (computed on first read)."""
+        self._hints_next = np.array(rects, dtype=HINT_LIST_DTYPE).reshape(-1)
+        try:
+            if np.array(glob_dist).flatten()[0] != -1:
+                return self.net_forward(None, None, glob_dist)
+            return self.net_forward(None, None)
+        finally:
+            self.__dict__.pop("_hints_next", None)
+
+    def _rasterise_hints(self):
+        ab, mask = raster_hints(self._hint_rects, self.img_l_mc.shape[-1])
+        d = self.__dict__
+        d["_input_ab"], d["_input_mask"] = ab, mask
+        d["_input_ab_mc"] = ab if (self.ab_mean == 0 and self.ab_norm == 1) else (ab - self.ab_mean) / self.ab_norm
+        d["_input_mask_mult"] = mask if self.mask_mult == 1 else mask * self.mask_mult
 
     def get_result_PSNR(self, result=-1, return_SE_map=False):
         use_own = np.array((result)).flatten()[0] == -1
@@ -209,24 +295,32 @@ class ColorizeImageB200(ColorizeImageBase):
         the pinned buffers (zero-copy graph path) and publish copies of the results as the reference's attributes."""
         buf = self._click_buffers(ctx, glob is not None)
         want_q = bool(want_rgb and self.gpu_prepost)
+        rects = self.__dict__.get("_hint_rects")            # net_forward_hints: the list goes to the device, not planes
         if ctx._wrapper_shared and glob is None and \
                 self._same_as_last_forward(ctx, buf, maskcent, mask_div, want_rgb, want_q, need_dist):
             # share_trunk: the other model of the pair just ran this very forward; its results are still in the buffers
             r = {"ab": buf["out_ab"], "rgb": buf["out_rgb"], "abq": buf["out_abq"]}
         else:
             self._stage_image(ctx, buf)
-            np.copyto(buf["ab"][0], self.input_ab_mc, casting='unsafe')
-            if mask_div == 1.0:
-                np.copyto(buf["mask"][0], self.input_mask_mult, casting='unsafe')
+            if rects is not None:
+                hints = engine.as_hints(rects)
+                ctx.set_hints(hints)
+                ab_in = mask_in = None
             else:
-                np.divide(self.input_mask_mult, mask_div, out=buf["mask"][0], casting='unsafe')
+                np.copyto(buf["ab"][0], self.input_ab_mc, casting='unsafe')
+                if mask_div == 1.0:
+                    np.copyto(buf["mask"][0], self.input_mask_mult, casting='unsafe')
+                else:
+                    np.divide(self.input_mask_mult, mask_div, out=buf["mask"][0], casting='unsafe')
+                ab_in, mask_in = buf["ab"], buf["mask"]
             if glob is not None:
                 buf["glob"][...] = glob
             ctx._wrapper_last = None
             # L_mc = None: the image uploaded by _stage_image (idc_set_image) -- a click moves only the hints
-            r = ctx.forward_host(None, buf["ab"], buf["mask"], maskcent, glob=buf["glob"], want_rgb=want_rgb,
+            r = ctx.forward_host(None, ab_in, mask_in, maskcent, glob=buf["glob"], want_rgb=want_rgb, n=1,
                                  want_abq=want_q, out_ab=buf["out_ab"], out_rgb=buf["out_rgb"] if want_rgb else None,
                                  out_abq=buf["out_abq"] if want_q else None)
+            ctx._wrapper_hints = None if rects is None else hints
             ctx._wrapper_last = (float(maskcent), float(mask_div), glob is not None, bool(want_rgb), want_q,
                                  bool(getattr(ctx, "_dist_resident", False)))
         self.output_ab_raw = r["ab"][0].copy()   # raw net output (the parity quantity, SURVEY q2)
@@ -261,6 +355,12 @@ class ColorizeImageB200(ColorizeImageBase):
             if not (ctx._wrapper_staged_l and np.array_equal(buf["L_mc"], l32)):
                 return False
             ctx._wrapper_staged_l = ctx._wrapper_staged_l[-3:] + [self.img_l_mc]
+        last_hints = getattr(ctx, "_wrapper_hints", None)
+        rects = self.__dict__.get("_hint_rects")
+        if rects is not None:                    # hint lists: compare the lists (as the engine received them), not planes
+            return last_hints is not None and np.array_equal(last_hints, engine.as_hints(rects))
+        if last_hints is not None:               # the last forward rasterised a list; the plane buffers are stale
+            return False
         mask32 = np.asarray(self.input_mask_mult, dtype=np.float32)
         if mask_div != 1.0:
             mask32 = mask32 / np.float32(mask_div)

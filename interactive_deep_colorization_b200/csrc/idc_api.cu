@@ -523,7 +523,7 @@ int side_branch_cap(Ctx* c) {
 
 int run_forward(Ctx* c, int n, const float* L, const float* ab, const float* mask, float maskcent, const float* glob,
                 float* out_ab, float* out_dist, uint8_t* out_rgb, cudaStream_t st, const HostPipe* hp = nullptr,
-                double* out_abq = nullptr) {
+                double* out_abq = nullptr, const char* hints_dev = nullptr) {
   c->launch_count = 0;
   c->gadd_active = false;
   c->click_served = false;
@@ -547,6 +547,8 @@ int run_forward(Ctx* c, int n, const float* L, const float* ab, const float* mas
   }
   const size_t HW = (size_t)c->H * c->W;
   const bool c11_umma = c->opt.conv1_1_umma && !c->simt && c->w11_umma;
+  // hint mode: the ab / mask planes conv1_1 reads are rasterised here from the hint block (already on the device)
+  if (hints_dev) CUDA_TRY(c, launch_hint_raster(c, n, hints_dev, const_cast<float*>(ab), const_cast<float*>(mask), st));
   if (hp) {
     for (int k = 0; k < hp->nchunks; ++k) {
       CUDA_TRY(c, cudaStreamWaitEvent(st, c->ev_in[k], 0));
@@ -644,11 +646,13 @@ int run_forward(Ctx* c, int n, const float* L, const float* ab, const float* mas
 }
 
 int check_forward_args(Ctx* c, int n, int h, int w, const void* L, const void* ab, const void* mask, const void* glob,
-                       const void* out_ab, const void* out_dist, bool resident_l_ok = false) {
+                       const void* out_ab, const void* out_dist, bool resident_l_ok = false, bool hints_ok = false) {
   if (!c->weights_ready) return fail(c, IDC_ERR_STATE, "idc_forward before idc_finalize_weights");
   if (n < 1 || n > c->max_n) return fail(c, IDC_ERR_ARG, "n=%d outside [1,%d]", n, c->max_n);
   if (h != c->H || w != c->W) return fail(c, IDC_ERR_ARG, "geometry %dx%d != ctx geometry %dx%d", h, w, c->H, c->W);
-  if ((!L && !resident_l_ok) || !ab || !mask || !out_ab) return fail(c, IDC_ERR_ARG, "null L/ab/mask/out_ab");
+  const bool hint_mode = hints_ok && !ab && !mask;     // idc_set_hints list instead of planes
+  if ((!L && !resident_l_ok) || ((!ab || !mask) && !hint_mode) || !out_ab)
+    return fail(c, IDC_ERR_ARG, "null L/ab/mask/out_ab");
   if (out_dist && !c->dist) return fail(c, IDC_ERR_ARG, "out_dist requires IDC_FLAG_DIST");
   if (glob && !c->glob) return fail(c, IDC_ERR_ARG, "glob requires IDC_FLAG_GLOBAL_HINTS");
   return IDC_OK;
@@ -812,8 +816,11 @@ int idc_forward_host(idc_ctx* c, int n, int h, int w, const float* L, const floa
 //     memory directly -- no CPU copy at all.  Buffers laid out back to back ([L | ab | mask | glob], [ab | rgb | abq])
 //     travel as ONE copy each way.  The graph is keyed on the pointers and re-captured when they change.
 //   * pageable caller buffers: staged through the context's pinned blocks by the CPU (one copy node each way).
+//   * hint mode (ab == mask == NULL): the ab / mask H2D is replaced by one fixed-size copy of the whole pinned hint block
+//     and the raster kernel; the list length lives in the block, so editing the hints never re-captures the graph.
 static int forward_host_small(idc_ctx* c, int n, const float* L, const float* ab, const float* mask, float maskcent,
-                              const float* glob, float* out_ab, float* out_dist, uint8_t* out_rgb, double* out_abq) {
+                              const float* glob, float* out_ab, float* out_dist, uint8_t* out_rgb, double* out_abq,
+                              bool hint_mode) {
   const size_t HW = (size_t)c->H * c->W, HW4 = (size_t)(c->H / 4) * (c->W / 4);
   cudaStream_t st = c->own_stream;
   const bool copy_dist = out_dist != nullptr;
@@ -830,7 +837,8 @@ static int forward_host_small(idc_ctx* c, int n, const float* L, const float* ab
   float* ddist = c->d_out + (size_t)c->max_n * 2 * HW;
   const size_t out_bytes = b_ab + (want_rgb ? b_rgb : 0) + (want_q ? b_q : 0);
   const uintptr_t flags = (uintptr_t)n | ((uintptr_t)want_dist << 8) | ((uintptr_t)want_rgb << 9) | ((uintptr_t)want_glob << 10) |
-                          ((uintptr_t)want_q << 11) | ((uintptr_t)copy_dist << 12) | ((uintptr_t)c->click_mode << 13);
+                          ((uintptr_t)want_q << 11) | ((uintptr_t)copy_dist << 12) | ((uintptr_t)c->click_mode << 13) |
+                          ((uintptr_t)hint_mode << 14);
   c->click_served = false;
   const bool have_L = L != nullptr;          // false: the image set by idc_set_image stays where it is
   const size_t in_floats = (size_t)n * (have_L ? 4 : 3) * HW + (want_glob ? (size_t)n * 316 : 0);
@@ -840,15 +848,18 @@ static int forward_host_small(idc_ctx* c, int n, const float* L, const float* ab
                 c->graph_maskcent == maskcent;
   bool replay = direct;
   if (!direct) {
-    direct = !copy_dist && (!have_L || is_pinned(L)) && is_pinned(ab) && is_pinned(mask) && (!glob || is_pinned(glob)) &&
-             is_pinned(out_ab) && (!out_rgb || is_pinned(out_rgb)) && (!out_abq || is_pinned(out_abq));
+    direct = !copy_dist && (!have_L || is_pinned(L)) && (hint_mode || (is_pinned(ab) && is_pinned(mask))) &&
+             (!glob || is_pinned(glob)) && is_pinned(out_ab) && (!out_rgb || is_pinned(out_rgb)) &&
+             (!out_abq || is_pinned(out_abq));
   }
   const void* staged_key[8] = {(void*)(flags | ((uintptr_t)have_L << 17)), nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
   const void** key = direct ? direct_key : staged_key;
   if (!direct) {   // stage the inputs
     if (have_L) memcpy(c->h_in, L, (size_t)n * HW * sizeof(float));
-    memcpy(c->h_in + (size_t)n * HW, ab, (size_t)n * 2 * HW * sizeof(float));
-    memcpy(c->h_in + (size_t)n * 3 * HW, mask, (size_t)n * HW * sizeof(float));
+    if (!hint_mode) {
+      memcpy(c->h_in + (size_t)n * HW, ab, (size_t)n * 2 * HW * sizeof(float));
+      memcpy(c->h_in + (size_t)n * 3 * HW, mask, (size_t)n * HW * sizeof(float));
+    }
     if (want_glob) memcpy(c->h_in + (size_t)n * 4 * HW, glob, (size_t)n * 316 * sizeof(float));
   }
   if (!replay && (!c->graph_exec || memcmp(key, c->graph_ptrs, sizeof(staged_key)) != 0 || c->graph_maskcent != maskcent)) {
@@ -861,7 +872,11 @@ static int forward_host_small(idc_ctx* c, int n, const float* L, const float* ab
     auto cp = [&](void* dst, const void* src, size_t bytes, cudaMemcpyKind kind) {
       if (ce == cudaSuccess && bytes) ce = cudaMemcpyAsync(dst, src, bytes, kind, st);
     };
-    if (direct) {
+    if (hint_mode) {   // the whole hint block (fixed size), then the L planes and the glob vector if they travel
+      cp(c->d_hints, c->h_hints, kHintBlockBytes, cudaMemcpyHostToDevice);
+      if (have_L) cp(dL, direct ? L : c->h_in, (size_t)n * HW * sizeof(float), cudaMemcpyHostToDevice);
+      if (want_glob) cp(dglob, direct ? glob : c->h_in + (size_t)n * 4 * HW, (size_t)n * 316 * sizeof(float), cudaMemcpyHostToDevice);
+    } else if (direct) {
       const bool contig = (!have_L || ab == L + (size_t)n * HW) && mask == ab + (size_t)n * 2 * HW &&
                           (!want_glob || glob == mask + (size_t)n * HW);
       if (contig) {
@@ -879,7 +894,7 @@ static int forward_host_small(idc_ctx* c, int n, const float* L, const float* ab
     int rc = IDC_OK;
     if (ce == cudaSuccess)
       rc = run_forward(c, n, dL, dab, dmask, maskcent, want_glob ? dglob : nullptr, dout, want_dist ? ddist : nullptr,
-                       want_rgb ? drgb : nullptr, st, nullptr, want_q ? dq : nullptr);
+                       want_rgb ? drgb : nullptr, st, nullptr, want_q ? dq : nullptr, hint_mode ? c->d_hints : nullptr);
     if (rc == IDC_OK) {
       if (direct) {
         const char* o0 = reinterpret_cast<const char*>(out_ab);
@@ -906,6 +921,7 @@ static int forward_host_small(idc_ctx* c, int n, const float* L, const float* ab
     ce = cudaGraphInstantiate(&c->graph_exec, g, 0);
     cudaGraphDestroy(g);
     CUDA_TRY(c, ce);
+    c->graph_captures++;
     memcpy(c->graph_ptrs, key, sizeof(staged_key));
     c->graph_maskcent = maskcent;
     c->graph_launches = c->launch_count;
@@ -963,13 +979,39 @@ int idc_set_image(idc_ctx* c, int n, int h, int w, const float* L) {
   return IDC_OK;
 }
 
+int idc_set_hints(idc_ctx* c, int count, const idc_hint* hints) {
+  if (!c) return IDC_ERR_ARG;
+  if (count < 0 || count > IDC_MAX_HINTS) return fail(c, IDC_ERR_ARG, "count=%d outside [0,%d]", count, IDC_MAX_HINTS);
+  if (count && !hints) return fail(c, IDC_ERR_ARG, "null hint list");
+  if (!c->h_hints) {
+    CUDA_TRY(c, cudaSetDevice(c->dev));
+    CUDA_TRY(c, cudaMalloc(&c->d_hints, kHintBlockBytes));
+    CUDA_TRY(c, cudaMallocHost(&c->h_hints, kHintBlockBytes));
+    memset(c->h_hints, 0, kHintBlockBytes);
+  }
+  // every idc_forward_host(_q) has synchronised before returning: no copy of the block is in flight
+  int* hdr = reinterpret_cast<int*>(c->h_hints);
+  hdr[0] = count;
+  if (count) memcpy(c->h_hints + kHintHdrBytes, hints, (size_t)count * sizeof(idc_hint));
+  return IDC_OK;
+}
+
 int idc_forward_host_q(idc_ctx* c, int n, int h, int w, const float* L, const float* ab, const float* mask,
                        float maskcent, const float* glob, float* out_ab, float* out_dist, uint8_t* out_rgb,
                        double* out_abq) {
   if (!c) return IDC_ERR_ARG;
-  int rc = check_forward_args(c, n, h, w, L, ab, mask, glob, out_ab, out_dist, /*resident_l_ok=*/true);   // NULL L: idc_set_image
+  // NULL L: idc_set_image; NULL ab and mask: idc_set_hints
+  int rc = check_forward_args(c, n, h, w, L, ab, mask, glob, out_ab, out_dist, /*resident_l_ok=*/true, /*hints_ok=*/true);
   if (rc != IDC_OK) return rc;
   if (out_abq && !out_rgb) return fail(c, IDC_ERR_ARG, "out_abq (quantised ab) is derived from out_rgb: pass both");
+  const bool hint_mode = !ab && !mask;
+  if (hint_mode) {
+    if (!c->h_hints) return fail(c, IDC_ERR_STATE, "ab and mask are NULL but idc_set_hints was never called");
+    const int count = *reinterpret_cast<const int*>(c->h_hints);
+    const idc_hint* hs = reinterpret_cast<const idc_hint*>(c->h_hints + kHintHdrBytes);
+    for (int i = 0; i < count; ++i)
+      if (hs[i].img < 0 || hs[i].img >= n) return fail(c, IDC_ERR_ARG, "hint %d: img=%d outside [0,%d)", i, hs[i].img, n);
+  }
   CUDA_TRY(c, cudaSetDevice(c->dev));
   if (int werr = *(volatile int*)c->h_err) {           // a watchdog left over from an asynchronous idc_forward
     *(volatile int*)c->h_err = 0;
@@ -982,7 +1024,7 @@ int idc_forward_host_q(idc_ctx* c, int n, int h, int w, const float* L, const fl
     return fail(c, IDC_ERR_STATE, "L_mc is NULL but no %d-image set is resident (idc_set_image)", n);
   const bool use_graph = !(c->flags & IDC_FLAG_NO_GRAPH) && n <= 4;
   if (use_graph) {
-    rc = forward_host_small(c, n, L, ab, mask, maskcent, glob, out_ab, out_dist, out_rgb, out_abq);
+    rc = forward_host_small(c, n, L, ab, mask, maskcent, glob, out_ab, out_dist, out_rgb, out_abq, hint_mode);
     if (rc != IDC_OK) return rc;
     if (int werr = *(volatile int*)c->h_err) {
       *(volatile int*)c->h_err = 0;
@@ -1030,18 +1072,26 @@ int idc_forward_host_q(idc_ctx* c, int n, int h, int w, const float* L, const fl
     cudaStream_t compute = st;
     st = c->s_in;                                   // the h2d lambda copies on `st`
     if (glob) CUDA_TRY(c, h2d(dglob, glob, (size_t)n * 316, (size_t)c->max_n * 4 * HW));
+    // hint mode: the block goes ahead of the first L chunk, so ev_in[0] (which the raster launch waits for) covers it
+    if (hint_mode) CUDA_TRY(c, cudaMemcpyAsync(c->d_hints, c->h_hints, kHintBlockBytes, cudaMemcpyHostToDevice, st));
     for (int k = 0; k < hp.nchunks; ++k) {
       const size_t i0 = hp.start[k], nk = hp.start[k + 1] - hp.start[k];
       if (L) CUDA_TRY(c, h2d(dL + i0 * HW, L + i0 * HW, nk * HW, i0 * HW));
-      CUDA_TRY(c, h2d(dab + i0 * 2 * HW, ab + i0 * 2 * HW, nk * 2 * HW, (size_t)c->max_n * HW + i0 * 2 * HW));
-      CUDA_TRY(c, h2d(dmask + i0 * HW, mask + i0 * HW, nk * HW, (size_t)c->max_n * 3 * HW + i0 * HW));
+      if (!hint_mode) {
+        CUDA_TRY(c, h2d(dab + i0 * 2 * HW, ab + i0 * 2 * HW, nk * 2 * HW, (size_t)c->max_n * HW + i0 * 2 * HW));
+        CUDA_TRY(c, h2d(dmask + i0 * HW, mask + i0 * HW, nk * HW, (size_t)c->max_n * 3 * HW + i0 * HW));
+      }
       CUDA_TRY(c, cudaEventRecord(c->ev_in[k], c->s_in));
     }
     st = compute;
   } else {
     if (L) CUDA_TRY(c, h2d(dL, L, n * HW, 0));
-    CUDA_TRY(c, h2d(dab, ab, n * 2 * HW, (size_t)c->max_n * HW));
-    CUDA_TRY(c, h2d(dmask, mask, n * HW, (size_t)c->max_n * 3 * HW));
+    if (hint_mode) {
+      CUDA_TRY(c, cudaMemcpyAsync(c->d_hints, c->h_hints, kHintBlockBytes, cudaMemcpyHostToDevice, st));
+    } else {
+      CUDA_TRY(c, h2d(dab, ab, n * 2 * HW, (size_t)c->max_n * HW));
+      CUDA_TRY(c, h2d(dmask, mask, n * HW, (size_t)c->max_n * 3 * HW));
+    }
     if (glob) CUDA_TRY(c, h2d(dglob, glob, (size_t)n * 316, (size_t)c->max_n * 4 * HW));
   }
 
@@ -1049,7 +1099,8 @@ int idc_forward_host_q(idc_ctx* c, int n, int h, int w, const float* L, const fl
   const bool want_dist = copy_dist || (c->dist_resident && c->dist);
   const bool want_rgb = out_rgb != nullptr, want_glob = glob != nullptr;
   rc = run_forward(c, n, dL, dab, dmask, maskcent, want_glob ? dglob : nullptr, dout, want_dist ? ddist : nullptr,
-                   want_rgb ? c->d_rgb : nullptr, st, hp.nchunks ? &hp : nullptr, out_abq ? c->d_abq : nullptr);
+                   want_rgb ? c->d_rgb : nullptr, st, hp.nchunks ? &hp : nullptr, out_abq ? c->d_abq : nullptr,
+                   hint_mode ? c->d_hints : nullptr);
   if (rc != IDC_OK) return rc;
   auto d2h = [&](void* dst, const void* d, size_t bytes, void* stage) -> cudaError_t {
     if (is_pinned(dst)) return cudaMemcpyAsync(dst, d, bytes, cudaMemcpyDeviceToHost, st);
@@ -1294,6 +1345,13 @@ int idc_cubic_lab2rgb_u8(int device, int h_in, int w_in, const double* ab, int h
   return launch_cubic_lab2rgb(ab, h_in, w_in, L, h, w, rgb, (cudaStream_t)stream) == cudaSuccess ? IDC_OK : IDC_ERR_CUDA;
 }
 
+int idc_gamut_ab(int device, double L, int gamut_size, int D, uint8_t* rgb, uint8_t* mask, void* stream) {
+  if (gamut_size < 0 || gamut_size > 4096 || D < 1 || !rgb || !mask) return IDC_ERR_ARG;
+  const int A = (2 * gamut_size + D - 1) / D + 1;        // len(np.arange(-g, g + D, D))
+  if (cudaSetDevice(device) != cudaSuccess) return IDC_ERR_CUDA;
+  return launch_gamut(L, gamut_size, D, A, rgb, mask, (cudaStream_t)stream) == cudaSuccess ? IDC_OK : IDC_ERR_CUDA;
+}
+
 int idc_get_activation(idc_ctx* c, const char* name, float* out, size_t out_floats, int* ch, int* h, int* w) {
   if (!c || !name) return IDC_ERR_ARG;
   auto it = c->buf_index.find(name);
@@ -1395,6 +1453,7 @@ const char* idc_op_name(idc_ctx* c, int i) {
   return (c && i >= 0 && i < (int)c->ops.size()) ? c->ops[i].name.c_str() : nullptr;
 }
 int idc_last_launch_count(idc_ctx* c) { return c ? c->launch_count : 0; }
+int idc_graph_captures(idc_ctx* c) { return c ? c->graph_captures : 0; }
 
 double idc_flops_per_image(idc_ctx* c) {
   if (!c) return 0;
@@ -1438,6 +1497,8 @@ int idc_destroy(idc_ctx* c) {
   if (c->h_click) cudaFreeHost(c->h_click);
   if (c->d_clickout) cudaFree(c->d_clickout);
   if (c->h_clickout) cudaFreeHost(c->h_clickout);
+  if (c->h_hints) cudaFreeHost(c->h_hints);
+  if (c->d_hints) cudaFree(c->d_hints);
   if (c->dbg_ev[0]) { cudaEventDestroy(c->dbg_ev[0]); cudaEventDestroy(c->dbg_ev[1]); }
   if (c->own_stream) cudaStreamDestroy(c->own_stream);
   if (c->s_click) { cudaStreamDestroy(c->s_click); cudaEventDestroy(c->ev_click[0]); cudaEventDestroy(c->ev_click[1]); }

@@ -184,6 +184,9 @@ struct Ctx {
   cudaStream_t s_click = nullptr;            // announced click: pmf + suggestions next to the full-map softmax
   cudaEvent_t ev_click[2] = {nullptr, nullptr};
   int image_n = 0;                           // idc_set_image: this many L planes are resident at the head of d_in
+  // idc_set_hints: [kHintHdrBytes header (int count) | IDC_MAX_HINTS x idc_hint], pinned host + device copy
+  char* h_hints = nullptr; char* d_hints = nullptr;
+  int graph_captures = 0;                    // click-graph instantiations (idc_graph_captures)
   cudaEvent_t ev_in[8] = {}, ev_out[8] = {};
   // CUDA graph cache for the batch-1 latency path
   cudaGraphExec_t graph_exec = nullptr;
@@ -222,6 +225,13 @@ cudaError_t launch_conv1_1(Ctx* c, int n, const float* L, const float* ab, const
 cudaError_t launch_conv1_1_umma(Ctx* c, int n, const float* L, const float* ab, const float* mask, float maskcent,
                                 cudaStream_t st, int img0 = 0);              // the same layer on the tensor cores
 cudaError_t conv1_1_umma_pack(Ctx* c);                                       // weight tile for it, from the arena (device)
+// hint block of idc_set_hints: a 16-byte header {count, 0, 0, 0}, then IDC_MAX_HINTS idc_hint entries.  It always
+// travels whole, so the copy is the same graph node whatever the count.
+constexpr size_t kHintHdrBytes = 16;
+constexpr size_t kHintBlockBytes = kHintHdrBytes + (size_t)IDC_MAX_HINTS * sizeof(idc_hint);
+// rasterise the hint block (device) into the ab [n,2,H,W] / mask [n,1,H,W] planes conv1_1 reads
+cudaError_t launch_hint_raster(Ctx* c, int n, const char* hints_dev, float* ab, float* mask, cudaStream_t st);
+cudaError_t launch_gamut(double L, int gamut_size, int D, int A, uint8_t* rgb, uint8_t* mask, cudaStream_t st);
 cudaError_t launch_out_head(Ctx* c, int n, float* out_ab, cudaStream_t st);   // SIMT / KEEP_CONV10 path
 cudaError_t launch_softmax529(Ctx* c, int n, float* out_dist, cudaStream_t st);
 cudaError_t launch_lab2rgb(Ctx* c, int n, int h, int w, const float* L, float l_offset, const float* ab,

@@ -14,6 +14,17 @@ def _np_ptr(a):
     return ctypes.c_void_p(a.ctypes.data)
 
 
+def as_hints(rects):
+    """A hint list as the C ABI's idc_hint array: a structured array with the fields img, y0, x0, y1, x1, a, b (any
+    numeric field types; a / b are rounded to float32 like the dense ab plane) or a sequence of such 7-tuples."""
+    if isinstance(rects, np.ndarray) and rects.dtype.names:
+        out = np.empty(rects.shape[0], _lib.HINT_DTYPE)
+        for f in _lib.HINT_DTYPE.names:
+            out[f] = rects[f]
+        return out
+    return np.array([tuple(r) for r in rects], dtype=_lib.HINT_DTYPE).reshape(-1)
+
+
 class LhnContext(object):
     """Local Hints Network forward context (the H100 stand-in for
     `SIGGRAPHGenerator(...).cuda().eval()`, /root/reference/data/colorize_image.py:221-232)."""
@@ -125,17 +136,32 @@ class LhnContext(object):
         assert L_mc.dtype == np.float32 and L_mc.flags["C_CONTIGUOUS"]
         _lib.check(self.h, self.lib.idc_set_image(self.h, int(L_mc.shape[0]), self.H, self.W, _np_ptr(L_mc)))
 
+    def set_hints(self, rects):
+        """The hint list the next forward_host(..., None, None, n=...) rasterises on the device (idc_set_hints):
+        rectangles (img, y0, x0, y1, x1, a, b), inclusive and clipped to the image; later ones paint over earlier ones.
+        See `as_hints` for the accepted forms."""
+        h = as_hints(rects)
+        if h.shape[0] > _lib.MAX_HINTS:
+            raise ValueError("at most %d hints, got %d" % (_lib.MAX_HINTS, h.shape[0]))
+        _lib.check(self.h, self.lib.idc_set_hints(self.h, int(h.shape[0]), _np_ptr(h) if h.shape[0] else None))
+
+    def graph_captures(self):
+        """Click-graph instantiations of this context so far."""
+        return self.lib.idc_graph_captures(self.h)
+
     def forward_host(self, L_mc, ab, mask, maskcent=0.0, glob=None, want_dist=False, want_rgb=False,
-                     out_ab=None, out_dist=None, out_rgb=None, want_abq=False, out_abq=None):
+                     out_ab=None, out_dist=None, out_rgb=None, want_abq=False, out_abq=None, n=None):
         """numpy float32 C-contiguous host arrays (pinned or pageable) -> dict of numpy arrays.
         Synchronous; includes H2D + D2H.  want_abq: also the reference's quantised output_ab
-        (rgb2lab(rgb)[1:], float64; implies want_rgb).  L_mc None = the image uploaded by set_image."""
+        (rgb2lab(rgb)[1:], float64; implies want_rgb).  L_mc None = the image uploaded by set_image.
+        ab and mask None = the hint list of set_hints, rasterised on the device; pass the batch size as n."""
         want_rgb = want_rgb or want_abq
-        n = ab.shape[0]
+        if n is None:
+            n = (ab if ab is not None else L_mc).shape[0]
         if L_mc is not None:                 # an explicit L replaces the resident image: wrappers must re-stage theirs
             self._wrapper_staged_l, self._wrapper_last = [], None
-        for a in (ab, mask) + (() if L_mc is None else (L_mc,)):
-            assert a.dtype == np.float32 and a.flags["C_CONTIGUOUS"]
+        for a in (ab, mask, L_mc):
+            assert a is None or (a.dtype == np.float32 and a.flags["C_CONTIGUOUS"])
         if out_ab is None:
             out_ab = np.empty((n, 2, self.H, self.W), np.float32)
         if want_dist and out_dist is None:
@@ -144,7 +170,8 @@ class LhnContext(object):
             out_rgb = np.empty((n, self.H, self.W, 3), np.uint8)
         if want_abq and out_abq is None:
             out_abq = np.empty((n, 2, self.H, self.W), np.float64)
-        rc = self.lib.idc_forward_host_q(self.h, n, self.H, self.W, None if L_mc is None else _np_ptr(L_mc), _np_ptr(ab), _np_ptr(mask),
+        rc = self.lib.idc_forward_host_q(self.h, n, self.H, self.W, None if L_mc is None else _np_ptr(L_mc),
+                                         None if ab is None else _np_ptr(ab), None if mask is None else _np_ptr(mask),
                                          float(maskcent), _np_ptr(glob) if glob is not None else None,
                                          _np_ptr(out_ab), _np_ptr(out_dist) if want_dist else None,
                                          _np_ptr(out_rgb) if want_rgb else None,
@@ -154,11 +181,23 @@ class LhnContext(object):
                 "abq": out_abq}
 
     # ---- zero-copy click path ---------------------------------------------------------------
-    def click_buffers(self, n=1, glob=False):
+    def click_buffers(self, n=1, glob=False, hints=False):
         """Page-locked I/O arrays for the interactive call (n <= 4), laid out back to back so that a click is one H2D and
         one D2H with NO copy by the CPU: pass them to forward_host (L_mc / ab / mask (/ glob) as inputs, out_ab / out_rgb /
-        out_abq as outputs).  -> dict of numpy views; they stay valid until close()."""
+        out_abq as outputs).  -> dict of numpy views; they stay valid until close().  hints=True: for hint-list clicks
+        (set_hints); there is no ab / mask block ("ab" and "mask" are None)."""
         HW = self.H * self.W
+        if hints:
+            n_in = n * HW + (n * 316 if glob else 0)
+            sizes = (n_in * 4, n * 2 * HW * 4 + n * 3 * HW + n * 2 * HW * 8)
+            blocks = [self._host_block(nbytes) for nbytes in sizes]
+            fin = blocks[0].view(np.float32)
+            b_ab, b_rgb = n * 2 * HW * 4, n * 3 * HW
+            return {"L_mc": fin[:n * HW].reshape(n, 1, self.H, self.W), "ab": None, "mask": None,
+                    "glob": fin[n * HW:].reshape(n, 316) if glob else None,
+                    "out_ab": blocks[1][:b_ab].view(np.float32).reshape(n, 2, self.H, self.W),
+                    "out_rgb": blocks[1][b_ab:b_ab + b_rgb].reshape(n, self.H, self.W, 3),
+                    "out_abq": blocks[1][b_ab + b_rgb:].view(np.float64).reshape(n, 2, self.H, self.W)}
         n_in = n * 4 * HW + (n * 316 if glob else 0)
         b_ab, b_rgb, b_q = n * 2 * HW * 4, n * 3 * HW, n * 2 * HW * 8
         sizes = (n_in * 4, b_ab + b_rgb + b_q)
@@ -178,6 +217,13 @@ class LhnContext(object):
                "out_rgb": blocks[1][b_ab:b_ab + b_rgb].reshape(n, self.H, self.W, 3),
                "out_abq": blocks[1][b_ab + b_rgb:].view(np.float64).reshape(n, 2, self.H, self.W)}
         return out
+
+    def _host_block(self, nbytes):
+        p = self.lib.idc_host_alloc(nbytes)
+        if not p:
+            raise _lib.IdcError(-2, "idc_host_alloc(%d) failed" % nbytes)
+        self._pinned.append(p)
+        return np.frombuffer((ctypes.c_char * nbytes).from_address(p), dtype=np.uint8)
 
     def set_dist_resident(self, on=True):
         """Interactive mode: the dist head runs on every forward_host but stays on the device."""

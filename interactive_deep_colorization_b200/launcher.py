@@ -13,11 +13,15 @@ Per-click colour suggestions: the reference commented out `self.predict_color()`
 `enable_per_click_suggestions()` re-enables exactly those two calls by wrapping `GUIDraw.update_ui` (its return value
 `is_predict` is true precisely where the commented-out lines sit).  `use_gpu_display()` swaps the per-click display
 step of `compute_result` (:280-283: cv2 cubic resize + lab2rgb, ~10 ms of numpy) for the fused GPU kernel.
+`use_device_hints()` hands the user edits to the models as a rectangle list (rasterised on the device) instead of
+painting and converting a whole image per call, and `use_gpu_gamut()` computes the gamut map on the device.
 """
 from __future__ import print_function
 
 import argparse
 import sys
+
+import numpy as np
 
 BACKENDS = ("b200", "b200-caffe")
 
@@ -112,6 +116,101 @@ def use_gpu_display(gui_draw_cls, update_signal=None):
     return gui_draw_cls
 
 
+def gui_hint_list(ui_control):
+    """The hint list `ui_control.get_input()` would paint (ui/ui_control.py:177-187): one rectangle per user edit, in
+    paint order, each from that edit's own scale_point / width / scale exactly as PointEdit.updateInput places its
+    filled cv2.rectangle (:52-63), with the ab of its colour.  Each distinct colour is converted once, all in one
+    color.rgb2lab batch, instead of the whole painted image."""
+    from . import color
+    from .colorize_image import HINT_LIST_DTYPE
+    edits = list(ui_control.userEdits)
+    rects = np.zeros(len(edits), HINT_LIST_DTYPE)
+    rgb = np.zeros((len(edits), 3), np.uint8)
+    for i, ue in enumerate(edits):
+        w = int(ue.width / ue.scale)
+        xa, ya = ue.scale_point(ue.pnt.x(), ue.pnt.y(), -w)
+        xb, yb = ue.scale_point(ue.pnt.x(), ue.pnt.y(), w)
+        rects[i] = (0, min(ya, yb), min(xa, xb), max(ya, yb), max(xa, xb), 0.0, 0.0)   # cv2 orders the corners
+        rgb[i] = (ue.color.red(), ue.color.green(), ue.color.blue())
+    if len(edits):
+        uniq, inv = np.unique(rgb, axis=0, return_inverse=True)
+        lab = color.rgb2lab(uniq[np.newaxis])[0]
+        rects["a"], rects["b"] = lab[inv.reshape(-1), 1], lab[inv.reshape(-1), 2]
+    return rects
+
+
+class _LazyGuiPlanes(object):
+    """`im_ab0` / `im_mask0` of GUIDraw after a hint-list forward: what the dense statements would have stored (ab of
+    the painted image, mask > 0), read from the model's lazily rasterised input planes when save_result asks."""
+
+    def __init__(self, name):
+        self.name = name
+
+    def __get__(self, obj, cls=None):
+        if obj is None:
+            return self
+        d = obj.__dict__
+        if self.name not in d:
+            model = d.get("_b200_hint_model")
+            if model is None:
+                raise AttributeError(self.name)
+            d[self.name] = model.input_ab if self.name == "im_ab0" else model.input_mask > 0
+        return d[self.name]
+
+    def __set__(self, obj, value):
+        obj.__dict__[self.name] = value
+
+
+def use_device_hints(gui_draw_cls, update_signal=None, gpu_display=True):
+    """Replace the `get_input()` + `rgb2lab` statements of `compute_result` / `predict_color` (ui/gui_draw.py:250-258,
+    :272-279): the models get the user edits as a hint list (net_forward_hints), which the click graph rasterises on the
+    device.  The display step is `prepost.display_rgb_gpu` (gpu_display) or the reference's host statements
+    (:280-283).  `self.im_ab0` / `self.im_mask0` stay readable for save_result; they are computed when read."""
+    from . import color, prepost
+
+    def _hint_forward(self, model):
+        for k in ("im_ab0", "im_mask0"):
+            self.__dict__.pop(k, None)
+        model.net_forward_hints(gui_hint_list(self.uiControl))
+        self.__dict__["_b200_hint_model"] = model
+
+    def compute_result(self):
+        _hint_forward(self, self.model)
+        if gpu_display:
+            self.result = prepost.display_rgb_gpu(np.asarray(self.model.output_ab), self.l_win, self.model._device())
+        else:
+            import cv2
+            ab_win = cv2.resize(self.model.output_ab.transpose((1, 2, 0)), (self.win_w, self.win_h),
+                                interpolation=cv2.INTER_CUBIC)
+            pred_lab = np.concatenate((self.l_win[..., np.newaxis], ab_win), axis=2)
+            self.result = (np.clip(color.lab2rgb(pred_lab), 0, 1) * 255).astype('uint8')
+        if update_signal is not None:
+            update_signal(self, self.result)
+        self.update()
+
+    def predict_color(self):
+        if self.dist_model is not None and self.image_loaded:
+            _hint_forward(self, self.dist_model)
+
+    gui_draw_cls.compute_result = compute_result
+    gui_draw_cls.predict_color = predict_color
+    gui_draw_cls.im_ab0 = _LazyGuiPlanes("im_ab0")
+    gui_draw_cls.im_mask0 = _LazyGuiPlanes("im_mask0")
+    return gui_draw_cls
+
+
+def use_gpu_gamut(lab_gamut_module, device=0):
+    """Patch `abGrid.update_gamut` (data/lab_gamut.py:66-78, run on every colour change by ui/gui_gamut.py:17-20) with
+    the device kernel (prepost.gamut_gpu): same (masked_rgb, mask), also stored on the grid object."""
+    from . import prepost
+
+    def update_gamut(self, l_in):
+        self.masked_rgb, self.mask = prepost.gamut_gpu(l_in, self.gamut_size, self.D, device)
+        return self.masked_rgb, self.mask
+    lab_gamut_module.abGrid.update_gamut = update_gamut
+    return lab_gamut_module
+
+
 def main(argv=None):
     args = parse_args(argv)
     for arg in vars(args):
@@ -137,6 +236,10 @@ def main(argv=None):
         enable_per_click_suggestions(gui_draw.GUIDraw)
     if not args.host_display:
         use_gpu_display(gui_draw.GUIDraw, emit)
+    # hints as rectangle lists rasterised on the device, and the gamut map on the device (both replace per-click numpy)
+    use_device_hints(gui_draw.GUIDraw, emit, gpu_display=not args.host_display)
+    from data import lab_gamut
+    use_gpu_gamut(lab_gamut, args.gpu)
     app = QApplication(sys.argv)
     window = gui_design.GUIDesign(color_model=colorModel, dist_model=distModel, img_file=args.image_file,
                                   load_size=args.load_size, win_size=args.win_size)

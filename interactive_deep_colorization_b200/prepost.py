@@ -143,6 +143,20 @@ def fullres_rgb_gpu(ab, l_fullres, device=0):
     return d_rgb.cpu().numpy()
 
 
+def gamut_gpu(L, gamut_size=110, D=1, device=0):
+    """The GUI's gamut map on the device: `abGrid(gamut_size, D).update_gamut(L)` (data/lab_gamut.py:66-78) ->
+    (masked_rgb uint8 [A,B,3], mask bool [A,B]); row <-> a, column <-> b (include/idc_b200.h: idc_gamut_ab)."""
+    torch = _torch()
+    A = len(np.arange(-gamut_size, gamut_size + D, D))
+    d_rgb = torch.empty((A, A, 3), dtype=torch.uint8, device="cuda:%d" % device)
+    d_mask = torch.empty((A, A), dtype=torch.uint8, device=d_rgb.device)
+    rc = _lib.load().idc_gamut_ab(device, float(L), int(gamut_size), int(D), d_rgb.data_ptr(), d_mask.data_ptr(),
+                                  torch.cuda.current_stream(d_rgb.device).cuda_stream)
+    if rc != _lib.IDC_OK:
+        raise _lib.IdcError(rc, "idc_gamut_ab failed")
+    return d_rgb.cpu().numpy(), d_mask.cpu().numpy().astype(bool)
+
+
 def pts_in_hull():
     """The 313 in-gamut ab bin centres (data fixture of the reference: data/color_bins/pts_in_hull.npy)."""
     import os

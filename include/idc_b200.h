@@ -212,9 +212,24 @@ int idc_ab_reccs_pmf(int device, const float* pmf_host, int K, int max_iter, int
  *                            -> softmax(T * logits) -> annealed mean over the 313 bin centres = pred_ab [n,2,h,w]
  *                            (DEVICE pointer; T = 2.6 in the reference, :827-848).
  *   idc_caffe313_dist_pixel: dist_ab_S[:, y, x] = softmax(S * upsampled logits) at ONE full-resolution
- *                            pixel (S = 0.2, :808-820) -> 313 floats in HOST memory. */
+ *                            pixel (S = 0.2, :808-820) -> 313 floats in HOST memory.
+ *   idc_caffe313_dist_map:   the whole dist_ab_S blob (`self.net.blobs['dist_ab_S'].data`, data/colorize_image.py:499)
+ *                            -> out_dist [n,313,h,w] DEVICE memory, asynchronous on `stream`.  Every pixel equals
+ *                            idc_caffe313_dist_pixel bit for bit.  IDC_ERR_ARG for n outside [1, max_n] or NULL,
+ *                            IDC_ERR_STATE without IDC_FLAG_CAFFE313. */
 int idc_caffe313_pred_ab(idc_ctx* ctx, int n, float T, float* out_ab, void* stream);
 int idc_caffe313_dist_pixel(idc_ctx* ctx, int img, int y, int x, float S, float* out313_host);
+int idc_caffe313_dist_map(idc_ctx* ctx, int n, float S, float* out_dist, void* stream);
+
+/* Distribution entropy (`compute_entropy`, data/colorize_image.py:356-358 and :545-547:
+ * `np.sum(dist_ab * np.log(dist_ab), axis=0)`, the NEGATIVE entropy): out[i, p] = sum_k dist[i, k, p] * logf(dist[i, k, p])
+ * in float32, bins summed in order 0 .. bins-1 like numpy's axis-0 sum; a zero bin gives NaN, as in numpy.
+ *   idc_negentropy:       dist [n,bins,hw] -> out [n,hw], DEVICE ptrs, asynchronous on `stream` (also serves an
+ *                         out_dist of idc_forward or of idc_caffe313_dist_map).
+ *   idc_dist_negentropy:  the resident 529-bin distribution of image img (idc_set_dist_resident) -> out [h/4, w/4]
+ *                         HOST memory; IDC_ERR_STATE when no resident distribution holds image img. */
+int idc_negentropy(int device, int n, int bins, int hw, const float* dist, float* out, void* stream);
+int idc_dist_negentropy(idc_ctx* ctx, int img, float* out_host);
 
 /* Stand-alone post-process: lab2rgb_transpose (data/colorize_image.py:20-28).
  * L [n,1,h,w] in [0,100] (NOT mean-centred), ab [n,2,h,w] -> rgb [n,h,w,3] uint8. DEVICE ptrs. */

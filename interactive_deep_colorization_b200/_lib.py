@@ -56,6 +56,9 @@ SYMBOLS = [
     ("idc_ab_reccs_pmf", _c.c_int, [_c.c_int, _P, _c.c_int, _c.c_int, _c.c_int, _P, _P, _P, _P]),
     ("idc_caffe313_pred_ab", _c.c_int, [_P, _c.c_int, _c.c_float, _P, _P]),
     ("idc_caffe313_dist_pixel", _c.c_int, [_P, _c.c_int, _c.c_int, _c.c_int, _c.c_float, _P]),
+    ("idc_caffe313_dist_map", _c.c_int, [_P, _c.c_int, _c.c_float, _P, _P]),
+    ("idc_negentropy", _c.c_int, [_c.c_int, _c.c_int, _c.c_int, _c.c_int, _P, _P, _P]),
+    ("idc_dist_negentropy", _c.c_int, [_P, _c.c_int, _P]),
     ("idc_lab2rgb_u8", _c.c_int, [_c.c_int, _c.c_int, _c.c_int, _c.c_int, _P, _P, _P, _P]),
     ("idc_rgb2lab_f64", _c.c_int, [_c.c_int, _c.c_int, _c.c_int, _c.c_int, _P, _P, _P]),
     ("idc_global_stats", _c.c_int, [_c.c_int, _c.c_int, _c.c_int, _P, _P, _P, _P]),

@@ -8,7 +8,8 @@ GUI (`ui/gui_draw.py:109-113,258-286`) and the notebooks work unchanged:
     ColorizeImageB200Dist  <-> ColorizeImageTorchDist  (:279-372)
     ColorizeImageB200GlobDist <-> ColorizeImageCaffeGlobDist (:445-463) semantics on the torch scaling
 
-Differences, all deliberate: no matplotlib / scikit-image imports (colour math in .color);
+Differences, all deliberate: no scikit-image import (colour math in .color) and matplotlib only inside the
+plot_dist_* methods;
 `prep_net` also accepts an in-memory `state_dict`; the network forward, the 529-bin softmax
 and the Lab->RGB post-process run in libidc_b200.so.  There is no CPU fallback.
 """
@@ -458,8 +459,9 @@ class _LazyUpsampledDist(object):
     (`fetch` pulls 529 floats per lookup) or is a host [529, X/4, X/4] array; either way it is
     replicated on read."""
 
-    def __init__(self, d64=None, fetch=None, shape64=None):
-        self.d64, self._fetch = d64, fetch
+    def __init__(self, d64=None, fetch=None, shape64=None, negentropy=None):
+        """negentropy: callable -> [X/4, X/4] sum_k d log d of the device-resident plane (compute_entropy)."""
+        self.d64, self._fetch, self._negentropy = d64, fetch, negentropy
         s = d64.shape if d64 is not None else shape64
         self.shape = (s[0], s[1] * 4, s[2] * 4)
         self.dtype = np.dtype(np.float32)
@@ -481,7 +483,53 @@ class _LazyUpsampledDist(object):
         return a.astype(dtype) if dtype is not None else a
 
 
-class ColorizeImageB200Dist(ColorizeImageB200):
+class _LazyDistFull(object):
+    """`dist_ab_full` [AB, X, X] or `dist_ab_grid` [A, B, X, X] (float64, zero outside `in_hull`; reference :312-317)
+    over a lazy `dist_ab`.  Indexing one pixel (`[:, h, w]`, `[:, :, h, w]`) reads that pixel's column of `dist_ab`
+    only; np.asarray materialises the reference's float64 array."""
+
+    def __init__(self, dist, in_hull, shape):
+        self._dist, self._in_hull = dist, in_hull
+        self.shape = tuple(shape)
+        self.ndim = len(self.shape)
+        self.dtype = np.dtype(np.float64)
+
+    def __getitem__(self, idx):
+        k = self.ndim - 2
+        if isinstance(idx, tuple) and len(idx) == self.ndim and all(isinstance(i, (int, np.integer)) for i in idx[k:]):
+            h, w = range(self.shape[-2])[int(idx[k])], range(self.shape[-1])[int(idx[k + 1])]
+            col = np.zeros(self._in_hull.shape[0])
+            col[self._in_hull] = np.asarray(self._dist[:, h, w])
+            return col.reshape(self.shape[:k])[idx[:k]]
+        return self.__array__()[idx]
+
+    def __array__(self, dtype=None, copy=None):
+        full = np.zeros((self._in_hull.shape[0],) + self.shape[-2:])
+        full[self._in_hull] = np.asarray(self._dist)
+        full = full.reshape(self.shape)
+        return full.astype(dtype) if dtype is not None else full
+
+
+class _DistPlots(object):
+    """plot_dist_grid / plot_dist_entropy of both distribution models (reference :360-372, :549-561).  matplotlib is
+    imported on call, so the package imports without it."""
+
+    def plot_dist_grid(self, h, w):
+        import matplotlib.pyplot as plt
+        plt.figure()
+        plt.imshow(self.dist_ab_grid[:, :, h, w], extent=[-110, 110, 110, -110], interpolation='nearest')
+        plt.colorbar()
+        plt.ylabel('a')
+        plt.xlabel('b')
+
+    def plot_dist_entropy(self):
+        import matplotlib.pyplot as plt
+        plt.figure()
+        plt.imshow(-self.dist_entropy, interpolation='nearest')
+        plt.colorbar()
+
+
+class ColorizeImageB200Dist(_DistPlots, ColorizeImageB200):
     """<-> ColorizeImageTorchDist (reference :279-372)."""
 
     def __init__(self, Xd=256, maskcent=False, engine="wgmma", fast_fp16=False, materialize_full=False):
@@ -556,7 +604,10 @@ class ColorizeImageB200Dist(ColorizeImageB200):
             self.dist_ab_grid = self.dist_ab_full.reshape((self.A, self.B, self.Xd, self.Xd))
         else:
             self.dist_ab = _LazyUpsampledDist(fetch=lambda y4, x4: ctx.fetch_dist(0, y4, x4),
-                                              shape64=(529, Xh // 4, Xw // 4))
+                                              shape64=(529, Xh // 4, Xw // 4),
+                                              negentropy=lambda: ctx.dist_negentropy(0))
+            self.dist_ab_full = _LazyDistFull(self.dist_ab, self.in_hull, (self.AB, Xh, Xw))
+            self.dist_ab_grid = _LazyDistFull(self.dist_ab, self.in_hull, (self.A, self.B, Xh, Xw))
         self._dist_ctx = ctx
         self.dist_ab_set = True
         # reference returns the regression output scaled by 110 twice (model.py:166-168, q1)
@@ -594,6 +645,12 @@ class ColorizeImageB200Dist(ColorizeImageB200):
         return (centers, conf) if return_conf else centers
 
     def compute_entropy(self):
+        neg = getattr(self.dist_ab, "_negentropy", None)
+        if neg is not None:
+            # the resident distribution: sum_k d log d at (X/4)^2 on the device, replicated x4 like the map itself
+            # (replicated pixels have identical distributions, so this is the reference's value at every pixel)
+            self.dist_entropy = np.repeat(np.repeat(neg(), 4, axis=0), 4, axis=1)
+            return
         d = np.asarray(self.dist_ab)
         self.dist_entropy = np.sum(d * np.log(d), axis=0)
 
@@ -737,12 +794,14 @@ class ColorizeImageB200CaffeGlobDist(ColorizeImageB200Caffe):
 class _LazyDist313(object):
     """[313, X, X] view of `dist_ab_S`: one pixel (313 floats) is computed on demand from the resident 313-bin logits
     (idc_caffe313_dist_pixel); the reference materialises 313 x X x X floats per forward and reads one pixel of it per
-    click (reference :505, :521)."""
+    click (reference :505, :521).  The whole map (np.asarray, any other index) is one idc_caffe313_dist_map launch and
+    one copy to the host, kept on this view: net_forward makes a new view, so the copy lives for one forward."""
 
     def __init__(self, ctx, X, S):
         self._ctx, self._S = ctx, S
         self.shape = (313, X, X)
         self.dtype = np.dtype(np.float32)
+        self._host = self._full = None
 
     def __getitem__(self, idx):
         if isinstance(idx, tuple) and len(idx) == 3 and all(isinstance(i, (int, np.integer)) for i in idx[1:]):
@@ -750,12 +809,27 @@ class _LazyDist313(object):
         return self.__array__()[idx]
 
     def __array__(self, dtype=None, copy=None):
-        X = self.shape[1]
-        a = np.stack([np.stack([self._ctx.caffe313_dist_pixel(0, y, x, self._S) for x in range(X)], -1) for y in range(X)], -2)
-        return a.astype(dtype) if dtype is not None else a
+        if self._host is None:
+            self._host = self._ctx.caffe313_dist_map(1, self._S)[0].cpu().numpy()
+        a = self._host
+        if dtype is not None:
+            return a.astype(dtype)
+        return a.copy() if copy else a
+
+    def full(self, in_hull):
+        """dist_ab_full [529, X, X] float64 (reference :503): the cached map scattered to the in-gamut bins, once."""
+        if self._full is None:
+            self._full = np.zeros((in_hull.shape[0],) + self.shape[1:])
+            self._full[in_hull] = self.__array__()
+        return self._full
+
+    def negentropy(self):
+        """compute_entropy's sum_k d log d [X, X] float32: map and sum on the device, only [X, X] is copied back."""
+        from . import prepost
+        return prepost.negentropy_gpu(self._ctx.caffe313_dist_map(1, self._S))[0].cpu().numpy()
 
 
-class ColorizeImageB200CaffeDist(ColorizeImageB200Caffe):
+class ColorizeImageB200CaffeDist(_DistPlots, ColorizeImageB200Caffe):
     """<-> ColorizeImageCaffeDist (reference :466-561): the 313-bin distribution model.  `pred_ab` is the annealed
     mean of the 313-bin head (deploy_nopred.prototxt:827-850), `dist_ab` the S-softened distribution (:808-820)."""
     _caffe313 = True
@@ -804,9 +878,7 @@ class ColorizeImageB200CaffeDist(ColorizeImageB200Caffe):
 
     @property
     def dist_ab_full(self):
-        full = np.zeros((self.AB, self.Xd, self.Xd))
-        full[self.in_hull, :, :] = np.asarray(self.dist_ab)
-        return full
+        return self.dist_ab.full(self.in_hull)
 
     @property
     def dist_ab_grid(self):
@@ -839,5 +911,4 @@ class ColorizeImageB200CaffeDist(ColorizeImageB200Caffe):
         return (centers, conf) if return_conf else centers
 
     def compute_entropy(self):
-        d = np.asarray(self.dist_ab)
-        self.dist_entropy = np.sum(d * np.log(d), axis=0)
+        self.dist_entropy = self.dist_ab.negentropy()

@@ -1307,6 +1307,33 @@ int idc_caffe313_dist_pixel(idc_ctx* c, int img, int y, int x, float S, float* o
   return IDC_OK;
 }
 
+int idc_caffe313_dist_map(idc_ctx* c, int n, float S, float* out_dist, void* stream) {
+  if (!c || !out_dist || n < 1 || n > c->max_n) return IDC_ERR_ARG;
+  if (!c->caffe313) return fail(c, IDC_ERR_STATE, "ctx was not created with IDC_FLAG_CAFFE313");
+  CUDA_TRY(c, cudaSetDevice(c->dev));
+  CUDA_TRY(c, launch_dist313_map(c, n, S, out_dist, (cudaStream_t)stream));
+  return IDC_OK;
+}
+
+int idc_negentropy(int device, int n, int bins, int hw, const float* dist, float* out, void* stream) {
+  if (n < 1 || n > 65535 || bins < 1 || hw < 1 || !dist || !out) return IDC_ERR_ARG;
+  if (cudaSetDevice(device) != cudaSuccess) return IDC_ERR_CUDA;
+  return launch_negentropy(n, bins, hw, dist, out, (cudaStream_t)stream) == cudaSuccess ? IDC_OK : IDC_ERR_CUDA;
+}
+
+int idc_dist_negentropy(idc_ctx* c, int img, float* out_host) {
+  if (!c || !out_host) return IDC_ERR_ARG;
+  if (img < 0 || img >= c->dist_valid_n || !c->d_out)
+    return fail(c, IDC_ERR_STATE, "no resident distribution for image %d (run idc_forward_host with resident mode on)", img);
+  const size_t HW = (size_t)c->H * c->W, HW4 = (size_t)(c->H / 4) * (c->W / 4);
+  const float* d = c->d_out + (size_t)c->max_n * 2 * HW + (size_t)img * 529 * HW4;
+  CUDA_TRY(c, cudaSetDevice(c->dev));
+  if (!c->d_negent) CUDA_TRY(c, cudaMalloc(&c->d_negent, HW4 * sizeof(float)));
+  CUDA_TRY(c, launch_negentropy(1, 529, (int)HW4, d, c->d_negent, 0));
+  CUDA_TRY(c, cudaMemcpy(out_host, c->d_negent, HW4 * sizeof(float), cudaMemcpyDeviceToHost));
+  return IDC_OK;
+}
+
 int idc_lab2rgb_u8(int device, int n, int h, int w, const float* L, const float* ab, uint8_t* rgb, void* stream) {
   if (n < 1 || h < 1 || w < 1 || !L || !ab || !rgb) return IDC_ERR_ARG;
   if (cudaSetDevice(device) != cudaSuccess) return IDC_ERR_CUDA;
@@ -1481,6 +1508,7 @@ int idc_destroy(idc_ctx* c) {
   if (c->splitk_counters) cudaFree(c->splitk_counters);
   if (c->w11_umma) cudaFree(c->w11_umma);
   if (c->d_reccs) cudaFree(c->d_reccs);
+  if (c->d_negent) cudaFree(c->d_negent);
   if (c->gvec) cudaFree(c->gvec);
   if (c->gtmp) cudaFree(c->gtmp);
   if (c->h_err) cudaFreeHost(c->h_err);

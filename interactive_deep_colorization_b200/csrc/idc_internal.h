@@ -198,6 +198,7 @@ struct Ctx {
   bool gadd_active = false;     // a global-hints vector was supplied to this forward
   int last_n = 0;
   double* d_reccs = nullptr;    // idc_ab_reccs scratch (results of every restart, then the 529x2 gamut points)
+  float* d_negent = nullptr;    // idc_dist_negentropy result, (H/4)*(W/4) floats
   bool dist_resident = false;   // keep the dist of the last forward_host on the device (idc_fetch_dist)
   int dist_valid_n = 0;
   // idc_set_click: the clicked pixel's pmf + K colour suggestions ride on a side branch of the click graph
@@ -238,6 +239,8 @@ cudaError_t launch_lab2rgb(Ctx* c, int n, int h, int w, const float* L, float l_
                            uint8_t* rgb, cudaStream_t st, double* abq = nullptr);   // c may be null (stand-alone call)
 cudaError_t launch_decode313(Ctx* c, int n, float T, float* out_ab, cudaStream_t st);
 cudaError_t launch_dist313_pixel(Ctx* c, int img, int y, int x, float S, float* out313_dev, cudaStream_t st);
+cudaError_t launch_dist313_map(Ctx* c, int n, float S, float* out_dev, cudaStream_t st);
+cudaError_t launch_negentropy(int n, int bins, int hw, const float* dist, float* out, cudaStream_t st);
 cudaError_t launch_ab_reccs(const float* pmf, size_t bin_stride, const float* pts_dev, int K, int max_iter,
                             int n_init, double* out_dev, cudaStream_t st, const int* dyn = nullptr);
 cudaError_t launch_click_pmf(Ctx* c, const int* click_dev, int n_img, int* out_hdr, float* out_pmf, cudaStream_t st);

@@ -272,6 +272,22 @@ class LhnContext(object):
         _lib.check(self.h, self.lib.idc_caffe313_dist_pixel(self.h, int(img), int(y), int(x), float(S), _np_ptr(out)))
         return out
 
+    def caffe313_dist_map(self, n=1, S=0.2):
+        """The whole dist_ab_S map [n,313,H,W] (device tensor, torch's current stream) from the 313-bin logits of the
+        last forward; every pixel equals caffe313_dist_pixel bit for bit."""
+        import torch
+        out = torch.empty((n, 313, self.H, self.W), dtype=torch.float32, device="cuda:%d" % self.device)
+        st = torch.cuda.current_stream(self.device).cuda_stream
+        _lib.check(self.h, self.lib.idc_caffe313_dist_map(self.h, int(n), float(S), out.data_ptr(), st))
+        return out
+
+    def dist_negentropy(self, img=0):
+        """sum_k d * log(d) over the 529 bins of the resident distribution of image img -> [H/4, W/4] float32 (the
+        reference's compute_entropy statement before its x4 upsample); only this plane leaves the device."""
+        out = np.empty((self.H // 4, self.W // 4), np.float32)
+        _lib.check(self.h, self.lib.idc_dist_negentropy(self.h, int(img), _np_ptr(out)))
+        return out
+
     # ---- introspection (tests) -------------------------------------------------------------
     def op_names(self):
         return [self.lib.idc_op_name(self.h, i).decode() for i in range(self.lib.idc_num_ops(self.h))]

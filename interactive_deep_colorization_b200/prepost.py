@@ -157,6 +157,24 @@ def gamut_gpu(L, gamut_size=110, D=1, device=0):
     return d_rgb.cpu().numpy(), d_mask.cpu().numpy().astype(bool)
 
 
+def negentropy_gpu(dist):
+    """`np.sum(d * np.log(d), axis=0)` per image (compute_entropy, data/colorize_image.py:356-358) on the device:
+    dist is a CUDA float32 tensor [n, bins, ...] (e.g. a forward's out_dist or LhnContext.caffe313_dist_map) ->
+    device tensor [n, ...].  float32, bins summed in order, NaN where a bin is exactly 0 (include/idc_b200.h:
+    idc_negentropy)."""
+    torch = _torch()
+    assert dist.is_cuda and dist.dtype == torch.float32 and dist.dim() >= 2
+    d = dist.contiguous()
+    n, bins = d.shape[0], d.shape[1]
+    out = torch.empty((n,) + tuple(d.shape[2:]), dtype=torch.float32, device=d.device)
+    hw = out[0].numel() if n else 0
+    rc = _lib.load().idc_negentropy(d.device.index, n, bins, hw, d.data_ptr(), out.data_ptr(),
+                                    torch.cuda.current_stream(d.device).cuda_stream)
+    if rc != _lib.IDC_OK:
+        raise _lib.IdcError(rc, "idc_negentropy failed")
+    return out
+
+
 def pts_in_hull():
     """The 313 in-gamut ab bin centres (data fixture of the reference: data/color_bins/pts_in_hull.npy)."""
     import os

@@ -249,6 +249,23 @@ int idc_rgb2lab_f64(int device, int n, int h, int w, const uint8_t* rgb, double*
 int idc_global_stats(int device, int h, int w, const uint8_t* rgb, const float* pts313, float* out316, void* stream);
 int idc_zoom_lab2rgb_u8(int device, int h_in, int w_in, const double* ab, int h, int w, const double* L_full,
                         uint8_t* rgb, void* stream);
+/* f1, the full-resolution renders of the wrapper (data/colorize_image.py):
+ *   get_img_gray_fullres   (:119-121)  lab2rgb_transpose(img_l_fullres, 0)
+ *   get_input_img_fullres  (:133-136)  lab2rgb_transpose(img_l_fullres, zoom(input_ab, order=1))
+ *   get_img_mask_fullres   (:145-149)  lab2rgb_transpose(100. * (1 - zoom(input_mask, order=0)), 0)
+ *   get_sup_fullres        (:154-158)  lab2rgb_transpose(50 * zoom(input_mask, order=0), zoom(input_ab, order=0))
+ * -> uint8 rgb [h,w,3].  ab [2,h_in,w_in] (NULL: ab = 0) is zoomed to [h,w] with ab_order 0 or 1 exactly as
+ * scipy.ndimage.zoom (1.18) does it, mode 'constant': a sample whose coordinate o * ((n_in-1)/(n_out-1)) lies past the
+ * last input reads 0.  ab_f32 = 1 rounds the zoomed ab to float32 (scipy's result for a float32 plane).  L is
+ *   IDC_RENDER_L_PLANE  the plane L [h,w]
+ *   IDC_RENDER_L_MASK   100 * (1 - m)        m = mask [h_in,w_in] zoomed with order 0 (the same edge rule)
+ *   IDC_RENDER_L_SUP    50 * m
+ * with mask_f32 = 1 evaluating those statements in float32 (numpy's result for a float32 mask).  float64 otherwise.
+ * DEVICE ptrs, asynchronous on `stream`.  IDC_ERR_ARG, before any device call, for h, w, h_in, w_in < 1, ab_order,
+ * ab_f32 or mask_f32 outside {0, 1}, an unknown l_mode or a NULL plane that l_mode reads, and a NULL rgb. */
+enum { IDC_RENDER_L_PLANE = 0, IDC_RENDER_L_MASK = 1, IDC_RENDER_L_SUP = 2 };
+int idc_render_planes_u8(int device, int h_in, int w_in, const double* ab, int ab_order, int ab_f32, const double* mask,
+                         int mask_f32, int l_mode, const double* L, int h, int w, uint8_t* rgb, void* stream);
 
 /* f1, image-load side (data/colorize_image.py:52-66): cv2.resize(im, (w_dst, h_dst)) of a uint8 [h,w,3] image with
  * OpenCV's default INTER_LINEAR -- the 8-bit path of OpenCV is fixed-point arithmetic and is restated integer for

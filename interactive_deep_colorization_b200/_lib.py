@@ -24,6 +24,7 @@ FLAG_KEEP_CONV10 = 1 << 5
 FLAG_CAFFE313 = 1 << 6
 F32, F64, I64 = 0, 1, 2
 MAX_HINTS = 1024                      # IDC_MAX_HINTS
+RENDER_L_PLANE, RENDER_L_MASK, RENDER_L_SUP = 0, 1, 2     # idc_render_planes_u8 l_mode
 # idc_hint: inclusive pixel rectangle of image `img` painted with one ab colour (28 bytes, no padding)
 HINT_DTYPE = np.dtype([("img", "<i4"), ("y0", "<i4"), ("x0", "<i4"), ("y1", "<i4"), ("x1", "<i4"),
                        ("a", "<f4"), ("b", "<f4")])
@@ -63,6 +64,8 @@ SYMBOLS = [
     ("idc_rgb2lab_f64", _c.c_int, [_c.c_int, _c.c_int, _c.c_int, _c.c_int, _P, _P, _P]),
     ("idc_global_stats", _c.c_int, [_c.c_int, _c.c_int, _c.c_int, _P, _P, _P, _P]),
     ("idc_zoom_lab2rgb_u8", _c.c_int, [_c.c_int, _c.c_int, _c.c_int, _P, _c.c_int, _c.c_int, _P, _P, _P]),
+    ("idc_render_planes_u8", _c.c_int, [_c.c_int, _c.c_int, _c.c_int, _P, _c.c_int, _c.c_int, _P, _c.c_int, _c.c_int,
+                                        _P, _c.c_int, _c.c_int, _P, _P]),
     ("idc_resize_u8_linear", _c.c_int, [_c.c_int, _c.c_int, _c.c_int, _P, _c.c_int, _c.c_int, _P, _P]),
     ("idc_cubic_lab2rgb_u8", _c.c_int, [_c.c_int, _c.c_int, _c.c_int, _P, _c.c_int, _c.c_int, _P, _P, _P]),
     ("idc_get_activation", _c.c_int, [_P, _c.c_char_p, _P, _c.c_size_t, _c.POINTER(_c.c_int),

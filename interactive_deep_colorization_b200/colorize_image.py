@@ -451,6 +451,51 @@ class ColorizeImageB200(ColorizeImageBase):
         from . import prepost
         return prepost.fullres_rgb_gpu(self.output_ab, self.img_l_fullres, self._device())
 
+    # ----- row f1, the other full-resolution renders (reference :119-158) on the GPU under the same gate -----
+    def _device_render(self, *planes):
+        """float32 / float64 planes of three dimensions render on the device; anything else (a bool GUI mask, integer
+        planes) takes the ColorizeImageBase statements, which then raise or convert exactly as they always did."""
+        return self.gpu_prepost and self.net_set and all(
+            getattr(p, "dtype", None) in (np.float32, np.float64) and getattr(p, "ndim", 0) == 3 for p in planes)
+
+    def _fullres_hw(self, plane, like):
+        """(h, w) of `_to_fullres(plane, like, order)`: scipy's int(round(n * factor)) per axis."""
+        H, W = self.img_l_fullres.shape[1:]
+        return (int(round(plane.shape[1] * (1. * H / like.shape[1]))), int(round(plane.shape[2] * (1. * W / like.shape[2]))))
+
+    def get_img_gray_fullres(self):
+        L = self.img_l_fullres
+        if not self._device_render(L) or L.shape[0] != 1:
+            return ColorizeImageBase.get_img_gray_fullres(self)
+        from . import prepost
+        return prepost.render_planes_gpu(L.shape[1], L.shape[2], L=L, device=self._device())
+
+    def get_input_img_fullres(self):
+        L, ab = self.img_l_fullres, self.input_ab
+        if not self._device_render(L, ab) or L.shape[0] != 1 or ab.shape[0] != 2 or \
+                self._fullres_hw(ab, ab) != tuple(L.shape[1:]):
+            return ColorizeImageBase.get_input_img_fullres(self)
+        from . import prepost
+        return prepost.render_planes_gpu(L.shape[1], L.shape[2], ab=ab, ab_order=1, L=L, device=self._device())
+
+    def get_img_mask_fullres(self):
+        mask, like = self.input_mask, self.input_ab
+        if not self._device_render(mask, like) or mask.shape[0] != 1:
+            return ColorizeImageBase.get_img_mask_fullres(self)
+        from . import _lib, prepost
+        h, w = self._fullres_hw(mask, like)
+        return prepost.render_planes_gpu(h, w, mask=mask, l_mode=_lib.RENDER_L_MASK, device=self._device())
+
+    def get_sup_fullres(self):
+        mask, ab, like = self.input_mask, self.input_ab, self.output_ab
+        if not self._device_render(mask, ab, like) or mask.shape[0] != 1 or ab.shape[0] != 2 or \
+                mask.shape[1:] != ab.shape[1:]:
+            return ColorizeImageBase.get_sup_fullres(self)
+        from . import _lib, prepost
+        h, w = self._fullres_hw(mask, like)
+        return prepost.render_planes_gpu(h, w, ab=ab, ab_order=0, mask=mask, l_mode=_lib.RENDER_L_SUP,
+                                         device=self._device())
+
 
 class _LazyUpsampledDist(object):
     """[529, X, X] view of the [529, X/4, X/4] distribution.  The reference materialises the nearest x4

@@ -1359,6 +1359,18 @@ int idc_zoom_lab2rgb_u8(int device, int h_in, int w_in, const double* ab, int h,
   return launch_zoom_lab2rgb(ab, h_in, w_in, L_full, h, w, rgb, (cudaStream_t)stream) == cudaSuccess ? IDC_OK : IDC_ERR_CUDA;
 }
 
+int idc_render_planes_u8(int device, int h_in, int w_in, const double* ab, int ab_order, int ab_f32, const double* mask,
+                         int mask_f32, int l_mode, const double* L, int h, int w, uint8_t* rgb, void* stream) {
+  if (h_in < 1 || w_in < 1 || h < 1 || w < 1 || !rgb) return IDC_ERR_ARG;
+  if ((ab_order != 0 && ab_order != 1) || (ab_f32 != 0 && ab_f32 != 1) || (mask_f32 != 0 && mask_f32 != 1)) return IDC_ERR_ARG;
+  if (l_mode == IDC_RENDER_L_PLANE ? !L : (l_mode == IDC_RENDER_L_MASK || l_mode == IDC_RENDER_L_SUP) ? !mask : true)
+    return IDC_ERR_ARG;
+  if ((size_t)h * w > (size_t)0x7fffffff * 256) return IDC_ERR_ARG;      // grid.x limit at 256 threads per block
+  if (cudaSetDevice(device) != cudaSuccess) return IDC_ERR_CUDA;
+  return launch_render_planes(ab, ab_order, ab_f32, mask, mask_f32, l_mode, L, h_in, w_in, h, w, rgb,
+                              (cudaStream_t)stream) == cudaSuccess ? IDC_OK : IDC_ERR_CUDA;
+}
+
 int idc_resize_u8_linear(int device, int h_src, int w_src, const uint8_t* src, int h_dst, int w_dst, uint8_t* dst, void* stream) {
   if (h_src < 1 || w_src < 1 || h_dst < 1 || w_dst < 1 || !src || !dst) return IDC_ERR_ARG;
   if (cudaSetDevice(device) != cudaSuccess) return IDC_ERR_CUDA;

@@ -248,6 +248,8 @@ cudaError_t launch_global_stats(int h, int w, const uint8_t* rgb, const float* p
 cudaError_t launch_rgb2lab(int n, int h, int w, const uint8_t* rgb, double* lab, cudaStream_t st);
 cudaError_t launch_zoom_lab2rgb(const double* ab, int hin, int win, const double* Lfull, int H, int W, uint8_t* rgb,
                                 cudaStream_t st);
+cudaError_t launch_render_planes(const double* ab, int ab_order, int ab_f32, const double* mask, int mask_f32, int l_mode,
+                                 const double* L, int hin, int win, int H, int W, uint8_t* rgb, cudaStream_t st);
 cudaError_t launch_resize_linear_u8(const uint8_t* src, int hs, int ws, uint8_t* dst, int hd, int wd, cudaStream_t st);
 cudaError_t launch_cubic_lab2rgb(const double* ab, int hin, int win, const double* L, int H, int W, uint8_t* rgb,
                                  cudaStream_t st);

@@ -2,6 +2,7 @@
 
     rgb2lab_gpu        skimage color.rgb2lab on uint8 RGB  (reference data/colorize_image.py:31-36,172-178,196-198)
     fullres_rgb_gpu    get_img_fullres (:123-131): scipy zoom(order=1) of ab + Lab->RGB at full resolution
+    render_planes_gpu  the grey, input, mask and supervision renders at full resolution (:119-158)
 
 float64 arithmetic on the device, like the reference's numpy path.  torch supplies device memory only.
 """
@@ -140,6 +141,41 @@ def fullres_rgb_gpu(ab, l_fullres, device=0):
                                          d_rgb.data_ptr(), st)
     if rc != _lib.IDC_OK:
         raise _lib.IdcError(rc, "idc_zoom_lab2rgb_u8 failed")
+    return d_rgb.cpu().numpy()
+
+
+def render_planes_gpu(h, w, ab=None, ab_order=1, mask=None, l_mode=_lib.RENDER_L_PLANE, L=None, device=0):
+    """The full-resolution renders (get_img_gray_fullres, get_input_img_fullres, get_img_mask_fullres, get_sup_fullres,
+    data/colorize_image.py:119-158) -> uint8 [h,w,3]; include/idc_b200.h: idc_render_planes_u8.
+    ab [2,h_in,w_in] float32 / float64 or None (ab = 0), zoomed to [h,w] with ab_order as scipy.ndimage.zoom does;
+    mask [1,h_in,w_in] (or [h_in,w_in]) float32 / float64, zoomed with order 0, for l_mode RENDER_L_MASK / RENDER_L_SUP;
+    L [1,h,w] (or [h,w]) float64 numpy or DeviceLab for RENDER_L_PLANE (a DeviceLab plane never leaves the device).
+    A float32 plane gives scipy's / numpy's float32 results, as the host statements would."""
+    torch = _torch()
+    dev = torch.device("cuda:%d" % device)
+    planes = [p for p in (ab, mask) if p is not None]
+    h_in, w_in = planes[0].shape[-2:] if planes else (h, w)
+    d_ab = d_mask = d_L = None
+    ab_f32 = mask_f32 = 0
+    if ab is not None:
+        ab_f32 = int(ab.dtype == np.float32)
+        d_ab = torch.from_numpy(np.ascontiguousarray(ab, dtype=np.float64).reshape(2, h_in, w_in)).to(dev)
+    if mask is not None:
+        mask_f32 = int(mask.dtype == np.float32)
+        d_mask = torch.from_numpy(np.ascontiguousarray(mask, dtype=np.float64).reshape(h_in, w_in)).to(dev)
+    if L is not None:
+        if isinstance(L, DeviceLab):
+            d_L = L.device_plane(0).contiguous()
+        else:
+            d_L = torch.from_numpy(np.ascontiguousarray(np.asarray(L, dtype=np.float64).reshape(h, w))).to(dev)
+        assert tuple(d_L.shape) == (h, w), (tuple(d_L.shape), h, w)
+    ptr = lambda t: None if t is None else t.data_ptr()
+    d_rgb = torch.empty((h, w, 3), dtype=torch.uint8, device=dev)
+    rc = _lib.load().idc_render_planes_u8(device, int(h_in), int(w_in), ptr(d_ab), int(ab_order), ab_f32, ptr(d_mask),
+                                          mask_f32, int(l_mode), ptr(d_L), int(h), int(w), d_rgb.data_ptr(),
+                                          torch.cuda.current_stream(dev).cuda_stream)
+    if rc != _lib.IDC_OK:
+        raise _lib.IdcError(rc, "idc_render_planes_u8 failed")
     return d_rgb.cpu().numpy()
 
 

@@ -238,15 +238,17 @@ int idc_lab2rgb_u8(int device, int n, int h, int w, const float* L, const float*
 
 /* f1 (steps either side of the network), float64 like the reference's numpy/skimage/scipy path; DEVICE ptrs.
  * idc_rgb2lab_f64:      skimage color.rgb2lab of uint8 RGB [n,h,w,3] -> Lab planes [n,3,h,w] float64
- *                       (data/colorize_image.py:31-36, :172-178 image prep, :196-198 _set_out_ab_).
- * idc_zoom_lab2rgb_u8:  get_img_fullres (:123-131): scipy.ndimage.zoom(order=1) of ab [2,h_in,w_in] to
- *                       [h,w], then lab2rgb_transpose with the full-resolution L [h,w] -> uint8 [h,w,3]. */
+ *                       (data/colorize_image.py:31-36, :172-178 image prep, :196-198 _set_out_ab_). */
 int idc_rgb2lab_f64(int device, int n, int h, int w, const uint8_t* rgb, double* lab, void* stream);
 /* f3: global statistics of a reference image (models/global_model/global_stats.prototxt:1-244; NNEncLayer with
  * NN=1, caffe_files/caffe_traininglayers.py:161-196; usage DemoGlobalHistogramTransfer.ipynb:176-182):
  * uint8 RGB [h,w,3] (h,w multiples of 4) + the 313 ab bin centres [313,2] -> out[316] =
  * [313-bin histogram of the 4x4-pooled ab, 1, mean HSV saturation, 1] = the `glob` input of idc_forward. DEVICE ptrs. */
 int idc_global_stats(int device, int h, int w, const uint8_t* rgb, const float* pts313, float* out316, void* stream);
+/* f1, get_img_fullres (:123-131): scipy.ndimage.zoom(order=1) of ab [2,h_in,w_in] float64 to [h,w], then
+ * lab2rgb_transpose with the full-resolution L [h,w] -> uint8 [h,w,3].  The same call as
+ * idc_render_planes_u8(device, h_in, w_in, ab, 1, 0, NULL, 0, IDC_RENDER_L_PLANE, L_full, h, w, rgb, stream), so the
+ * zoom follows scipy's edge rule below; IDC_ERR_ARG also for a NULL ab. */
 int idc_zoom_lab2rgb_u8(int device, int h_in, int w_in, const double* ab, int h, int w, const double* L_full,
                         uint8_t* rgb, void* stream);
 /* f1, the full-resolution renders of the wrapper (data/colorize_image.py):
@@ -273,7 +275,9 @@ int idc_render_planes_u8(int device, int h_in, int w_in, const double* ab, int a
 int idc_resize_u8_linear(int device, int h_src, int w_src, const uint8_t* src, int h_dst, int w_dst, uint8_t* dst,
                          void* stream);
 /* f1, GUI display step (ui/gui_draw.py:280-283): cv2.resize(ab [2,h_in,w_in] float64, (w,h), INTER_CUBIC), concatenated
- * with the window-size L [h,w] float64, skimage lab2rgb, clip, x255, truncating cast -> uint8 [h,w,3].  DEVICE ptrs. */
+ * with the window-size L [h,w] float64, skimage lab2rgb, clip, x255, truncating cast -> uint8 [h,w,3].  The resize
+ * evaluates OpenCV's float32 weights and float64 tap sums in OpenCV's order, so the resized ab equals cv2's bit for
+ * bit.  DEVICE ptrs. */
 int idc_cubic_lab2rgb_u8(int device, int h_in, int w_in, const double* ab, int h, int w, const double* L, uint8_t* rgb,
                          void* stream);
 /* The GUI's gamut map (data/lab_gamut.py:66-78, abGrid(gamut_size, D).update_gamut(L), called on every colour change

@@ -1354,9 +1354,8 @@ int idc_rgb2lab_f64(int device, int n, int h, int w, const uint8_t* rgb, double*
 
 int idc_zoom_lab2rgb_u8(int device, int h_in, int w_in, const double* ab, int h, int w, const double* L_full,
                         uint8_t* rgb, void* stream) {
-  if (h_in < 1 || w_in < 1 || h < 1 || w < 1 || !ab || !L_full || !rgb) return IDC_ERR_ARG;
-  if (cudaSetDevice(device) != cudaSuccess) return IDC_ERR_CUDA;
-  return launch_zoom_lab2rgb(ab, h_in, w_in, L_full, h, w, rgb, (cudaStream_t)stream) == cudaSuccess ? IDC_OK : IDC_ERR_CUDA;
+  if (!ab) return IDC_ERR_ARG;
+  return idc_render_planes_u8(device, h_in, w_in, ab, 1, 0, nullptr, 0, IDC_RENDER_L_PLANE, L_full, h, w, rgb, stream);
 }
 
 int idc_render_planes_u8(int device, int h_in, int w_in, const double* ab, int ab_order, int ab_f32, const double* mask,

@@ -246,8 +246,6 @@ cudaError_t launch_ab_reccs(const float* pmf, size_t bin_stride, const float* pt
 cudaError_t launch_click_pmf(Ctx* c, const int* click_dev, int n_img, int* out_hdr, float* out_pmf, cudaStream_t st);
 cudaError_t launch_global_stats(int h, int w, const uint8_t* rgb, const float* pts, float* out316, cudaStream_t st);
 cudaError_t launch_rgb2lab(int n, int h, int w, const uint8_t* rgb, double* lab, cudaStream_t st);
-cudaError_t launch_zoom_lab2rgb(const double* ab, int hin, int win, const double* Lfull, int H, int W, uint8_t* rgb,
-                                cudaStream_t st);
 cudaError_t launch_render_planes(const double* ab, int ab_order, int ab_f32, const double* mask, int mask_f32, int l_mode,
                                  const double* L, int hin, int win, int H, int W, uint8_t* rgb, cudaStream_t st);
 cudaError_t launch_resize_linear_u8(const uint8_t* src, int hs, int ws, uint8_t* dst, int hd, int wd, cudaStream_t st);
@@ -270,6 +268,30 @@ inline bool pdl_take(Ctx* c) {
 inline void pdl_break(Ctx* c) { if (c) c->chain = false; }
 
 #ifdef __CUDACC__
+// Lab -> sRGB uint8, float64 math like the reference's numpy/skimage path: skimage 0.13 color.lab2rgb (lab2xyz +
+// xyz2rgb), clip, *255, truncating cast (data/colorize_image.py:27).  Every render and the display step end here.
+__device__ __forceinline__ double lab_finv(double t) {
+  return t > 0.2068966 ? t * t * t : (t - 16.0 / 116.0) / 7.787;
+}
+__device__ __forceinline__ double srgb_gamma(double c) {
+  return c > 0.0031308 ? 1.055 * pow(c, 1.0 / 2.4) - 0.055 : 12.92 * c;
+}
+__device__ __forceinline__ void lab_to_rgb_u8(double l, double a, double b, uint8_t* out) {
+  const double fy = (l + 16.0) / 116.0;
+  const double fx = a / 500.0 + fy;
+  double fz = fy - b / 200.0;
+  if (fz < 0.0) fz = 0.0;
+  const double X = lab_finv(fx) * 0.95047, Y = lab_finv(fy) * 1.0, Z = lab_finv(fz) * 1.08883;
+  // inverse of the sRGB->XYZ matrix used by skimage (xyz_from_rgb), float64
+  double R = 3.240481343200526 * X + -1.5371515162713185 * Y + -0.4985363261688878 * Z;
+  double G = -0.9692549499965682 * X + 1.8759900014898907 * Y + 0.04155592655829284 * Z;
+  double B = 0.05564663913517716 * X + -0.20404133836651123 * Y + 1.0573110696453443 * Z;
+  R = srgb_gamma(R); G = srgb_gamma(G); B = srgb_gamma(B);
+  out[0] = (uint8_t)(fmin(fmax(R, 0.0), 1.0) * 255.0);
+  out[1] = (uint8_t)(fmin(fmax(G, 0.0), 1.0) * 255.0);
+  out[2] = (uint8_t)(fmin(fmax(B, 0.0), 1.0) * 255.0);
+}
+
 __device__ __forceinline__ void pdl_prologue_done() {   // small kernels: let the successor start, then wait for the predecessor
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   asm volatile("griddepcontrol.wait;" ::: "memory");

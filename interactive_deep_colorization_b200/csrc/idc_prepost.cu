@@ -6,16 +6,22 @@
 //   cubic_lab2rgb_kernel      the GUI's display step (ui/gui_draw.py:280-283): cv2.resize(ab, win, INTER_CUBIC) of the
 //                             float64 ab planes, concatenated with the window-size L, skimage lab2rgb, clip, x255,
 //                             truncating cast -- one kernel, float64 like the host path.
-// Lab <-> RGB math is shared with idc_heads.cu (same formulas, SURVEY 8c).
+// The Lab -> RGB step is lab_to_rgb_u8 (idc_internal.h), the one idc_heads.cu's renders use.
 #include "idc_internal.h"
 
 namespace idc {
+
+// OpenCV's source coordinate of output d, (float)((d + 0.5) * scale - 0.5) (modules/imgproc/src/resize.cpp), with the
+// multiply and the subtract rounded separately as on the host (nvcc would fuse them).
+__device__ __forceinline__ float cv_src_coord(int d, double scale) {
+  return __double2float_rn(__dsub_rn(__dmul_rn(__dadd_rn((double)d, 0.5), scale), 0.5));
+}
 
 // OpenCV resize, INTER_LINEAR, CV_8U (modules/imgproc/src/resize.cpp: resizeGeneric_ with HResizeLinear / VResizeLinear,
 // INTER_RESIZE_COEF_BITS = 11).  x axis: fx is zeroed when the 2-tap window leaves the image; y axis: the coefficients
 // are kept and the ROW INDICES are clipped instead.
 __device__ __forceinline__ void cv_lin_coef(int d, double scale, int ssize, bool clamp_f, int& s, int& c0, int& c1) {
-  float f = __double2float_rn(((double)d + 0.5) * scale - 0.5);
+  float f = cv_src_coord(d, scale);
   s = (int)floorf(f);
   f = __fsub_rn(f, (float)s);
   if (clamp_f) {
@@ -64,36 +70,23 @@ cudaError_t launch_resize_linear_u8(const uint8_t* src, int hs, int ws, uint8_t*
   return cudaGetLastError();
 }
 
-// ---- Lab -> sRGB uint8 (same arithmetic as idc_heads.cu: lab2rgb_kernel) ----
-__device__ __forceinline__ double pp_lab_finv(double t) { return t > 0.2068966 ? t * t * t : (t - 16.0 / 116.0) / 7.787; }
-__device__ __forceinline__ double pp_srgb_gamma(double c) { return c > 0.0031308 ? 1.055 * pow(c, 1.0 / 2.4) - 0.055 : 12.92 * c; }
-__device__ __forceinline__ void pp_lab_to_rgb_u8(double l, double a, double b, uint8_t* out) {
-  const double fy = (l + 16.0) / 116.0;
-  const double fx = a / 500.0 + fy;
-  double fz = fy - b / 200.0;
-  if (fz < 0.0) fz = 0.0;
-  const double X = pp_lab_finv(fx) * 0.95047, Y = pp_lab_finv(fy) * 1.0, Z = pp_lab_finv(fz) * 1.08883;
-  double R = 3.240481343200526 * X + -1.5371515162713185 * Y + -0.4985363261688878 * Z;
-  double G = -0.9692549499965682 * X + 1.8759900014898907 * Y + 0.04155592655829284 * Z;
-  double B = 0.05564663913517716 * X + -0.20404133836651123 * Y + 1.0573110696453443 * Z;
-  R = pp_srgb_gamma(R); G = pp_srgb_gamma(G); B = pp_srgb_gamma(B);
-  out[0] = (uint8_t)(fmin(fmax(R, 0.0), 1.0) * 255.0);
-  out[1] = (uint8_t)(fmin(fmax(G, 0.0), 1.0) * 255.0);
-  out[2] = (uint8_t)(fmin(fmax(B, 0.0), 1.0) * 255.0);
-}
-
-// OpenCV interpolateCubic (A = -0.75), float coefficients; taps s-1 .. s+2 with clipped indices
+// OpenCV interpolateCubic (A = -0.75) in float32, each operation rounded on its own in OpenCV's order (nvcc would
+// contract the polynomial into FMAs); taps s-1 .. s+2 with clipped indices
 __device__ __forceinline__ void cv_cubic_coef(int d, double scale, int& s, float (&w)[4]) {
-  float f = __double2float_rn(((double)d + 0.5) * scale - 0.5);
+  const float f = cv_src_coord(d, scale);
   s = (int)floorf(f);
   const float x = __fsub_rn(f, (float)s);
-  const float A = -0.75f;
-  w[0] = ((A * (x + 1) - 5 * A) * (x + 1) + 8 * A) * (x + 1) - 4 * A;
-  w[1] = ((A + 2) * x - (A + 3)) * x * x + 1;
-  w[2] = ((A + 2) * (1 - x) - (A + 3)) * (1 - x) * (1 - x) + 1;
-  w[3] = 1.f - w[0] - w[1] - w[2];
+  const float A = -0.75f, A5 = 5 * A, A8 = 8 * A, A4 = 4 * A, A2 = A + 2, A3 = A + 3;   // exact in float32
+  const float x1 = __fadd_rn(x, 1.f), y = __fsub_rn(1.f, x);
+  w[0] = __fsub_rn(__fmul_rn(__fadd_rn(__fmul_rn(__fsub_rn(__fmul_rn(A, x1), A5), x1), A8), x1), A4);
+  w[1] = __fadd_rn(__fmul_rn(__fmul_rn(__fsub_rn(__fmul_rn(A2, x), A3), x), x), 1.f);
+  w[2] = __fadd_rn(__fmul_rn(__fmul_rn(__fsub_rn(__fmul_rn(A2, y), A3), y), y), 1.f);
+  w[3] = __fsub_rn(__fsub_rn(__fsub_rn(1.f, w[0]), w[1]), w[2]);
 }
 
+// cv2's float64 INTER_CUBIC (HResizeCubic, then VResizeCubic): per source row the four products v * wx summed left to
+// right, then the four rows weighted by wy the same way; every product and sum rounded on its own, so the resized ab
+// equals cv2's bit for bit (tests/cubic_ref.py)
 __global__ void cubic_lab2rgb_kernel(const double* __restrict__ ab, int hin, int win, const double* __restrict__ L,
                                      int H, int W, double scale_y, double scale_x, uint8_t* __restrict__ rgb) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -103,6 +96,9 @@ __global__ void cubic_lab2rgb_kernel(const double* __restrict__ ab, int hin, int
   float wx[4], wy[4];
   cv_cubic_coef(dx, scale_x, sx, wx);
   cv_cubic_coef(dy, scale_y, sy, wy);
+  int xs[4];
+#pragma unroll
+  for (int k = 0; k < 4; ++k) xs[k] = min(max(sx - 1 + k, 0), win - 1);
   double v[2];
 #pragma unroll
   for (int c = 0; c < 2; ++c) {
@@ -110,20 +106,16 @@ __global__ void cubic_lab2rgb_kernel(const double* __restrict__ ab, int hin, int
     double acc = 0.0;
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
-      int yy = sy - 1 + j;
-      yy = yy < 0 ? 0 : (yy > hin - 1 ? hin - 1 : yy);
-      double row = 0.0;
+      const double* r = p + (size_t)min(max(sy - 1 + j, 0), hin - 1) * win;
+      double row = __dmul_rn(r[xs[0]], (double)wx[0]);
 #pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        int xx = sx - 1 + k;
-        xx = xx < 0 ? 0 : (xx > win - 1 ? win - 1 : xx);
-        row += p[(size_t)yy * win + xx] * (double)wx[k];
-      }
-      acc += row * (double)wy[j];
+      for (int k = 1; k < 4; ++k) row = __dadd_rn(row, __dmul_rn(r[xs[k]], (double)wx[k]));
+      const double t = __dmul_rn(row, (double)wy[j]);
+      acc = j == 0 ? t : __dadd_rn(acc, t);
     }
     v[c] = acc;
   }
-  pp_lab_to_rgb_u8(L[i], v[0], v[1], rgb + i * 3);
+  lab_to_rgb_u8(L[i], v[0], v[1], rgb + i * 3);
 }
 
 cudaError_t launch_cubic_lab2rgb(const double* ab, int hin, int win, const double* L, int H, int W, uint8_t* rgb,

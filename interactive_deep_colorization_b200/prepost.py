@@ -1,7 +1,7 @@
 """GPU versions of the steps either side of the network (SURVEY 8f row f1).
 
     rgb2lab_gpu        skimage color.rgb2lab on uint8 RGB  (reference data/colorize_image.py:31-36,172-178,196-198)
-    fullres_rgb_gpu    get_img_fullres (:123-131): scipy zoom(order=1) of ab + Lab->RGB at full resolution
+    fullres_rgb_gpu    get_img_fullres (:123-131): scipy zoom(order=1) of the output ab + Lab->RGB at full resolution
     render_planes_gpu  the grey, input, mask and supervision renders at full resolution (:119-158)
 
 float64 arithmetic on the device, like the reference's numpy path.  torch supplies device memory only.
@@ -124,24 +124,10 @@ def display_rgb_gpu(ab, l_win, device=0):
 
 
 def fullres_rgb_gpu(ab, l_fullres, device=0):
-    """ab [2,h,w] (any float), l_fullres [1,H,W] or [H,W] float64 (numpy or DeviceLab) -> uint8 [H,W,3]."""
-    torch = _torch()
-    ab = np.ascontiguousarray(ab, dtype=np.float64)
-    d_ab = torch.from_numpy(ab).to("cuda:%d" % device)
-    if isinstance(l_fullres, DeviceLab):                  # L never left the device
-        d_L = l_fullres.device_plane(0).contiguous()
-        H, W = d_L.shape
-    else:
-        L = np.ascontiguousarray(np.asarray(l_fullres, dtype=np.float64).reshape(l_fullres.shape[-2], l_fullres.shape[-1]))
-        H, W = L.shape
-        d_L = torch.from_numpy(L).to(d_ab.device)
-    d_rgb = torch.empty((H, W, 3), dtype=torch.uint8, device=d_ab.device)
-    st = torch.cuda.current_stream(d_ab.device).cuda_stream
-    rc = _lib.load().idc_zoom_lab2rgb_u8(device, ab.shape[1], ab.shape[2], d_ab.data_ptr(), H, W, d_L.data_ptr(),
-                                         d_rgb.data_ptr(), st)
-    if rc != _lib.IDC_OK:
-        raise _lib.IdcError(rc, "idc_zoom_lab2rgb_u8 failed")
-    return d_rgb.cpu().numpy()
+    """get_img_fullres: ab [2,h,w] float32 / float64, l_fullres [1,H,W] or [H,W] float64 (numpy or DeviceLab) -> uint8
+    [H,W,3].  The input render of render_planes_gpu with the output ab, so the zoom is scipy's, edge rule included."""
+    H, W = l_fullres.shape[-2:]
+    return render_planes_gpu(H, W, ab=ab, ab_order=1, L=l_fullres, device=device)
 
 
 def render_planes_gpu(h, w, ab=None, ab_order=1, mask=None, l_mode=_lib.RENDER_L_PLANE, L=None, device=0):

@@ -218,3 +218,29 @@ def test_render_planes_argument_validation_without_gpu():
     for b in bad:
         a = dict(ok, **b)
         assert lib.idc_render_planes_u8(*a.values()) == -1, b
+
+
+@pytest.mark.parametrize("cls", CLASSES, ids=lambda c: c.__name__)
+def test_get_img_fullres_is_the_input_render_of_the_output_ab(cls, monkeypatch):
+    """Under the gate get_img_fullres renders through render_planes_gpu (scipy's zoom rule, cval rows included): the
+    output ab with order 1 and the full-resolution L, which is handed over as is (a DeviceLab stays on the device)."""
+    stub = _Stub()
+    monkeypatch.setattr(prepost, "render_planes_gpu", stub)
+    cm = _wrapper(cls)
+    cm.gpu_prepost = True
+    assert np.array_equal(cm.get_img_fullres(), np.full((75, 91, 3), 7, np.uint8))
+    ((h, w, kw),) = stub.calls
+    assert (h, w) == (75, 91) and kw["ab"] is cm.output_ab and kw["ab_order"] == 1 and kw["L"] is cm.img_l_fullres
+    assert "mask" not in kw and kw.get("l_mode", _lib.RENDER_L_PLANE) == _lib.RENDER_L_PLANE and kw["device"] == 0
+
+
+def test_zoom_lab2rgb_argument_validation_without_gpu():
+    """idc_zoom_lab2rgb_u8 (get_img_fullres in the C ABI) rejects what idc_render_planes_u8 rejects, and a NULL ab,
+    before touching a device."""
+    lib = _lib.load()
+    buf = np.zeros(64)
+    p = ctypes.c_void_p(buf.ctypes.data)
+    ok = dict(device=0, h_in=4, w_in=4, ab=p, h=8, w=8, L=p, rgb=p, stream=None)
+    for b in (dict(ab=None), dict(L=None), dict(rgb=None), dict(h=0), dict(w=-1), dict(h_in=0), dict(w_in=0),
+              dict(h=1 << 30, w=1 << 30)):
+        assert lib.idc_zoom_lab2rgb_u8(*dict(ok, **b).values()) == -1, b

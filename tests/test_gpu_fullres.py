@@ -1,5 +1,5 @@
-"""GPU: the full-resolution renders (render_planes_kernel, idc_render_planes_u8) -- get_img_gray_fullres,
-get_input_img_fullres, get_img_mask_fullres and get_sup_fullres of the wrapper classes (reference
+"""GPU: the full-resolution renders (render_planes_kernel, idc_render_planes_u8) -- get_img_fullres,
+get_img_gray_fullres, get_input_img_fullres, get_img_mask_fullres and get_sup_fullres of the wrapper classes (reference
 data/colorize_image.py:119-158) -- against scipy.ndimage.zoom + oracle/color_ref, and against ColorizeImageBase's own
 statements on the same object."""
 import cv2
@@ -7,17 +7,23 @@ import numpy as np
 import pytest
 from scipy.ndimage import zoom
 
-from interactive_deep_colorization_b200 import _lib, prepost
+from interactive_deep_colorization_b200 import _lib, color, prepost
 from interactive_deep_colorization_b200 import colorize_image as CI
 from oracle import color_ref
-from tests import zoom_ref
+from tests import util, zoom_ref
 from tests.test_gpu_configs import _caffe_scaled, _glob_sd
 
 pytestmark = pytest.mark.gpu
 PLANE, MASK, SUP = _lib.RENDER_L_PLANE, _lib.RENDER_L_MASK, _lib.RENDER_L_SUP
-GETTERS = ("get_img_gray_fullres", "get_input_img_fullres", "get_img_mask_fullres", "get_sup_fullres")
+GETTERS = ("get_img_fullres", "get_img_gray_fullres", "get_input_img_fullres", "get_img_mask_fullres",
+           "get_sup_fullres")
 # two output sizes past 256 whose float64 ratio 255/(n-1) rounds up (the last row / column reads cval)
 OVER = [n for n in range(400, 800) if zoom_ref.overshoot(256, n)[-1]][:2]
+
+
+def _rgb255(lab2rgb, L, ab):
+    """255 * clip(lab2rgb, 0, 1) of L [1,H,W] and ab [2,H,W]: a render before its truncating cast."""
+    return np.clip(lab2rgb(np.concatenate((L, ab), axis=0).transpose((1, 2, 0))), 0, 1) * 255
 
 
 def _close(got, want, what):
@@ -38,7 +44,7 @@ def _planes(h_in, w_in, H, W, dtype, seed):
 
 @pytest.mark.parametrize("h_in,w_in,H,W", [(256, 256, 256, 256), (256, 256, 507, 600), (256, 256, 100, 80),
                                            (64, 64, 75, 91), (256, 256, 1, 300), (64, 64, 91, 1),
-                                           (256, 256, 45, 53), (256, 256, OVER[0], OVER[1])])
+                                           (256, 256, 45, 53), (256, 256, OVER[0], OVER[1]), (256, 256, 768, 1280)])
 @pytest.mark.parametrize("dtype", [np.float64, np.float32])
 def test_render_planes_kernel_against_scipy(h_in, w_in, H, W, dtype):
     ab, mask, L = _planes(h_in, w_in, H, W, dtype, seed=H * 7 + W)
@@ -46,6 +52,10 @@ def test_render_planes_kernel_against_scipy(h_in, w_in, H, W, dtype):
     zeros = np.zeros((2, H, W))
     gray = prepost.render_planes_gpu(H, W, L=L)
     _close(gray, color_ref.lab2rgb_transpose(L, zeros), "gray")
+    # get_img_fullres: scipy's order-1 zoom of the (output) ab with the full-resolution L, exact off truncation edges
+    full = prepost.fullres_rgb_gpu(ab, L)
+    rgb255 = _rgb255(color_ref.lab2rgb, L, zoom(ab, f, order=1))
+    util.assert_render_exact(full, rgb255.astype(np.uint8), rgb255, ("fullres", H, W, dtype.__name__))
     for order in (0, 1):
         z_ab = zoom(ab, f, order=order)
         assert z_ab.dtype == dtype and z_ab.shape == (2, H, W)
@@ -64,8 +74,8 @@ def test_render_planes_kernel_against_scipy(h_in, w_in, H, W, dtype):
     sup = prepost.render_planes_gpu(H, W, ab=ab, ab_order=0, mask=mask, l_mode=SUP)
     for sel in ((oy, slice(None)), (slice(None), ox)):
         assert np.all(m[sel] == white) and np.all(sup[sel] == 0)
-        assert np.array_equal(inp[sel], gray[sel])
-    if (H, W) in ((45, 53), tuple(OVER)):
+        assert np.array_equal(inp[sel], gray[sel]) and np.array_equal(full[sel], gray[sel])
+    if (H, W) in ((45, 53), tuple(OVER), (768, 1280)):
         assert oy.sum() == 1 and ox.sum() == 1
 
 
@@ -125,6 +135,11 @@ def _wrapper(kind, synth_sd, tmp_path):
     return cm
 
 
+def _fullres_rgb255(cm):
+    """get_img_fullres's host statement before its truncating cast (ColorizeImageBase.get_img_fullres)."""
+    return _rgb255(color.lab2rgb, np.asarray(cm.img_l_fullres), cm._to_fullres(cm.output_ab, cm.output_ab, 1))
+
+
 def _check_getters(cm, what):
     """The device renders first (the host statements below copy the full-resolution L to the host)."""
     dev = {g: getattr(cm, g)() for g in GETTERS}
@@ -133,6 +148,8 @@ def _check_getters(cm, what):
         host = getattr(CI.ColorizeImageBase, g)(cm)
         if g == "get_img_mask_fullres":
             assert np.array_equal(dev[g], host), (what, g)
+        elif g == "get_img_fullres":
+            util.assert_render_exact(dev[g], host, _fullres_rgb255(cm), (what, g))
         else:
             _close(dev[g], host, (what, g))
 
@@ -169,3 +186,23 @@ def test_input_render_of_an_18_megapixel_photo(synth_sd, tmp_path):
     got = cm.get_input_img_fullres()
     assert cm.img_l_fullres._host is None
     _close(got, CI.ColorizeImageBase.get_input_img_fullres(cm), "18 MP input render")
+
+
+def test_fullres_render_of_a_24_megapixel_photo(synth_sd, tmp_path):
+    """256^2 -> 4000 x 6000: the float64 ratio 255 / (n - 1) rounds up on both axes, so scipy's last row and last
+    column read cval (ab = 0) and get_img_fullres shows them grey, like the reference."""
+    cm = CI.ColorizeImageB200(Xd=256)
+    cm.prep_net(state_dict=synth_sd)
+    _load(cm, tmp_path, 4000, 6000, seed=3)
+    ab, m = np.zeros((2, 256, 256)), np.zeros((1, 256, 256))
+    for (loc, p, val) in POINTS:
+        CI.put_point(ab, m, loc, p, val)
+    cm.net_forward(ab, m)
+    got = cm.get_img_fullres()
+    gray = cm.get_img_gray_fullres()
+    assert cm.img_l_fullres._host is None
+    oy, ox = zoom_ref.overshoot(256, 4000), zoom_ref.overshoot(256, 6000)
+    assert oy.sum() == 1 and oy[-1] and ox.sum() == 1 and ox[-1]
+    assert np.array_equal(got[-1], gray[-1]) and np.array_equal(got[:, -1], gray[:, -1])
+    assert np.any(got[:-1, :-1] != gray[:-1, :-1])                      # the hints do colour the inside
+    util.assert_render_exact(got, CI.ColorizeImageBase.get_img_fullres(cm), _fullres_rgb255(cm), "24 MP fullres render")

@@ -2,14 +2,15 @@
 
 On seeded synthetic photos at 507 x 600 and 3456 x 5184 (loaded with load_image, a dense net_forward of four hints at
 256^2, seeded synthetic weights from oracle/synth) it measures
-  * host wall time, median of --reps, ending with the uint8 result in host memory, of each of get_img_gray_fullres,
-    get_input_img_fullres, get_img_mask_fullres and get_sup_fullres: ColorizeImageB200's device path (`device_s`)
-    and the ColorizeImageBase statements on the same object (`host_s`, scipy zoom + float64 lab2rgb; the full-resolution
-    L is already on the host for them: that one-time copy is `l_copy_to_host_s`), and how far the two results are apart,
+  * host wall time, median of --reps, ending with the uint8 result in host memory, of each of get_img_fullres,
+    get_img_gray_fullres, get_input_img_fullres, get_img_mask_fullres and get_sup_fullres: ColorizeImageB200's device
+    path (`device_s`) and the ColorizeImageBase statements on the same object (`host_s`, scipy zoom + float64 lab2rgb;
+    the full-resolution L is already on the host for them: that one-time copy is `l_copy_to_host_s`), and how far the
+    two results are apart,
   * the GUI's save sequence (ui/gui_draw.py save_result: get_img_fullres, get_input_img_fullres, get_input_img,
     get_sup_img) with the host and with the device input render,
-  * CUDA-event kernel times, mean over --launches warmed launches, of render_planes_kernel in each mode (and of
-    zoom_lab2rgb_kernel for comparison), with the bytes each moves,
+  * CUDA-event kernel times, mean over --launches warmed launches, of render_planes_kernel in each mode (the input
+    mode is also get_img_fullres's launch), with the bytes each moves,
   * the card's name and power limit, read in the same run.
 
     python tools/fullres_profile.py --out DIR [--sizes 507x600,3456x5184] [--reps 5] [--host-reps 3] [--launches 50]
@@ -34,7 +35,8 @@ from interactive_deep_colorization_b200 import colorize_image as CI  # noqa: E40
 from oracle import synth  # noqa: E402
 
 HBM_BPS = 3.35e12       # H100 SXM data sheet
-GETTERS = ("get_img_gray_fullres", "get_input_img_fullres", "get_img_mask_fullres", "get_sup_fullres")
+GETTERS = ("get_img_fullres", "get_img_gray_fullres", "get_input_img_fullres", "get_img_mask_fullres",
+           "get_sup_fullres")
 POINTS = [([135, 160], 3, [23, -69]), ([100, 60], 5, [-40, 15.5]), ([250, 3], 2, [60, 60]), ([30, 200], 4, [-10, -80])]
 
 
@@ -134,13 +136,10 @@ def one_size(H, W, sd, tmp, reps, host_reps, launches):
         nbytes = 3 * H * W + (8 * H * W if mode == P else 0)
         kern["render_planes_kernel_" + name] = {"ms": ms, "bytes": nbytes, "GBps": nbytes / ms * 1e-6,
                                                 "floor_ms_at_3.35TBps": nbytes / HBM_BPS * 1e3}
-    ms = kernel_ms(lambda: lib.idc_zoom_lab2rgb_u8(0, 256, 256, d_ab.data_ptr(), H, W, d_L.data_ptr(), rgb.data_ptr(), st),
-                   launches)
-    kern["zoom_lab2rgb_kernel"] = {"ms": ms, "bytes": 11 * H * W, "GBps": 11 * H * W / ms * 1e-6}
     res["kernels"] = kern
     # bytes each device getter moves between host and device: its planes up (float64), the uint8 result down
-    up = {"get_img_gray_fullres": 0, "get_input_img_fullres": 2 * 8 * 256 * 256, "get_img_mask_fullres": 8 * 256 * 256,
-          "get_sup_fullres": 3 * 8 * 256 * 256}
+    up = {"get_img_fullres": 2 * 8 * 256 * 256, "get_img_gray_fullres": 0, "get_input_img_fullres": 2 * 8 * 256 * 256,
+          "get_img_mask_fullres": 8 * 256 * 256, "get_sup_fullres": 3 * 8 * 256 * 256}
     for g in GETTERS:
         res[g]["h2d_bytes"], res[g]["d2h_bytes"] = up[g], 3 * H * W
     res["l_copy_to_host_bytes"] = 8 * H * W

@@ -4,7 +4,7 @@
 
     rgb2lab_kernel          18 MP photo (3456 x 5184, bird_gray.jpg's size), uint8 -> float64 Lab
     resize_linear_u8_kernel 3456 x 5184 -> 256 x 256
-    zoom_lab2rgb_kernel     256^2 ab -> 3456 x 5184 full-resolution render
+    render_planes_kernel    256^2 ab -> 3456 x 5184 full-resolution render (get_img_fullres)
     cubic_lab2rgb_kernel    256^2 ab -> 512 x 512 display
     global_stats_kernel     256 x 256 reference image
     decode313_kernel        batch 16, 256^2 (Caffe-spec annealed mean), + hyper / pred313 GEMMs in the same forward

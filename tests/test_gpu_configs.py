@@ -260,12 +260,7 @@ def test_global_stats_kernel_vs_reference_nnenc():
         assert moved <= near + 0.01
 
 
-def _caffe_scaled(sd):
-    """A synthetic 'Caffe-scaled' weight set: conv1_1 expects raw L-50 / ab / mask*110 (SURVEY q4)."""
-    out = dict(sd)
-    s = torch.tensor([100.0, 110.0, 110.0, 110.0]).reshape(1, 4, 1, 1)
-    out["model1.0.weight"] = (sd["model1.0.weight"].double() / s.double()).float()
-    return out
+_caffe_scaled = util.caffe_scaled
 
 
 def test_caffe_named_wrappers(synth_sd):

@@ -54,6 +54,14 @@ def make_ctx(sd, H, W, max_n=1, **kw):
     return ctx
 
 
+def caffe_scaled(sd):
+    """A synthetic 'Caffe-scaled' weight set: conv1_1 expects raw L-50 / ab / mask*110 (SURVEY q4)."""
+    out = dict(sd)
+    s = torch.tensor([100.0, 110.0, 110.0, 110.0]).reshape(1, 4, 1, 1)
+    out["model1.0.weight"] = (sd["model1.0.weight"].double() / s.double()).float()
+    return out
+
+
 def dev(a):
     return torch.from_numpy(np.ascontiguousarray(a)).float().cuda().contiguous()
 

@@ -84,7 +84,8 @@ int idc_create(int device, int max_n, int h, int w, unsigned flags, idc_ctx** ou
  *   "side_dist"     0 / 1       batches <= 4: run the dist head (class + softmax) on a side stream / graph branch
  *   "tanh_scale"    110 / 100   regression head scale: tanh * 110 (model.py:175) or the Caffe nets' 100
  *                               (models/reference_model/deploy_nodist.prototxt:812-822, SURVEY q4)
- * Unknown names return IDC_ERR_KEY. */
+ * Unknown names return IDC_ERR_KEY.  A re-plan that fails returns its error and leaves the context refusing forwards
+ * with IDC_ERR_STATE until a later re-plan (idc_set_option or idc_adopt_weights) succeeds. */
 int idc_set_option(idc_ctx* ctx, const char* name, int value);
 
 /* Replaces one entry of `self.net.load_state_dict(state_dict)` (data/colorize_image.py:229).

@@ -39,7 +39,7 @@ constexpr float kBnEps = 1e-5f;  // nn.BatchNorm2d default (SURVEY q7)
 int add_buf(Ctx* c, const char* name, int H, int W, int C) {
   ActBuf b;
   b.name = name; b.H = H; b.W = W; b.C = C;
-  c->bufs.push_back(b);
+  c->bufs.push_back(std::move(b));
   c->buf_index[name] = (int)c->bufs.size() - 1;
   return (int)c->bufs.size() - 1;
 }
@@ -63,7 +63,7 @@ void add_conv(Ctx* c, const char* name, const char* wkey, const char* in, int s,
   op.cout = ob.C; op.cout_pad = ob.C; op.K = 9 * ib.C;
   op.epi.act = act; op.epi.has_bn = bnkey != nullptr; op.epi.gadd = gadd;
   op.flops_per_image = 2.0 * op.Hl * op.Wl * (double)op.cout * op.K;
-  c->ops.push_back(op);
+  c->ops.push_back(std::move(op));
 }
 
 // ConvTranspose2d(4x4, s2, p1) of `lo` + Conv2d(3x3) of the skip tensor, summed, then ReLU
@@ -101,7 +101,7 @@ void add_up(Ctx* c, const char* name, const char* dkey, const char* lo, const ch
   op.cout = ob.C; op.cout_pad = ob.C; op.K = 4 * lb.C + 9 * sb.C;
   op.epi.act = ACT_RELU;
   op.flops_per_image = 2.0 * 4 * op.Hl * op.Wl * (double)op.cout * op.K;
-  c->ops.push_back(op);
+  c->ops.push_back(std::move(op));
 }
 
 void build_plan(Ctx* c) {
@@ -156,7 +156,7 @@ void build_plan(Ctx* c) {
     op.Hl = ib.H; op.Wl = ib.W; op.out_buf = -1; op.os = 1;
     op.cout = 529; op.cout_pad = 576; op.K = ib.C; op.out_f32 = true; op.src_k[0] = 1;
     op.flops_per_image = 2.0 * op.Hl * op.Wl * 529.0 * op.K;
-    c->ops.push_back(op);
+    c->ops.push_back(std::move(op));
   }
   // Caffe-spec 313-bin head (row a14): hyper-column = conv3x3(conv3_3) + sum_l deconv4x4s2(conv{4..7}_3) +
   // conv3x3(conv8_3) -> ReLU (deploy_nopred.prototxt:651-763), then pred_313 = conv1x1 384->313 (:765-775)
@@ -191,7 +191,7 @@ void build_plan(Ctx* c) {
     op.cout = 384; op.cout_pad = 384; op.K = 4 * 4 * 512 + 2 * 9 * 256;
     op.epi.act = ACT_RELU;
     op.flops_per_image = 2.0 * 4 * op.Hl * op.Wl * 384.0 * op.K;
-    c->ops.push_back(op);
+    c->ops.push_back(std::move(op));
 
     ConvOp pr;
     pr.name = "pred313"; pr.kind = OP_CLASS; pr.wkey[0] = "caffe.pred_313"; pr.src_k[0] = 1;
@@ -200,7 +200,7 @@ void build_plan(Ctx* c) {
     pr.Hl = H / 4; pr.Wl = W / 4; pr.out_buf = -1; pr.os = 1;
     pr.cout = 313; pr.cout_pad = 320; pr.K = 384; pr.out_f32 = true;
     pr.flops_per_image = 2.0 * pr.Hl * pr.Wl * 313.0 * pr.K;
-    c->ops.push_back(pr);
+    c->ops.push_back(std::move(pr));
   }
   // level 9                                                                  model.py:162-163, 86-93
   add_up(c, "up9", "model9up.0", "conv8_3", "model2short9.0", "conv2_2", "a9_1");
@@ -223,7 +223,7 @@ void build_plan(Ctx* c) {
     op.cout = 128; op.cout_pad = 128; op.K = 9 * ib.C;
     op.epi.act = ACT_LEAKY02; op.fuse_out_head = true;
     op.flops_per_image = 2.0 * op.Hl * op.Wl * 128.0 * op.K;
-    c->ops.push_back(op);
+    c->ops.push_back(std::move(op));
   }
 }
 
@@ -305,7 +305,7 @@ void fold_bn(const HostTensor& g, const HostTensor& b, const HostTensor& m, cons
 
 int pack_weights(Ctx* c, char* host) {
   // translate device pointers (already laid out relative to c->arena) to host staging pointers
-  auto H = [&](void* dev) { return host + ((char*)dev - c->arena); };
+  auto H = [&](void* dev) { return host + ((char*)dev - c->arena.get()); };
   // conv1_1: [36][64], k = (ky*3+kx)*4 + cin                                       model.py:13
   {
     const HostTensor* w = find(c, "model1.0.weight");
@@ -437,51 +437,66 @@ int alloc_workspace(Ctx* c) {
     if (b.H == 0) continue;
     const size_t elems = (size_t)c->max_n * b.H * b.W * b.C;
     if (c->simt) {
-      CUDA_TRY(c, cudaMalloc(&b.p0, elems * sizeof(float)));
+      CUDA_TRY(c, cudaMalloc(b.p0.put(), elems * sizeof(float)));
     } else {
-      CUDA_TRY(c, cudaMalloc(&b.p0, elems * sizeof(__half)));
-      if (!c->fast) CUDA_TRY(c, cudaMalloc(&b.p1, elems * sizeof(__half)));
+      CUDA_TRY(c, cudaMalloc(b.p0.put(), elems * sizeof(__half)));
+      if (!c->fast) CUDA_TRY(c, cudaMalloc(b.p1.put(), elems * sizeof(__half)));
     }
   }
-  if (c->dist) CUDA_TRY(c, cudaMalloc(&c->logits, sizeof(float) * (size_t)c->max_n * (c->H / 4) * (c->W / 4) * 576));
+  if (c->dist) CUDA_TRY(c, cudaMalloc(c->logits.put(), sizeof(float) * (size_t)c->max_n * (c->H / 4) * (c->W / 4) * 576));
   if (c->caffe313) {
-    CUDA_TRY(c, cudaMalloc(&c->logits313, sizeof(float) * (size_t)c->max_n * (c->H / 4) * (c->W / 4) * 320));
-    CUDA_TRY(c, cudaMalloc(&c->pts313, sizeof(float) * 313 * 2));
+    CUDA_TRY(c, cudaMalloc(c->logits313.put(), sizeof(float) * (size_t)c->max_n * (c->H / 4) * (c->W / 4) * 320));
+    CUDA_TRY(c, cudaMalloc(c->pts313.put(), sizeof(float) * 313 * 2));
   }
   for (auto& op : c->ops)
-    if (op.out_f32) op.out_f32_ptr = (op.name == "pred313") ? c->logits313 : c->logits;
+    if (op.out_f32) op.out_f32_ptr = (op.name == "pred313") ? c->logits313.get() : c->logits.get();
   if (c->glob) {
-    CUDA_TRY(c, cudaMalloc(&c->gvec, sizeof(float) * (size_t)c->max_n * 512));
-    CUDA_TRY(c, cudaMalloc(&c->gtmp, sizeof(float) * (size_t)2 * c->max_n * 512));
+    CUDA_TRY(c, cudaMalloc(c->gvec.put(), sizeof(float) * (size_t)c->max_n * 512));
+    CUDA_TRY(c, cudaMalloc(c->gtmp.put(), sizeof(float) * (size_t)2 * c->max_n * 512));
   }
-  CUDA_TRY(c, cudaHostAlloc(&c->h_err, 64, cudaHostAllocMapped));
-  memset(c->h_err, 0, 64);
-  CUDA_TRY(c, cudaHostGetDevicePointer(&c->d_err, c->h_err, 0));
+  CUDA_TRY(c, cudaHostAlloc(c->h_err.put(), 64, cudaHostAllocMapped));
+  memset(c->h_err.get(), 0, 64);
+  CUDA_TRY(c, cudaHostGetDevicePointer(&c->d_err, c->h_err.get(), 0));
+  CUDA_TRY(c, cudaStreamCreateWithFlags(c->own_stream.put(), cudaStreamNonBlocking));
   return IDC_OK;
 }
 
+// Forwards are refused from here until every plan and the split-K workspace are in place: a failed (re-)plan leaves
+// weights_ready false until a later plan succeeds.
 int plan_engines(Ctx* c) {
-  if (c->simt) return IDC_OK;
+  c->weights_ready = false;
+  if (c->simt) { c->weights_ready = true; return IDC_OK; }
   c->splitk_ws_floats = 0; c->splitk_max_tiles = 0;
   for (auto& op : c->ops) {
     int rc = umma_plan_op(c, op);
     if (rc != IDC_OK) return rc;
   }
-  if (c->splitk_ws) { cudaFree(c->splitk_ws); c->splitk_ws = nullptr; }
-  if (c->splitk_counters) { cudaFree(c->splitk_counters); c->splitk_counters = nullptr; }
+  c->splitk_ws.reset();
+  c->splitk_counters.reset();
   if (c->splitk_ws_floats) {
-    CUDA_TRY(c, cudaMalloc(&c->splitk_ws, c->splitk_ws_floats * sizeof(float)));
-    CUDA_TRY(c, cudaMalloc(&c->splitk_counters, sizeof(int) * 2 * (size_t)c->splitk_max_tiles));
-    CUDA_TRY(c, cudaMemset(c->splitk_counters, 0, sizeof(int) * 2 * (size_t)c->splitk_max_tiles));
+    CUDA_TRY(c, cudaMalloc(c->splitk_ws.put(), c->splitk_ws_floats * sizeof(float)));
+    CUDA_TRY(c, cudaMalloc(c->splitk_counters.put(), sizeof(int) * 2 * (size_t)c->splitk_max_tiles));
+    CUDA_TRY(c, cudaMemset(c->splitk_counters.get(), 0, sizeof(int) * 2 * (size_t)c->splitk_max_tiles));
   }
+  c->weights_ready = true;
   return IDC_OK;
 }
 
+// a code the device watchdog left in the mapped flag: clear it and fail with msg (which formats the code)
+int take_watchdog(Ctx* c, const char* msg) {
+  volatile int* flag = c->h_err.get();
+  const int werr = *flag;
+  if (!werr) return IDC_OK;
+  *flag = 0;
+  return fail(c, IDC_ERR_WATCHDOG, msg, werr);
+}
+
 // idc_forward_host's copy/compute overlap: the batch is cut into image chunks; conv1_1 of chunk k waits for the
-// H2D of chunk k only (issued on Ctx::s_in), and the last op (c10_2 + fused model_out) runs per chunk so that the
-// D2H of ab chunk k (on Ctx::s_out) overlaps the compute of chunk k+1.  Everything in between runs on the whole batch.
+// H2D of chunk k only (issued on HostPipeStreams::s_in), and the last op (c10_2 + fused model_out) runs per chunk so
+// that the D2H of ab chunk k (on HostPipeStreams::s_out) overlaps the compute of chunk k+1.  Everything in between
+// runs on the whole batch.
 struct HostPipe {
-  static constexpr int kMaxChunks = 8;   // == the size of Ctx::ev_in / ev_out
+  static constexpr int kMaxChunks = 8;   // == the size of HostPipeStreams::ev_in / ev_out
   int nchunks = 0;
   int start[kMaxChunks + 1] = {};        // image ranges [start[k], start[k+1])
   float* ab_dst = nullptr;    // pinned host destination of out_ab (caller's buffer or the staging block)
@@ -494,32 +509,30 @@ constexpr size_t kClickRes = (size_t)kClickInit * (3 * 32 + 2) * sizeof(double);
 constexpr size_t kClickCopy = kClickHdr + kClickPmf + kClickRes;         // what travels back per click
 constexpr size_t kClickBytes = kClickCopy + 529 * 2 * sizeof(float);     // + the default gamut grid (device only)
 
+cudaError_t new_stream(Stream& s) { return cudaStreamCreateWithFlags(s.put(), cudaStreamNonBlocking); }
+cudaError_t new_event(Event& e) { return cudaEventCreateWithFlags(e.put(), cudaEventDisableTiming); }
+
 // After the class conv of a small-batch forward: the clicked pixel's pmf straight from its 529 logits (same per-row
 // softmax routine as the full map, so the same bits), K-means on it (K from the click header), the block to pinned host
 // memory.  Runs next to the full-map softmax on a branch of the dist head's side branch.
-bool click_tail_on(Ctx* c, int n) { return c->click_mode && c->d_clickout && n <= 4; }
+bool click_tail_on(Ctx* c, int n) { return c->click_mode && c->click && n <= 4; }
 
 cudaError_t click_tail(Ctx* c, int n, cudaStream_t st) {
   if (!click_tail_on(c, n)) return cudaSuccess;
-  int* hdr = reinterpret_cast<int*>(c->d_clickout);
-  float* pmf = reinterpret_cast<float*>(c->d_clickout + kClickHdr);
-  double* res = reinterpret_cast<double*>(c->d_clickout + kClickHdr + kClickPmf);
-  const float* pts = reinterpret_cast<const float*>(c->d_clickout + kClickCopy);
-  cudaError_t e = launch_click_pmf(c, c->d_click, n, hdr, pmf, st);
+  char* out = c->click->d_clickout.get();
+  int* hdr = reinterpret_cast<int*>(out);
+  float* pmf = reinterpret_cast<float*>(out + kClickHdr);
+  double* res = reinterpret_cast<double*>(out + kClickHdr + kClickPmf);
+  const float* pts = reinterpret_cast<const float*>(out + kClickCopy);
+  cudaError_t e = launch_click_pmf(c, c->click->d_click, n, hdr, pmf, st);
   if (e != cudaSuccess) return e;
   if ((e = launch_ab_reccs(pmf, 1, pts, 0, kClickMaxIter, kClickInit, res, st, hdr)) != cudaSuccess) return e;
   c->launch_count += 2;
-  return cudaMemcpyAsync(c->h_clickout, c->d_clickout, kClickCopy, cudaMemcpyDeviceToHost, st);
+  return cudaMemcpyAsync(c->click->h_clickout.get(), out, kClickCopy, cudaMemcpyDeviceToHost, st);
 }
 
 // persistent-grid cap (CTAs, even) that leaves kClickInit SMs to the side branch
-int side_branch_cap(Ctx* c) {
-  cudaDeviceProp prop;
-  static int sms[64] = {};
-  int& n = sms[c->dev < 64 ? c->dev : 0];
-  if (!n) { cudaGetDeviceProperties(&prop, c->dev); n = prop.multiProcessorCount; }
-  return ((n - kClickInit) / 2) * 2;
-}
+int side_branch_cap(Ctx* c) { return ((c->num_sms - kClickInit) / 2) * 2; }
 
 int run_forward(Ctx* c, int n, const float* L, const float* ab, const float* mask, float maskcent, const float* glob,
                 float* out_ab, float* out_dist, uint8_t* out_rgb, cudaStream_t st, const HostPipe* hp = nullptr,
@@ -528,30 +541,33 @@ int run_forward(Ctx* c, int n, const float* L, const float* ab, const float* mas
   c->gadd_active = false;
   c->click_served = false;
   pdl_break(c);                        // whatever precedes this forward on `st` is not one of its kernels
-  std::vector<cudaEvent_t>* ev = nullptr;
-  auto mark = [&]() {
-    if (!ev) return;
-    cudaEvent_t e;
-    if (!c->prof_pool.empty()) { e = c->prof_pool.back(); c->prof_pool.pop_back(); }
-    else cudaEventCreate(&e);
-    cudaEventRecord(e, st);
-    ev->push_back(e);
+  std::vector<Event>* ev = nullptr;
+  auto mark = [&]() -> cudaError_t {
+    if (!ev) return cudaSuccess;
+    Event e;
+    cudaError_t ce = cudaSuccess;
+    if (!c->prof_pool.empty()) { e = std::move(c->prof_pool.back()); c->prof_pool.pop_back(); }
+    else ce = cudaEventCreate(e.put());
+    if (ce == cudaSuccess) ce = cudaEventRecord(e.get(), st);
+    if (ce != cudaSuccess) return ce;
+    ev->push_back(std::move(e));
     pdl_break(c);                      // per-op timing: kernels must not overlap their predecessors
+    return cudaSuccess;
   };
   if (c->profiling) { c->prof_runs.emplace_back(); ev = &c->prof_runs.back(); }
-  mark();
-  if (hp) CUDA_TRY(c, cudaStreamWaitEvent(st, c->ev_in[0], 0));     // covers the glob vector too
+  CUDA_TRY(c, mark());
+  if (hp) CUDA_TRY(c, cudaStreamWaitEvent(st, c->pipe->ev_in[0].get(), 0));     // covers the glob vector too
   if (glob && c->glob) {
     CUDA_TRY(c, launch_global_mlp(c, n, glob, st));
     c->gadd_active = true;
   }
   const size_t HW = (size_t)c->H * c->W;
-  const bool c11_umma = c->opt.conv1_1_umma && !c->simt && c->w11_umma;
+  const bool c11_umma = c->opt.conv1_1_umma && !c->simt && c->w11_umma.get();
   // hint mode: the ab / mask planes conv1_1 reads are rasterised here from the hint block (already on the device)
   if (hints_dev) CUDA_TRY(c, launch_hint_raster(c, n, hints_dev, const_cast<float*>(ab), const_cast<float*>(mask), st));
   if (hp) {
     for (int k = 0; k < hp->nchunks; ++k) {
-      CUDA_TRY(c, cudaStreamWaitEvent(st, c->ev_in[k], 0));
+      CUDA_TRY(c, cudaStreamWaitEvent(st, c->pipe->ev_in[k].get(), 0));
       pdl_break(c);
       if (c11_umma) CUDA_TRY(c, launch_conv1_1_umma(c, hp->start[k + 1] - hp->start[k], L, ab, mask, maskcent, st, hp->start[k]));
       else CUDA_TRY(c, launch_conv1_1(c, hp->start[k + 1] - hp->start[k], L, ab, mask, maskcent, st, hp->start[k]));
@@ -560,7 +576,7 @@ int run_forward(Ctx* c, int n, const float* L, const float* ab, const float* mas
     if (c11_umma) CUDA_TRY(c, launch_conv1_1_umma(c, n, L, ab, mask, maskcent, st));
     else CUDA_TRY(c, launch_conv1_1(c, n, L, ab, mask, maskcent, st));
   }
-  mark();
+  CUDA_TRY(c, mark());
   // Interactive batches: the dist head (class 1x1 conv + 529-way softmax) only depends on conv8_3, and decoder levels
   // 9-10 do not depend on it -> it runs on a side stream (a parallel branch of the click graph) on the ~20 SMs the
   // 128-CTA launches of the main chain leave idle, instead of sitting between c8_3 and up9 on the critical path.
@@ -569,34 +585,34 @@ int run_forward(Ctx* c, int n, const float* L, const float* ab, const float* mas
   for (size_t oi = 0; oi < c->ops.size(); ++oi) {
     ConvOp& op = c->ops[oi];
     if (side_dist && op.kind == OP_CLASS && op.name == "class") {
-      if (!c->s_side) {
-        CUDA_TRY(c, cudaStreamCreateWithFlags(&c->s_side, cudaStreamNonBlocking));
-        CUDA_TRY(c, cudaEventCreateWithFlags(&c->ev_fork, cudaEventDisableTiming));
-        CUDA_TRY(c, cudaEventCreateWithFlags(&c->ev_join, cudaEventDisableTiming));
+      if (!c->side) {
+        auto g = std::make_unique<SideBranch>();
+        CUDA_TRY(c, new_stream(g->s_side));
+        CUDA_TRY(c, new_stream(g->s_click));
+        for (Event* e : {&g->ev_fork, &g->ev_join, &g->ev_click[0], &g->ev_click[1]}) CUDA_TRY(c, new_event(*e));
+        c->side = std::move(g);
       }
+      const SideBranch& sb = *c->side;
+      const cudaStream_t side = sb.s_side.get(), side_click = sb.s_click.get();
+      const cudaEvent_t ev_click[2] = {sb.ev_click[0].get(), sb.ev_click[1].get()};
       cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
       CUDA_TRY(c, cudaStreamIsCapturing(st, &cap));
       const bool main_chain = c->chain;
-      CUDA_TRY(c, cudaEventRecord(c->ev_fork, st));
-      CUDA_TRY(c, cudaStreamWaitEvent(c->s_side, c->ev_fork, 0));
+      CUDA_TRY(c, cudaEventRecord(sb.ev_fork.get(), st));
+      CUDA_TRY(c, cudaStreamWaitEvent(side, sb.ev_fork.get(), 0));
       pdl_break(c);                                        // first kernel of the branch follows an event wait
-      CUDA_TRY(c, umma_run_op(c, op, n, nullptr, (float)c->opt.tanh_scale, c->s_side, 0, 16));
+      CUDA_TRY(c, umma_run_op(c, op, n, nullptr, (float)c->opt.tanh_scale, side, 0, 16));
       const bool click = click_tail_on(c, n);
       if (click) {   // idc_set_click: clicked pixel's pmf + suggestions only need the logits -> a branch of the branch
-        if (!c->s_click) {
-          CUDA_TRY(c, cudaStreamCreateWithFlags(&c->s_click, cudaStreamNonBlocking));
-          CUDA_TRY(c, cudaEventCreateWithFlags(&c->ev_click[0], cudaEventDisableTiming));
-          CUDA_TRY(c, cudaEventCreateWithFlags(&c->ev_click[1], cudaEventDisableTiming));
-        }
-        CUDA_TRY(c, cudaEventRecord(c->ev_click[0], c->s_side));
-        CUDA_TRY(c, cudaStreamWaitEvent(c->s_click, c->ev_click[0], 0));
-        CUDA_TRY(c, click_tail(c, n, c->s_click));
-        CUDA_TRY(c, cudaEventRecord(c->ev_click[1], c->s_click));
+        CUDA_TRY(c, cudaEventRecord(ev_click[0], side));
+        CUDA_TRY(c, cudaStreamWaitEvent(side_click, ev_click[0], 0));
+        CUDA_TRY(c, click_tail(c, n, side_click));
+        CUDA_TRY(c, cudaEventRecord(ev_click[1], side_click));
         if (cap != cudaStreamCaptureStatusActive) pdl_break(c);      // live stream: the record sits between class and softmax
       }
-      CUDA_TRY(c, launch_softmax529(c, n, out_dist, c->s_side));     // PDL-chained behind `class` on the side stream
-      if (click) CUDA_TRY(c, cudaStreamWaitEvent(c->s_side, c->ev_click[1], 0));
-      CUDA_TRY(c, cudaEventRecord(c->ev_join, c->s_side));
+      CUDA_TRY(c, launch_softmax529(c, n, out_dist, side));          // PDL-chained behind `class` on the side stream
+      if (click) CUDA_TRY(c, cudaStreamWaitEvent(side, ev_click[1], 0));
+      CUDA_TRY(c, cudaEventRecord(sb.ev_join.get(), side));
       // in a capture the event record is not a node: up9 keeps its programmatic edge to c8_3; on a live stream the
       // record sits between the two kernels, so the next launch is serialised normally
       c->chain = (cap == cudaStreamCaptureStatusActive) ? main_chain : false;
@@ -609,20 +625,20 @@ int run_forward(Ctx* c, int n, const float* L, const float* ab, const float* mas
       for (int k = 0; k < hp->nchunks; ++k) {
         const int i0 = hp->start[k], nk = hp->start[k + 1] - i0;
         CUDA_TRY(c, umma_run_op(c, op, nk, out_ab, (float)c->opt.tanh_scale, st, i0));
-        CUDA_TRY(c, cudaEventRecord(c->ev_out[k], st));
+        CUDA_TRY(c, cudaEventRecord(c->pipe->ev_out[k].get(), st));
         pdl_break(c);
-        CUDA_TRY(c, cudaStreamWaitEvent(c->s_out, c->ev_out[k], 0));
+        CUDA_TRY(c, cudaStreamWaitEvent(c->pipe->s_out.get(), c->pipe->ev_out[k].get(), 0));
         CUDA_TRY(c, cudaMemcpyAsync(hp->ab_dst + (size_t)i0 * 2 * HW, out_ab + (size_t)i0 * 2 * HW,
-                                    (size_t)nk * 2 * HW * sizeof(float), cudaMemcpyDeviceToHost, c->s_out));
+                                    (size_t)nk * 2 * HW * sizeof(float), cudaMemcpyDeviceToHost, c->pipe->s_out.get()));
       }
     } else {
       // announced click: the suggestion kernel (8 CTAs of 1024 threads, a whole SM each) runs on the side branch next
       // to decoder levels 9-10; a full-width launch would queue behind it on 8 SMs and finish that much later.  Leaving 8
       // SMs free costs little: 512 tiles are 4 rounds on 132 and on 124 CTAs alike.
-      const int cap = (forked && c->click_mode && c->d_clickout) ? side_branch_cap(c) : 0;
+      const int cap = (forked && c->click_mode && c->click) ? side_branch_cap(c) : 0;
       CUDA_TRY(c, umma_run_op(c, op, n, op.fuse_out_head ? out_ab : nullptr, (float)c->opt.tanh_scale, st, 0, cap));
     }
-    mark();
+    CUDA_TRY(c, mark());
   }
   const bool fused = !c->simt && !(c->flags & IDC_FLAG_KEEP_CONV10);
   if (!fused) CUDA_TRY(c, launch_out_head(c, n, out_ab, st));
@@ -636,10 +652,10 @@ int run_forward(Ctx* c, int n, const float* L, const float* ab, const float* mas
     c->launch_count++;
   }
   if (forked) {
-    CUDA_TRY(c, cudaStreamWaitEvent(st, c->ev_join, 0));   // join: whatever follows on `st` sees the distribution
+    CUDA_TRY(c, cudaStreamWaitEvent(st, c->side->ev_join.get(), 0));   // join: whatever follows on `st` sees the distribution
     pdl_break(c);
   }
-  mark();
+  CUDA_TRY(c, mark());
   pdl_break(c);
   c->last_n = n;
   return IDC_OK;
@@ -675,22 +691,20 @@ int idc_create(int device, int max_n, int h, int w, unsigned flags, idc_ctx** ou
   if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return IDC_ERR_CUDA;
   if (prop.major != 9 || prop.minor != 0) return IDC_ERR_UNSUPPORTED;  // sm_90a cubins only; no fallback
   if (cudaSetDevice(device) != cudaSuccess) return IDC_ERR_CUDA;
-  idc_ctx* c = new idc_ctx();
-  c->dev = device; c->max_n = max_n; c->H = h; c->W = w; c->flags = flags;
+  std::unique_ptr<idc_ctx> c(new idc_ctx());
+  c->dev = device; c->num_sms = prop.multiProcessorCount; c->max_n = max_n; c->H = h; c->W = w; c->flags = flags;
   c->simt = flags & IDC_FLAG_ENGINE_SIMT;
   c->fast = (flags & IDC_FLAG_FAST_FP16) && !c->simt;
   c->dist = flags & IDC_FLAG_DIST;
   c->glob = flags & IDC_FLAG_GLOBAL_HINTS;
   c->caffe313 = flags & IDC_FLAG_CAFFE313;
-  build_plan(c);
-  int rc = alloc_workspace(c);
+  build_plan(c.get());
+  int rc = alloc_workspace(c.get());
   if (rc != IDC_OK) {
     fprintf(stderr, "idc_create: %s\n", c->err.c_str());
-    idc_destroy(c);
     return rc;
   }
-  cudaStreamCreateWithFlags(&c->own_stream, cudaStreamNonBlocking);
-  *out = c;
+  *out = c.release();
   return IDC_OK;
 }
 
@@ -704,13 +718,13 @@ int idc_set_option(idc_ctx* c, const char* name, int value) {
   for (auto& t : tab)
     if (!strcmp(t.n, name)) {
       *t.v = value;
-      if (c->weights_ready && strcmp(name, "host_pipe") && strcmp(name, "tanh_scale") && strcmp(name, "side_dist") && strcmp(name, "conv1_1_umma")) {      // plan-time option changed after planning: re-plan
+      if (c->weights_adopted && strcmp(name, "host_pipe") && strcmp(name, "tanh_scale") && strcmp(name, "side_dist") && strcmp(name, "conv1_1_umma")) {      // plan-time option changed after planning: re-plan
         CUDA_TRY(c, cudaSetDevice(c->dev));
         CUDA_TRY(c, cudaDeviceSynchronize());
         int rc = plan_engines(c);
         if (rc != IDC_OK) return rc;
       }
-      if (c->graph_exec) { cudaGraphExecDestroy(c->graph_exec); c->graph_exec = nullptr; }
+      c->graph_exec.reset();
       return IDC_OK;
     }
   return fail(c, IDC_ERR_KEY, "unknown option '%s'", name);
@@ -733,17 +747,17 @@ int idc_load_tensor(idc_ctx* c, const char* key, const void* data, int dtype, in
     default: return fail(c, IDC_ERR_ARG, "unknown dtype %d", dtype);
   }
   c->raw[key] = std::move(t);
-  c->weights_ready = false;
+  c->weights_ready = c->weights_adopted = false;
   return IDC_OK;
 }
 
 int idc_reserve_weights(idc_ctx* c) {
   if (!c) return IDC_ERR_ARG;
   CUDA_TRY(c, cudaSetDevice(c->dev));
-  if (!c->arena) {
+  if (!c->arena.get()) {
     c->arena_bytes = layout_arena(c, nullptr);
-    CUDA_TRY(c, cudaMalloc(&c->arena, c->arena_bytes));
-    layout_arena(c, c->arena);
+    CUDA_TRY(c, cudaMalloc(c->arena.put(), c->arena_bytes));
+    layout_arena(c, c->arena.get());
   }
   return IDC_OK;
 }
@@ -758,31 +772,31 @@ int idc_finalize_weights(idc_ctx* c) {
   if (c->caffe313) {
     const HostTensor* pts = find(c, "caffe.pts_in_hull");
     if (!check_dims(pts, {313, 2})) return fail(c, IDC_ERR_KEY, "missing/bad caffe.pts_in_hull [313,2]");
-    CUDA_TRY(c, cudaMemcpy(c->pts313, pts->data.data(), sizeof(float) * 626, cudaMemcpyHostToDevice));
+    CUDA_TRY(c, cudaMemcpy(c->pts313.get(), pts->data.data(), sizeof(float) * 626, cudaMemcpyHostToDevice));
   }
-  CUDA_TRY(c, cudaMemcpy(c->arena, host.data(), c->arena_bytes, cudaMemcpyHostToDevice));
+  CUDA_TRY(c, cudaMemcpy(c->arena.get(), host.data(), c->arena_bytes, cudaMemcpyHostToDevice));
   return idc_adopt_weights(c);
 }
 
 int idc_adopt_weights(idc_ctx* c) {
-  if (!c || !c->arena) return fail(c, IDC_ERR_STATE, "no arena");
+  if (!c || !c->arena.get()) return fail(c, IDC_ERR_STATE, "no arena");
   CUDA_TRY(c, cudaSetDevice(c->dev));
-  int rc = plan_engines(c);
-  if (rc != IDC_OK) return rc;
   // conv1_1 takes its weights as a kernel parameter: read them back from the (possibly received) arena
   CUDA_TRY(c, cudaMemcpy(c->h_w11.w, c->w11, sizeof(c->h_w11.w), cudaMemcpyDeviceToHost));
   CUDA_TRY(c, cudaMemcpy(c->h_w11.b, c->b11, sizeof(c->h_w11.b), cudaMemcpyDeviceToHost));
   if (!c->simt) CUDA_TRY(c, conv1_1_umma_pack(c));      // tensor-core conv1_1: derived on the device, so ranks != 0 need nothing extra
+  int rc = plan_engines(c);                             // sets weights_ready
+  if (rc != IDC_OK) return rc;
   c->raw.clear();
-  c->weights_ready = true;
-  if (c->graph_exec) { cudaGraphExecDestroy(c->graph_exec); c->graph_exec = nullptr; }
+  c->weights_adopted = true;
+  c->graph_exec.reset();
   return IDC_OK;
 }
 
 int idc_weights_arena(idc_ctx* c, void** dev_ptr, size_t* bytes) {
   if (!c || !dev_ptr || !bytes) return IDC_ERR_ARG;
-  if (!c->arena) return fail(c, IDC_ERR_STATE, "arena not allocated");
-  *dev_ptr = c->arena; *bytes = c->arena_bytes;
+  if (!c->arena.get()) return fail(c, IDC_ERR_STATE, "arena not allocated");
+  *dev_ptr = c->arena.get(); *bytes = c->arena_bytes;
   return IDC_OK;
 }
 
@@ -792,10 +806,8 @@ int idc_forward(idc_ctx* c, int n, int h, int w, const float* L, const float* ab
   int rc = check_forward_args(c, n, h, w, L, ab, mask, glob, out_ab, out_dist);
   if (rc != IDC_OK) return rc;
   CUDA_TRY(c, cudaSetDevice(c->dev));
-  if (int werr = *(volatile int*)c->h_err) {           // left by an earlier (asynchronous) forward
-    *(volatile int*)c->h_err = 0;
-    return fail(c, IDC_ERR_WATCHDOG, "device pipeline watchdog fired earlier (code %d)", werr);
-  }
+  rc = take_watchdog(c, "device pipeline watchdog fired earlier (code %d)");   // left by an earlier (asynchronous) forward
+  if (rc != IDC_OK) return rc;
   return run_forward(c, n, L, ab, mask, maskcent, glob, out_ab, out_dist, out_rgb, (cudaStream_t)stream);
 }
 
@@ -822,19 +834,20 @@ static int forward_host_small(idc_ctx* c, int n, const float* L, const float* ab
                               const float* glob, float* out_ab, float* out_dist, uint8_t* out_rgb, double* out_abq,
                               bool hint_mode) {
   const size_t HW = (size_t)c->H * c->W, HW4 = (size_t)(c->H / 4) * (c->W / 4);
-  cudaStream_t st = c->own_stream;
+  cudaStream_t st = c->own_stream.get();
+  const HostStaging& sg = *c->stage;
   const bool copy_dist = out_dist != nullptr;
   const bool want_dist = copy_dist || (c->dist_resident && c->dist);
   const bool want_rgb = out_rgb != nullptr, want_glob = glob != nullptr, want_q = out_abq != nullptr;
   // compact device layouts for this n
-  float* dL = c->d_in; float* dab = dL + (size_t)n * HW; float* dmask = dab + (size_t)n * 2 * HW;
+  float* dL = sg.d_in.get(); float* dab = dL + (size_t)n * HW; float* dmask = dab + (size_t)n * 2 * HW;
   float* dglob = dmask + (size_t)n * HW;
   const size_t b_ab = (size_t)n * 2 * HW * sizeof(float), b_rgb = (size_t)n * 3 * HW, b_q = (size_t)n * 2 * HW * sizeof(double);
-  char* dsm = c->d_small; char* hsm = c->h_small;
+  char* dsm = sg.d_small.get(); char* hsm = sg.h_small.get();
   float* dout = reinterpret_cast<float*>(dsm);
   uint8_t* drgb = reinterpret_cast<uint8_t*>(dsm + b_ab);
   double* dq = reinterpret_cast<double*>(dsm + b_ab + b_rgb);
-  float* ddist = c->d_out + (size_t)c->max_n * 2 * HW;
+  float* ddist = sg.d_out.get() + (size_t)c->max_n * 2 * HW;
   const size_t out_bytes = b_ab + (want_rgb ? b_rgb : 0) + (want_q ? b_q : 0);
   const uintptr_t flags = (uintptr_t)n | ((uintptr_t)want_dist << 8) | ((uintptr_t)want_rgb << 9) | ((uintptr_t)want_glob << 10) |
                           ((uintptr_t)want_q << 11) | ((uintptr_t)copy_dist << 12) | ((uintptr_t)c->click_mode << 13) |
@@ -844,7 +857,7 @@ static int forward_host_small(idc_ctx* c, int n, const float* L, const float* ab
   const size_t in_floats = (size_t)n * (have_L ? 4 : 3) * HW + (want_glob ? (size_t)n * 316 : 0);
   const void* direct_key[8] = {(void*)(flags | (1u << 16)), L, ab, mask, glob, out_ab, out_rgb, out_abq};
   // fast path: same pinned buffers as the captured graph -> replay without touching the driver's pointer tables
-  bool direct = c->graph_exec && !copy_dist && memcmp(direct_key, c->graph_ptrs, sizeof(direct_key)) == 0 &&
+  bool direct = c->graph_exec.get() && !copy_dist && memcmp(direct_key, c->graph_ptrs, sizeof(direct_key)) == 0 &&
                 c->graph_maskcent == maskcent;
   bool replay = direct;
   if (!direct) {
@@ -855,15 +868,15 @@ static int forward_host_small(idc_ctx* c, int n, const float* L, const float* ab
   const void* staged_key[8] = {(void*)(flags | ((uintptr_t)have_L << 17)), nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
   const void** key = direct ? direct_key : staged_key;
   if (!direct) {   // stage the inputs
-    if (have_L) memcpy(c->h_in, L, (size_t)n * HW * sizeof(float));
+    if (have_L) memcpy(sg.h_in.get(), L, (size_t)n * HW * sizeof(float));
     if (!hint_mode) {
-      memcpy(c->h_in + (size_t)n * HW, ab, (size_t)n * 2 * HW * sizeof(float));
-      memcpy(c->h_in + (size_t)n * 3 * HW, mask, (size_t)n * HW * sizeof(float));
+      memcpy(sg.h_in.get() + (size_t)n * HW, ab, (size_t)n * 2 * HW * sizeof(float));
+      memcpy(sg.h_in.get() + (size_t)n * 3 * HW, mask, (size_t)n * HW * sizeof(float));
     }
-    if (want_glob) memcpy(c->h_in + (size_t)n * 4 * HW, glob, (size_t)n * 316 * sizeof(float));
+    if (want_glob) memcpy(sg.h_in.get() + (size_t)n * 4 * HW, glob, (size_t)n * 316 * sizeof(float));
   }
-  if (!replay && (!c->graph_exec || memcmp(key, c->graph_ptrs, sizeof(staged_key)) != 0 || c->graph_maskcent != maskcent)) {
-    if (c->graph_exec) { cudaGraphExecDestroy(c->graph_exec); c->graph_exec = nullptr; }
+  if (!replay && (!c->graph_exec.get() || memcmp(key, c->graph_ptrs, sizeof(staged_key)) != 0 || c->graph_maskcent != maskcent)) {
+    c->graph_exec.reset();
     cudaGraph_t g = nullptr;
     CUDA_TRY(c, cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
     const bool prof = c->profiling;
@@ -873,9 +886,9 @@ static int forward_host_small(idc_ctx* c, int n, const float* L, const float* ab
       if (ce == cudaSuccess && bytes) ce = cudaMemcpyAsync(dst, src, bytes, kind, st);
     };
     if (hint_mode) {   // the whole hint block (fixed size), then the L planes and the glob vector if they travel
-      cp(c->d_hints, c->h_hints, kHintBlockBytes, cudaMemcpyHostToDevice);
-      if (have_L) cp(dL, direct ? L : c->h_in, (size_t)n * HW * sizeof(float), cudaMemcpyHostToDevice);
-      if (want_glob) cp(dglob, direct ? glob : c->h_in + (size_t)n * 4 * HW, (size_t)n * 316 * sizeof(float), cudaMemcpyHostToDevice);
+      cp(c->hints->d_hints.get(), c->hints->h_hints.get(), kHintBlockBytes, cudaMemcpyHostToDevice);
+      if (have_L) cp(dL, direct ? L : sg.h_in.get(), (size_t)n * HW * sizeof(float), cudaMemcpyHostToDevice);
+      if (want_glob) cp(dglob, direct ? glob : sg.h_in.get() + (size_t)n * 4 * HW, (size_t)n * 316 * sizeof(float), cudaMemcpyHostToDevice);
     } else if (direct) {
       const bool contig = (!have_L || ab == L + (size_t)n * HW) && mask == ab + (size_t)n * 2 * HW &&
                           (!want_glob || glob == mask + (size_t)n * HW);
@@ -889,12 +902,12 @@ static int forward_host_small(idc_ctx* c, int n, const float* L, const float* ab
       }
     } else {
       const size_t off = have_L ? 0 : (size_t)n * HW;
-      cp(c->d_in + off, c->h_in + off, in_floats * sizeof(float), cudaMemcpyHostToDevice);
+      cp(sg.d_in.get() + off, sg.h_in.get() + off, in_floats * sizeof(float), cudaMemcpyHostToDevice);
     }
     int rc = IDC_OK;
     if (ce == cudaSuccess)
       rc = run_forward(c, n, dL, dab, dmask, maskcent, want_glob ? dglob : nullptr, dout, want_dist ? ddist : nullptr,
-                       want_rgb ? drgb : nullptr, st, nullptr, want_q ? dq : nullptr, hint_mode ? c->d_hints : nullptr);
+                       want_rgb ? drgb : nullptr, st, nullptr, want_q ? dq : nullptr, hint_mode ? c->hints->d_hints.get() : nullptr);
     if (rc == IDC_OK) {
       if (direct) {
         const char* o0 = reinterpret_cast<const char*>(out_ab);
@@ -910,7 +923,7 @@ static int forward_host_small(idc_ctx* c, int n, const float* L, const float* ab
       } else {
         cp(hsm, dsm, out_bytes, cudaMemcpyDeviceToHost);
         if (copy_dist)
-          cp(c->h_out + (size_t)c->max_n * 2 * HW, ddist, (size_t)n * 529 * HW4 * sizeof(float), cudaMemcpyDeviceToHost);
+          cp(sg.h_out.get() + (size_t)c->max_n * 2 * HW, ddist, (size_t)n * 529 * HW4 * sizeof(float), cudaMemcpyDeviceToHost);
       }
     }
     c->profiling = prof;
@@ -918,7 +931,7 @@ static int forward_host_small(idc_ctx* c, int n, const float* L, const float* ab
     if (rc != IDC_OK) { if (g) cudaGraphDestroy(g); return rc; }
     if (ce != cudaSuccess) { if (g) cudaGraphDestroy(g); CUDA_TRY(c, ce); }
     CUDA_TRY(c, ce2);
-    ce = cudaGraphInstantiate(&c->graph_exec, g, 0);
+    ce = cudaGraphInstantiate(c->graph_exec.put(), g, 0);
     cudaGraphDestroy(g);
     CUDA_TRY(c, ce);
     c->graph_captures++;
@@ -926,40 +939,42 @@ static int forward_host_small(idc_ctx* c, int n, const float* L, const float* ab
     c->graph_maskcent = maskcent;
     c->graph_launches = c->launch_count;
   }
-  if (c->dbg_graph_timing) CUDA_TRY(c, cudaEventRecord(c->dbg_ev[0], st));
-  CUDA_TRY(c, cudaGraphLaunch(c->graph_exec, st));
-  if (c->dbg_graph_timing) CUDA_TRY(c, cudaEventRecord(c->dbg_ev[1], st));
+  if (c->dbg_graph_timing) CUDA_TRY(c, cudaEventRecord(c->dbg_ev[0].get(), st));
+  CUDA_TRY(c, cudaGraphLaunch(c->graph_exec.get(), st));
+  if (c->dbg_graph_timing) CUDA_TRY(c, cudaEventRecord(c->dbg_ev[1].get(), st));
   c->launch_count = c->graph_launches;
   c->last_n = n;
   CUDA_TRY(c, cudaStreamSynchronize(st));
-  if (c->dbg_graph_timing) cudaEventElapsedTime(&c->dbg_graph_ms, c->dbg_ev[0], c->dbg_ev[1]);
+  if (c->dbg_graph_timing) cudaEventElapsedTime(&c->dbg_graph_ms, c->dbg_ev[0].get(), c->dbg_ev[1].get());
   if (!direct) {
     memcpy(out_ab, hsm, b_ab);
     if (want_rgb) memcpy(out_rgb, hsm + b_ab, b_rgb);
     if (want_q) memcpy(out_abq, hsm + b_ab + b_rgb, b_q);
-    if (copy_dist) memcpy(out_dist, c->h_out + (size_t)c->max_n * 2 * HW, (size_t)n * 529 * HW4 * sizeof(float));
+    if (copy_dist) memcpy(out_dist, sg.h_out.get() + (size_t)c->max_n * 2 * HW, (size_t)n * 529 * HW4 * sizeof(float));
   }
   c->dist_valid_n = want_dist ? n : 0;
-  c->click_served = want_dist && c->click_mode && c->h_clickout;     // the side branch delivered the click's answer
+  c->click_served = want_dist && c->click_mode && c->click;     // the side branch delivered the click's answer
   if (have_L) c->image_n = n;          // the planes just uploaded are the resident image now
   return IDC_OK;
 }
 
 static int ensure_host_staging(idc_ctx* c) {
-  if (c->d_in) return IDC_OK;
+  if (c->stage) return IDC_OK;
   const size_t HW = (size_t)c->H * c->W, HW4 = (size_t)(c->H / 4) * (c->W / 4);
   const int small_n = c->max_n < 4 ? c->max_n : 4;
-  c->in_floats = (size_t)c->max_n * (4 * HW + 316);
-  c->out_floats = (size_t)c->max_n * (2 * HW + (c->dist ? 529 * HW4 : 0));
+  const size_t in_floats = (size_t)c->max_n * (4 * HW + 316);
+  const size_t out_floats = (size_t)c->max_n * (2 * HW + (c->dist ? 529 * HW4 : 0));
   const size_t small_bytes = (size_t)small_n * (2 * HW * 4 + 3 * HW + 2 * HW * 8);
-  CUDA_TRY(c, cudaMalloc(&c->d_in, c->in_floats * sizeof(float)));
-  CUDA_TRY(c, cudaMalloc(&c->d_out, c->out_floats * sizeof(float)));
-  CUDA_TRY(c, cudaMalloc(&c->d_rgb, (size_t)c->max_n * HW * 3));
-  CUDA_TRY(c, cudaMalloc(&c->d_small, small_bytes));
-  CUDA_TRY(c, cudaMallocHost(&c->h_in, c->in_floats * sizeof(float)));
-  CUDA_TRY(c, cudaMallocHost(&c->h_out, c->out_floats * sizeof(float)));
-  CUDA_TRY(c, cudaMallocHost(&c->h_rgb, (size_t)c->max_n * HW * 3));
-  CUDA_TRY(c, cudaMallocHost(&c->h_small, small_bytes));
+  auto g = std::make_unique<HostStaging>();
+  CUDA_TRY(c, cudaMalloc(g->d_in.put(), in_floats * sizeof(float)));
+  CUDA_TRY(c, cudaMalloc(g->d_out.put(), out_floats * sizeof(float)));
+  CUDA_TRY(c, cudaMalloc(g->d_rgb.put(), (size_t)c->max_n * HW * 3));
+  CUDA_TRY(c, cudaMalloc(g->d_small.put(), small_bytes));
+  CUDA_TRY(c, cudaMallocHost(g->h_in.put(), in_floats * sizeof(float)));
+  CUDA_TRY(c, cudaMallocHost(g->h_out.put(), out_floats * sizeof(float)));
+  CUDA_TRY(c, cudaMallocHost(g->h_rgb.put(), (size_t)c->max_n * HW * 3));
+  CUDA_TRY(c, cudaMallocHost(g->h_small.put(), small_bytes));
+  c->stage = std::move(g);
   return IDC_OK;
 }
 
@@ -972,9 +987,9 @@ int idc_set_image(idc_ctx* c, int n, int h, int w, const float* L) {
   int rc = ensure_host_staging(c);
   if (rc != IDC_OK) return rc;
   c->image_n = 0;
-  CUDA_TRY(c, cudaStreamSynchronize(c->own_stream));
+  CUDA_TRY(c, cudaStreamSynchronize(c->own_stream.get()));
   // the L planes sit at the head of the input block for every batch size (small and large path alike)
-  CUDA_TRY(c, cudaMemcpy(c->d_in, L, (size_t)n * c->H * c->W * sizeof(float), cudaMemcpyHostToDevice));
+  CUDA_TRY(c, cudaMemcpy(c->stage->d_in.get(), L, (size_t)n * c->H * c->W * sizeof(float), cudaMemcpyHostToDevice));
   c->image_n = n;
   return IDC_OK;
 }
@@ -983,16 +998,18 @@ int idc_set_hints(idc_ctx* c, int count, const idc_hint* hints) {
   if (!c) return IDC_ERR_ARG;
   if (count < 0 || count > IDC_MAX_HINTS) return fail(c, IDC_ERR_ARG, "count=%d outside [0,%d]", count, IDC_MAX_HINTS);
   if (count && !hints) return fail(c, IDC_ERR_ARG, "null hint list");
-  if (!c->h_hints) {
+  if (!c->hints) {
     CUDA_TRY(c, cudaSetDevice(c->dev));
-    CUDA_TRY(c, cudaMalloc(&c->d_hints, kHintBlockBytes));
-    CUDA_TRY(c, cudaMallocHost(&c->h_hints, kHintBlockBytes));
-    memset(c->h_hints, 0, kHintBlockBytes);
+    auto g = std::make_unique<HintBlock>();
+    CUDA_TRY(c, cudaMalloc(g->d_hints.put(), kHintBlockBytes));
+    CUDA_TRY(c, cudaMallocHost(g->h_hints.put(), kHintBlockBytes));
+    memset(g->h_hints.get(), 0, kHintBlockBytes);
+    c->hints = std::move(g);
   }
   // every idc_forward_host(_q) has synchronised before returning: no copy of the block is in flight
-  int* hdr = reinterpret_cast<int*>(c->h_hints);
-  hdr[0] = count;
-  if (count) memcpy(c->h_hints + kHintHdrBytes, hints, (size_t)count * sizeof(idc_hint));
+  char* block = c->hints->h_hints.get();
+  *reinterpret_cast<int*>(block) = count;
+  if (count) memcpy(block + kHintHdrBytes, hints, (size_t)count * sizeof(idc_hint));
   return IDC_OK;
 }
 
@@ -1006,17 +1023,16 @@ int idc_forward_host_q(idc_ctx* c, int n, int h, int w, const float* L, const fl
   if (out_abq && !out_rgb) return fail(c, IDC_ERR_ARG, "out_abq (quantised ab) is derived from out_rgb: pass both");
   const bool hint_mode = !ab && !mask;
   if (hint_mode) {
-    if (!c->h_hints) return fail(c, IDC_ERR_STATE, "ab and mask are NULL but idc_set_hints was never called");
-    const int count = *reinterpret_cast<const int*>(c->h_hints);
-    const idc_hint* hs = reinterpret_cast<const idc_hint*>(c->h_hints + kHintHdrBytes);
+    if (!c->hints) return fail(c, IDC_ERR_STATE, "ab and mask are NULL but idc_set_hints was never called");
+    const char* block = c->hints->h_hints.get();
+    const int count = *reinterpret_cast<const int*>(block);
+    const idc_hint* hs = reinterpret_cast<const idc_hint*>(block + kHintHdrBytes);
     for (int i = 0; i < count; ++i)
       if (hs[i].img < 0 || hs[i].img >= n) return fail(c, IDC_ERR_ARG, "hint %d: img=%d outside [0,%d)", i, hs[i].img, n);
   }
   CUDA_TRY(c, cudaSetDevice(c->dev));
-  if (int werr = *(volatile int*)c->h_err) {           // a watchdog left over from an asynchronous idc_forward
-    *(volatile int*)c->h_err = 0;
-    return fail(c, IDC_ERR_WATCHDOG, "device pipeline watchdog fired earlier (code %d)", werr);
-  }
+  rc = take_watchdog(c, "device pipeline watchdog fired earlier (code %d)");   // left over from an asynchronous idc_forward
+  if (rc != IDC_OK) return rc;
   const size_t HW = (size_t)c->H * c->W, HW4 = (size_t)(c->H / 4) * (c->W / 4);
   rc = ensure_host_staging(c);
   if (rc != IDC_OK) return rc;
@@ -1025,27 +1041,25 @@ int idc_forward_host_q(idc_ctx* c, int n, int h, int w, const float* L, const fl
   const bool use_graph = !(c->flags & IDC_FLAG_NO_GRAPH) && n <= 4;
   if (use_graph) {
     rc = forward_host_small(c, n, L, ab, mask, maskcent, glob, out_ab, out_dist, out_rgb, out_abq, hint_mode);
-    if (rc != IDC_OK) return rc;
-    if (int werr = *(volatile int*)c->h_err) {
-      *(volatile int*)c->h_err = 0;
-      return fail(c, IDC_ERR_WATCHDOG, "device pipeline watchdog fired (code %d)", werr);
-    }
-    return IDC_OK;
+    return rc != IDC_OK ? rc : take_watchdog(c, "device pipeline watchdog fired (code %d)");
   }
-  if (out_abq && !c->d_abq) {
-    CUDA_TRY(c, cudaMalloc(&c->d_abq, (size_t)c->max_n * 2 * HW * sizeof(double)));
-    CUDA_TRY(c, cudaMallocHost(&c->h_abq, (size_t)c->max_n * 2 * HW * sizeof(double)));
+  if (out_abq && !c->abq) {
+    auto g = std::make_unique<AbqStaging>();
+    CUDA_TRY(c, cudaMalloc(g->d_abq.put(), (size_t)c->max_n * 2 * HW * sizeof(double)));
+    CUDA_TRY(c, cudaMallocHost(g->h_abq.put(), (size_t)c->max_n * 2 * HW * sizeof(double)));
+    c->abq = std::move(g);
   }
-  cudaStream_t st = c->own_stream;
+  cudaStream_t st = c->own_stream.get();
+  const HostStaging& sg = *c->stage;
   // device-side layout of the staging block: [L | ab | mask | glob], [out_ab | out_dist]
-  float* dL = c->d_in; float* dab = dL + (size_t)c->max_n * HW; float* dmask = dab + (size_t)c->max_n * 2 * HW;
+  float* dL = sg.d_in.get(); float* dab = dL + (size_t)c->max_n * HW; float* dmask = dab + (size_t)c->max_n * 2 * HW;
   float* dglob = dmask + (size_t)c->max_n * HW;
-  float* dout = c->d_out; float* ddist = dout + (size_t)c->max_n * 2 * HW;
+  float* dout = sg.d_out.get(); float* ddist = dout + (size_t)c->max_n * 2 * HW;
   auto h2d = [&](float* d, const float* src, size_t count, size_t stage_off) -> cudaError_t {
     const float* s = src;
     if (!is_pinned(src)) {   // pageable caller memory: stage through our pinned block
-      memcpy(c->h_in + stage_off, src, count * sizeof(float));
-      s = c->h_in + stage_off;
+      memcpy(sg.h_in.get() + stage_off, src, count * sizeof(float));
+      s = sg.h_in.get() + stage_off;
     }
     return cudaMemcpyAsync(d, s, count * sizeof(float), cudaMemcpyHostToDevice, st);
   };
@@ -1058,22 +1072,24 @@ int idc_forward_host_q(idc_ctx* c, int n, int h, int w, const float* L, const fl
   if (pipe_on && n >= 8 && fused_head && !last_splits && !c->profiling) {
     hp.nchunks = n >= 32 ? 4 : 2;   // measured: 8 chunks at n = 64 is 1.3 % slower end to end than 4
     for (int k = 0; k <= hp.nchunks; ++k) hp.start[k] = (int)((long long)n * k / hp.nchunks);
-    hp.ab_dst = is_pinned(out_ab) ? out_ab : c->h_out;
-    if (!c->s_in) {
-      CUDA_TRY(c, cudaStreamCreateWithFlags(&c->s_in, cudaStreamNonBlocking));
-      CUDA_TRY(c, cudaStreamCreateWithFlags(&c->s_out, cudaStreamNonBlocking));
+    hp.ab_dst = is_pinned(out_ab) ? out_ab : sg.h_out.get();
+    if (!c->pipe) {
+      auto g = std::make_unique<HostPipeStreams>();
+      CUDA_TRY(c, new_stream(g->s_in));
+      CUDA_TRY(c, new_stream(g->s_out));
       for (int k = 0; k < HostPipe::kMaxChunks; ++k) {
-        CUDA_TRY(c, cudaEventCreateWithFlags(&c->ev_in[k], cudaEventDisableTiming));
-        CUDA_TRY(c, cudaEventCreateWithFlags(&c->ev_out[k], cudaEventDisableTiming));
+        CUDA_TRY(c, new_event(g->ev_in[k]));
+        CUDA_TRY(c, new_event(g->ev_out[k]));
       }
+      c->pipe = std::move(g);
     }
   }
   if (hp.nchunks) {
     cudaStream_t compute = st;
-    st = c->s_in;                                   // the h2d lambda copies on `st`
+    st = c->pipe->s_in.get();                       // the h2d lambda copies on `st`
     if (glob) CUDA_TRY(c, h2d(dglob, glob, (size_t)n * 316, (size_t)c->max_n * 4 * HW));
     // hint mode: the block goes ahead of the first L chunk, so ev_in[0] (which the raster launch waits for) covers it
-    if (hint_mode) CUDA_TRY(c, cudaMemcpyAsync(c->d_hints, c->h_hints, kHintBlockBytes, cudaMemcpyHostToDevice, st));
+    if (hint_mode) CUDA_TRY(c, cudaMemcpyAsync(c->hints->d_hints.get(), c->hints->h_hints.get(), kHintBlockBytes, cudaMemcpyHostToDevice, st));
     for (int k = 0; k < hp.nchunks; ++k) {
       const size_t i0 = hp.start[k], nk = hp.start[k + 1] - hp.start[k];
       if (L) CUDA_TRY(c, h2d(dL + i0 * HW, L + i0 * HW, nk * HW, i0 * HW));
@@ -1081,13 +1097,13 @@ int idc_forward_host_q(idc_ctx* c, int n, int h, int w, const float* L, const fl
         CUDA_TRY(c, h2d(dab + i0 * 2 * HW, ab + i0 * 2 * HW, nk * 2 * HW, (size_t)c->max_n * HW + i0 * 2 * HW));
         CUDA_TRY(c, h2d(dmask + i0 * HW, mask + i0 * HW, nk * HW, (size_t)c->max_n * 3 * HW + i0 * HW));
       }
-      CUDA_TRY(c, cudaEventRecord(c->ev_in[k], c->s_in));
+      CUDA_TRY(c, cudaEventRecord(c->pipe->ev_in[k].get(), st));
     }
     st = compute;
   } else {
     if (L) CUDA_TRY(c, h2d(dL, L, n * HW, 0));
     if (hint_mode) {
-      CUDA_TRY(c, cudaMemcpyAsync(c->d_hints, c->h_hints, kHintBlockBytes, cudaMemcpyHostToDevice, st));
+      CUDA_TRY(c, cudaMemcpyAsync(c->hints->d_hints.get(), c->hints->h_hints.get(), kHintBlockBytes, cudaMemcpyHostToDevice, st));
     } else {
       CUDA_TRY(c, h2d(dab, ab, n * 2 * HW, (size_t)c->max_n * HW));
       CUDA_TRY(c, h2d(dmask, mask, n * HW, (size_t)c->max_n * 3 * HW));
@@ -1099,30 +1115,27 @@ int idc_forward_host_q(idc_ctx* c, int n, int h, int w, const float* L, const fl
   const bool want_dist = copy_dist || (c->dist_resident && c->dist);
   const bool want_rgb = out_rgb != nullptr, want_glob = glob != nullptr;
   rc = run_forward(c, n, dL, dab, dmask, maskcent, want_glob ? dglob : nullptr, dout, want_dist ? ddist : nullptr,
-                   want_rgb ? c->d_rgb : nullptr, st, hp.nchunks ? &hp : nullptr, out_abq ? c->d_abq : nullptr,
-                   hint_mode ? c->d_hints : nullptr);
+                   want_rgb ? sg.d_rgb.get() : nullptr, st, hp.nchunks ? &hp : nullptr, out_abq ? c->abq->d_abq.get() : nullptr,
+                   hint_mode ? c->hints->d_hints.get() : nullptr);
   if (rc != IDC_OK) return rc;
   auto d2h = [&](void* dst, const void* d, size_t bytes, void* stage) -> cudaError_t {
     if (is_pinned(dst)) return cudaMemcpyAsync(dst, d, bytes, cudaMemcpyDeviceToHost, st);
     return cudaMemcpyAsync(stage, d, bytes, cudaMemcpyDeviceToHost, st);
   };
-  if (!hp.nchunks) CUDA_TRY(c, d2h(out_ab, dout, n * 2 * HW * sizeof(float), c->h_out));
-  if (copy_dist) CUDA_TRY(c, d2h(out_dist, ddist, n * 529 * HW4 * sizeof(float), c->h_out + (size_t)c->max_n * 2 * HW));
-  if (want_rgb) CUDA_TRY(c, d2h(out_rgb, c->d_rgb, n * HW * 3, c->h_rgb));
-  if (out_abq) CUDA_TRY(c, d2h(out_abq, c->d_abq, n * 2 * HW * sizeof(double), c->h_abq));
+  float* h_out = sg.h_out.get();
+  if (!hp.nchunks) CUDA_TRY(c, d2h(out_ab, dout, n * 2 * HW * sizeof(float), h_out));
+  if (copy_dist) CUDA_TRY(c, d2h(out_dist, ddist, n * 529 * HW4 * sizeof(float), h_out + (size_t)c->max_n * 2 * HW));
+  if (want_rgb) CUDA_TRY(c, d2h(out_rgb, sg.d_rgb.get(), n * HW * 3, sg.h_rgb.get()));
+  if (out_abq) CUDA_TRY(c, d2h(out_abq, c->abq->d_abq.get(), n * 2 * HW * sizeof(double), c->abq->h_abq.get()));
   CUDA_TRY(c, cudaStreamSynchronize(st));
-  if (hp.nchunks) CUDA_TRY(c, cudaStreamSynchronize(c->s_out));
+  if (hp.nchunks) CUDA_TRY(c, cudaStreamSynchronize(c->pipe->s_out.get()));
   if (L) c->image_n = n;
-  if (!is_pinned(out_ab)) memcpy(out_ab, c->h_out, n * 2 * HW * sizeof(float));
-  if (copy_dist && !is_pinned(out_dist)) memcpy(out_dist, c->h_out + (size_t)c->max_n * 2 * HW, n * 529 * HW4 * sizeof(float));
+  if (!is_pinned(out_ab)) memcpy(out_ab, h_out, n * 2 * HW * sizeof(float));
+  if (copy_dist && !is_pinned(out_dist)) memcpy(out_dist, h_out + (size_t)c->max_n * 2 * HW, n * 529 * HW4 * sizeof(float));
   c->dist_valid_n = want_dist ? n : 0;
-  if (want_rgb && !is_pinned(out_rgb)) memcpy(out_rgb, c->h_rgb, n * HW * 3);
-  if (out_abq && !is_pinned(out_abq)) memcpy(out_abq, c->h_abq, n * 2 * HW * sizeof(double));
-  if (int werr = *(volatile int*)c->h_err) {
-    *(volatile int*)c->h_err = 0;
-    return fail(c, IDC_ERR_WATCHDOG, "device pipeline watchdog fired (code %d)", werr);
-  }
-  return IDC_OK;
+  if (want_rgb && !is_pinned(out_rgb)) memcpy(out_rgb, sg.h_rgb.get(), n * HW * 3);
+  if (out_abq && !is_pinned(out_abq)) memcpy(out_abq, c->abq->h_abq.get(), n * 2 * HW * sizeof(double));
+  return take_watchdog(c, "device pipeline watchdog fired (code %d)");
 }
 
 void* idc_host_alloc(size_t bytes) {
@@ -1145,8 +1158,8 @@ int idc_set_dist_resident(idc_ctx* c, int on) {
 
 // does the pinned click block hold the answer for this pixel?
 static bool click_answers(idc_ctx* c, int img, int y4, int x4) {
-  if (!c->click_served || !c->h_clickout) return false;
-  const int* hdr = reinterpret_cast<const int*>(c->h_clickout);
+  if (!c->click_served || !c->click) return false;
+  const int* hdr = reinterpret_cast<const int*>(c->click->h_clickout.get());
   return hdr[7] == 1 && hdr[0] == img && hdr[1] == y4 && hdr[2] == x4;
 }
 
@@ -1155,20 +1168,22 @@ int idc_set_click(idc_ctx* c, int img, int y4, int x4, int K) {
   if (!c->dist) return fail(c, IDC_ERR_ARG, "idc_set_click requires IDC_FLAG_DIST");
   if (K < 0 || K > 32) return fail(c, IDC_ERR_ARG, "idc_set_click: need 0 <= K <= 32");
   CUDA_TRY(c, cudaSetDevice(c->dev));
-  if (!c->h_click) {
-    CUDA_TRY(c, cudaHostAlloc(&c->h_click, 64, cudaHostAllocMapped));
-    memset(c->h_click, 0, 64);
-    c->h_click[1] = -1;
-    CUDA_TRY(c, cudaHostGetDevicePointer(&c->d_click, c->h_click, 0));
-    CUDA_TRY(c, cudaMalloc(&c->d_clickout, kClickBytes));
-    CUDA_TRY(c, cudaMemset(c->d_clickout, 0, kClickBytes));
-    CUDA_TRY(c, cudaMallocHost(&c->h_clickout, kClickCopy));
-    memset(c->h_clickout, 0, kClickCopy);
+  if (!c->click) {
+    auto g = std::make_unique<ClickBlock>();
+    CUDA_TRY(c, cudaHostAlloc(g->h_click.put(), 64, cudaHostAllocMapped));
+    memset(g->h_click.get(), 0, 64);
+    g->h_click.get()[1] = -1;
+    CUDA_TRY(c, cudaHostGetDevicePointer(&g->d_click, g->h_click.get(), 0));
+    CUDA_TRY(c, cudaMalloc(g->d_clickout.put(), kClickBytes));
+    CUDA_TRY(c, cudaMemset(g->d_clickout.get(), 0, kClickBytes));
+    CUDA_TRY(c, cudaMallocHost(g->h_clickout.put(), kClickCopy));
+    memset(g->h_clickout.get(), 0, kClickCopy);
     float pts[529 * 2];   // the PyTorch wrapper's gamut grid (data/colorize_image.py:283): bin i = (g[i % 23], g[i / 23])
     for (int i = 0; i < 529; ++i) { pts[2 * i] = -110.f + 10.f * (i % 23); pts[2 * i + 1] = -110.f + 10.f * (i / 23); }
-    CUDA_TRY(c, cudaMemcpy(c->d_clickout + kClickCopy, pts, sizeof(pts), cudaMemcpyHostToDevice));
+    CUDA_TRY(c, cudaMemcpy(g->d_clickout.get() + kClickCopy, pts, sizeof(pts), cudaMemcpyHostToDevice));
+    c->click = std::move(g);
   }
-  volatile int* h = c->h_click;
+  volatile int* h = c->click->h_click.get();
   h[0] = img; h[1] = y4; h[2] = x4; h[3] = K; h[4] = h[4] + 1;
   c->click_mode = y4 >= 0;           // part of the graph key: switching the mode re-captures the click graph once
   c->click_served = false;
@@ -1177,11 +1192,11 @@ int idc_set_click(idc_ctx* c, int img, int y4, int x4, int K) {
 
 int idc_fetch_dist(idc_ctx* c, int img, int y4, int x4, float* out) {
   if (!c || !out) return IDC_ERR_ARG;
-  if (img < 0 || img >= c->dist_valid_n || !c->d_out)
+  if (img < 0 || img >= c->dist_valid_n || !c->stage)
     return fail(c, IDC_ERR_STATE, "no resident distribution for image %d (run idc_forward_host with resident mode on)", img);
   const int H4 = c->H / 4, W4 = c->W / 4;
   const size_t HW = (size_t)c->H * c->W, HW4 = (size_t)H4 * W4;
-  const float* d = c->d_out + (size_t)c->max_n * 2 * HW + (size_t)img * 529 * HW4;
+  const float* d = c->stage->d_out.get() + (size_t)c->max_n * 2 * HW + (size_t)img * 529 * HW4;
   CUDA_TRY(c, cudaSetDevice(c->dev));
   if (y4 < 0) {
     CUDA_TRY(c, cudaMemcpy(out, d, 529 * HW4 * sizeof(float), cudaMemcpyDeviceToHost));
@@ -1189,7 +1204,7 @@ int idc_fetch_dist(idc_ctx* c, int img, int y4, int x4, float* out) {
   }
   if (y4 >= H4 || x4 < 0 || x4 >= W4) return fail(c, IDC_ERR_ARG, "pixel (%d,%d) outside the %dx%d grid", y4, x4, H4, W4);
   if (click_answers(c, img, y4, x4)) {       // idc_set_click: the forward already brought this pixel back
-    memcpy(out, c->h_clickout + kClickHdr, 529 * sizeof(float));
+    memcpy(out, c->click->h_clickout.get() + kClickHdr, 529 * sizeof(float));
     return IDC_OK;
   }
   // one float per bin, bins are HW4 floats apart (NCHW)
@@ -1244,14 +1259,15 @@ int idc_ab_reccs(idc_ctx* c, int img, int y4, int x4, int K, int max_iter, int n
   if (!c || !centers_host) return IDC_ERR_ARG;
   if (!reccs_args_ok(K, max_iter, n_init))
     return fail(c, IDC_ERR_ARG, "idc_ab_reccs: need 1 <= K <= 32, max_iter >= 1, 1 <= n_init <= %d", kReccsMaxInit);
-  if (img < 0 || img >= c->dist_valid_n || !c->d_out)
+  if (img < 0 || img >= c->dist_valid_n || !c->stage)
     return fail(c, IDC_ERR_STATE, "no resident distribution for image %d (run idc_forward_host with resident mode on)", img);
   const int H4 = c->H / 4, W4 = c->W / 4;
   if (y4 < 0 || y4 >= H4 || x4 < 0 || x4 >= W4) return fail(c, IDC_ERR_ARG, "pixel (%d,%d) outside the %dx%d grid", y4, x4, H4, W4);
   const size_t HW = (size_t)c->H * c->W, HW4 = (size_t)H4 * W4;
   // idc_set_click with the same pixel and K, default restarts / iterations / gamut grid: the click graph already
   // clustered this pmf on its side branch and the results are in pinned host memory
-  if (click_answers(c, img, y4, x4) && reinterpret_cast<const int*>(c->h_clickout)[3] == K && max_iter == kClickMaxIter &&
+  const char* clickout = c->click ? c->click->h_clickout.get() : nullptr;
+  if (click_answers(c, img, y4, x4) && reinterpret_cast<const int*>(clickout)[3] == K && max_iter == kClickMaxIter &&
       n_init == kClickInit) {
     bool default_pts = pts_host == nullptr;
     if (!default_pts) {
@@ -1260,15 +1276,15 @@ int idc_ab_reccs(idc_ctx* c, int img, int y4, int x4, int K, int max_iter, int n
         default_pts = pts_host[2 * i] == -110.f + 10.f * (i % 23) && pts_host[2 * i + 1] == -110.f + 10.f * (i / 23);
     }
     if (default_pts) {
-      reccs_pick(reinterpret_cast<const double*>(c->h_clickout + kClickHdr + kClickPmf), K, n_init, centers_host, conf_host,
+      reccs_pick(reinterpret_cast<const double*>(clickout + kClickHdr + kClickPmf), K, n_init, centers_host, conf_host,
                  iters_out);
       return IDC_OK;
     }
   }
-  const float* d = c->d_out + (size_t)c->max_n * 2 * HW + (size_t)img * 529 * HW4 + (size_t)y4 * W4 + x4;
+  const float* d = c->stage->d_out.get() + (size_t)c->max_n * 2 * HW + (size_t)img * 529 * HW4 + (size_t)y4 * W4 + x4;
   CUDA_TRY(c, cudaSetDevice(c->dev));
-  if (!c->d_reccs) CUDA_TRY(c, cudaMalloc(&c->d_reccs, kReccsScratchBytes));
-  CUDA_TRY(c, reccs_run(d, HW4, c->d_reccs, K, max_iter, n_init, pts_host, centers_host, conf_host, iters_out));
+  if (!c->d_reccs.get()) CUDA_TRY(c, cudaMalloc(c->d_reccs.put(), kReccsScratchBytes));
+  CUDA_TRY(c, reccs_run(d, HW4, c->d_reccs.get(), K, max_iter, n_init, pts_host, centers_host, conf_host, iters_out));
   return IDC_OK;
 }
 
@@ -1276,13 +1292,13 @@ int idc_ab_reccs_pmf(int device, const float* pmf_host, int K, int max_iter, int
                      float* centers_host, float* conf_host, int* iters_out) {
   if (!pmf_host || !centers_host || !reccs_args_ok(K, max_iter, n_init)) return IDC_ERR_ARG;
   if (cudaSetDevice(device) != cudaSuccess) return IDC_ERR_CUDA;
-  char* buf = nullptr;
-  if (cudaMalloc(&buf, kReccsScratchBytes + 529 * sizeof(float)) != cudaSuccess) return IDC_ERR_CUDA;
-  float* pmf_dev = reinterpret_cast<float*>(buf + kReccsScratchBytes);
+  DevMem<char> buf;
+  if (cudaMalloc(buf.put(), kReccsScratchBytes + 529 * sizeof(float)) != cudaSuccess) return IDC_ERR_CUDA;
+  float* pmf_dev = reinterpret_cast<float*>(buf.get() + kReccsScratchBytes);
   cudaError_t e = cudaMemcpy(pmf_dev, pmf_host, 529 * sizeof(float), cudaMemcpyHostToDevice);
   if (e == cudaSuccess)
-    e = reccs_run(pmf_dev, 1, reinterpret_cast<double*>(buf), K, max_iter, n_init, pts_host, centers_host, conf_host, iters_out);
-  cudaFree(buf);
+    e = reccs_run(pmf_dev, 1, reinterpret_cast<double*>(buf.get()), K, max_iter, n_init, pts_host, centers_host, conf_host,
+                  iters_out);
   return e == cudaSuccess ? IDC_OK : IDC_ERR_CUDA;
 }
 
@@ -1298,12 +1314,9 @@ int idc_caffe313_dist_pixel(idc_ctx* c, int img, int y, int x, float S, float* o
   if (!c || !out313_host || img < 0 || img >= c->max_n || y < 0 || y >= c->H || x < 0 || x >= c->W) return IDC_ERR_ARG;
   if (!c->caffe313) return fail(c, IDC_ERR_STATE, "ctx was not created with IDC_FLAG_CAFFE313");
   CUDA_TRY(c, cudaSetDevice(c->dev));
-  float* d = nullptr;
-  CUDA_TRY(c, cudaMalloc(&d, 320 * sizeof(float)));
-  cudaError_t e = launch_dist313_pixel(c, img, y, x, S, d, 0);
-  if (e == cudaSuccess) e = cudaMemcpy(out313_host, d, 313 * sizeof(float), cudaMemcpyDeviceToHost);
-  cudaFree(d);
-  CUDA_TRY(c, e);
+  if (!c->d_dist313.get()) CUDA_TRY(c, cudaMalloc(c->d_dist313.put(), 320 * sizeof(float)));
+  CUDA_TRY(c, launch_dist313_pixel(c, img, y, x, S, c->d_dist313.get(), 0));
+  CUDA_TRY(c, cudaMemcpy(out313_host, c->d_dist313.get(), 313 * sizeof(float), cudaMemcpyDeviceToHost));
   return IDC_OK;
 }
 
@@ -1323,14 +1336,14 @@ int idc_negentropy(int device, int n, int bins, int hw, const float* dist, float
 
 int idc_dist_negentropy(idc_ctx* c, int img, float* out_host) {
   if (!c || !out_host) return IDC_ERR_ARG;
-  if (img < 0 || img >= c->dist_valid_n || !c->d_out)
+  if (img < 0 || img >= c->dist_valid_n || !c->stage)
     return fail(c, IDC_ERR_STATE, "no resident distribution for image %d (run idc_forward_host with resident mode on)", img);
   const size_t HW = (size_t)c->H * c->W, HW4 = (size_t)(c->H / 4) * (c->W / 4);
-  const float* d = c->d_out + (size_t)c->max_n * 2 * HW + (size_t)img * 529 * HW4;
+  const float* d = c->stage->d_out.get() + (size_t)c->max_n * 2 * HW + (size_t)img * 529 * HW4;
   CUDA_TRY(c, cudaSetDevice(c->dev));
-  if (!c->d_negent) CUDA_TRY(c, cudaMalloc(&c->d_negent, HW4 * sizeof(float)));
-  CUDA_TRY(c, launch_negentropy(1, 529, (int)HW4, d, c->d_negent, 0));
-  CUDA_TRY(c, cudaMemcpy(out_host, c->d_negent, HW4 * sizeof(float), cudaMemcpyDeviceToHost));
+  if (!c->d_negent.get()) CUDA_TRY(c, cudaMalloc(c->d_negent.put(), HW4 * sizeof(float)));
+  CUDA_TRY(c, launch_negentropy(1, 529, (int)HW4, d, c->d_negent.get(), 0));
+  CUDA_TRY(c, cudaMemcpy(out_host, c->d_negent.get(), HW4 * sizeof(float), cudaMemcpyDeviceToHost));
   return IDC_OK;
 }
 
@@ -1446,22 +1459,20 @@ int idc_get_profile(idc_ctx* c, float* ms, int max_slots) {
   if (max_slots < slots) return fail(c, IDC_ERR_ARG, "need %d slots", slots);
   CUDA_TRY(c, cudaSetDevice(c->dev));
   CUDA_TRY(c, cudaDeviceSynchronize());
-  if (int werr = *(volatile int*)c->h_err) {
-    *(volatile int*)c->h_err = 0;
-    return fail(c, IDC_ERR_WATCHDOG, "device pipeline watchdog fired (code %d)", werr);
-  }
+  const int rc = take_watchdog(c, "device pipeline watchdog fired (code %d)");
+  if (rc != IDC_OK) return rc;
   for (int i = 0; i < slots; ++i) ms[i] = 0.f;
   int runs = 0;
   for (auto& ev : c->prof_runs) {
     if ((int)ev.size() == slots + 1) {
       for (int i = 0; i < slots; ++i) {
         float t = 0.f;
-        cudaEventElapsedTime(&t, ev[i], ev[i + 1]);
+        cudaEventElapsedTime(&t, ev[i].get(), ev[i + 1].get());
         ms[i] += t;
       }
       runs++;
     }
-    for (cudaEvent_t e : ev) c->prof_pool.push_back(e);
+    for (Event& e : ev) c->prof_pool.push_back(std::move(e));
   }
   c->prof_runs.clear();
   if (runs) for (int i = 0; i < slots; ++i) ms[i] /= runs;
@@ -1477,11 +1488,14 @@ double idc_op_flops(idc_ctx* c, int i) {
 extern "C" int idc_debug_graph_timing(idc_ctx* c, int enable, float* ms) {
   if (!c) return IDC_ERR_ARG;
   CUDA_TRY(c, cudaSetDevice(c->dev));
-  if (enable && !c->dbg_ev[0]) {
-    CUDA_TRY(c, cudaEventCreate(&c->dbg_ev[0]));
-    CUDA_TRY(c, cudaEventCreate(&c->dbg_ev[1]));
+  if (enable && !c->dbg_ev[0].get()) {
+    Event ev[2];
+    CUDA_TRY(c, cudaEventCreate(ev[0].put()));
+    CUDA_TRY(c, cudaEventCreate(ev[1].put()));
+    c->dbg_ev[0] = std::move(ev[0]);
+    c->dbg_ev[1] = std::move(ev[1]);
   }
-  c->dbg_graph_timing = enable != 0 && c->dbg_ev[0];
+  c->dbg_graph_timing = enable != 0 && c->dbg_ev[0].get();
   if (ms) *ms = c->dbg_graph_ms;
   return IDC_OK;
 }
@@ -1506,46 +1520,6 @@ int idc_destroy(idc_ctx* c) {
   if (!c) return IDC_ERR_ARG;
   cudaSetDevice(c->dev);
   cudaDeviceSynchronize();
-  if (c->graph_exec) cudaGraphExecDestroy(c->graph_exec);
-  for (auto& op : c->ops) umma_free_op(op);
-  for (auto& ev : c->prof_runs) for (cudaEvent_t e : ev) cudaEventDestroy(e);
-  for (cudaEvent_t e : c->prof_pool) cudaEventDestroy(e);
-  for (auto& b : c->bufs) { if (b.p0) cudaFree(b.p0); if (b.p1) cudaFree(b.p1); }
-  if (c->arena) cudaFree(c->arena);
-  if (c->logits) cudaFree(c->logits);
-  if (c->logits313) cudaFree(c->logits313);
-  if (c->pts313) cudaFree(c->pts313);
-  if (c->splitk_ws) cudaFree(c->splitk_ws);
-  if (c->splitk_counters) cudaFree(c->splitk_counters);
-  if (c->w11_umma) cudaFree(c->w11_umma);
-  if (c->d_reccs) cudaFree(c->d_reccs);
-  if (c->d_negent) cudaFree(c->d_negent);
-  if (c->gvec) cudaFree(c->gvec);
-  if (c->gtmp) cudaFree(c->gtmp);
-  if (c->h_err) cudaFreeHost(c->h_err);
-  if (c->d_in) cudaFree(c->d_in);
-  if (c->d_out) cudaFree(c->d_out);
-  if (c->d_rgb) cudaFree(c->d_rgb);
-  if (c->d_small) cudaFree(c->d_small);
-  if (c->h_small) cudaFreeHost(c->h_small);
-  if (c->d_abq) cudaFree(c->d_abq);
-  if (c->h_abq) cudaFreeHost(c->h_abq);
-  if (c->h_in) cudaFreeHost(c->h_in);
-  if (c->h_out) cudaFreeHost(c->h_out);
-  if (c->h_rgb) cudaFreeHost(c->h_rgb);
-  if (c->h_click) cudaFreeHost(c->h_click);
-  if (c->d_clickout) cudaFree(c->d_clickout);
-  if (c->h_clickout) cudaFreeHost(c->h_clickout);
-  if (c->h_hints) cudaFreeHost(c->h_hints);
-  if (c->d_hints) cudaFree(c->d_hints);
-  if (c->dbg_ev[0]) { cudaEventDestroy(c->dbg_ev[0]); cudaEventDestroy(c->dbg_ev[1]); }
-  if (c->own_stream) cudaStreamDestroy(c->own_stream);
-  if (c->s_click) { cudaStreamDestroy(c->s_click); cudaEventDestroy(c->ev_click[0]); cudaEventDestroy(c->ev_click[1]); }
-  if (c->s_side) { cudaStreamDestroy(c->s_side); cudaEventDestroy(c->ev_fork); cudaEventDestroy(c->ev_join); }
-  if (c->s_in) {
-    cudaStreamDestroy(c->s_in); cudaStreamDestroy(c->s_out);
-    for (int k = 0; k < HostPipe::kMaxChunks; ++k) { cudaEventDestroy(c->ev_in[k]); cudaEventDestroy(c->ev_out[k]); }
-  }
   delete c;
   return IDC_OK;
 }

@@ -8,12 +8,37 @@
 #include <stdint.h>
 
 #include <map>
+#include <memory>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/idc_b200.h"
 
 namespace idc {
+
+// ---- owners of CUDA handles ----
+// Move-only; the destructor releases the handle.  Readers take the raw handle with get(); put() releases the current
+// handle and returns the address a cudaMalloc* / cuda*Create call writes the new one to.  HostMem also owns mapped
+// cudaHostAlloc blocks; their device alias is a plain pointer kept beside the owner.
+template <typename H, auto Release>
+class Owner {
+ public:
+  Owner() = default;
+  Owner(Owner&& o) noexcept { std::swap(h_, o.h_); }
+  Owner& operator=(Owner&& o) noexcept { std::swap(h_, o.h_); return *this; }
+  ~Owner() { reset(); }
+  H get() const { return h_; }
+  H* put() { reset(); return &h_; }
+  void reset() { if (h_) Release(h_); h_ = nullptr; }
+ private:
+  H h_ = nullptr;
+};
+template <typename T> using DevMem = Owner<T*, cudaFree>;
+template <typename T> using HostMem = Owner<T*, cudaFreeHost>;
+using Stream = Owner<cudaStream_t, cudaStreamDestroy>;
+using Event = Owner<cudaEvent_t, cudaEventDestroy>;
+using GraphExec = Owner<cudaGraphExec_t, cudaGraphExecDestroy>;
 
 constexpr int kMaxTaps = 34;  // up-layer: 4 deconv + 9 shortcut taps; Caffe hyper-column: 4x4 deconv + 2x9 conv taps
 constexpr int kMaxSrc = 6;
@@ -43,8 +68,7 @@ struct Tap {
 struct ActBuf {
   std::string name;
   int H = 0, W = 0, C = 0;
-  void* p0 = nullptr;
-  void* p1 = nullptr;
+  DevMem<void> p0, p1;
 };
 
 // Per-output-channel epilogue vectors (device, fp32[cout_pad]).
@@ -68,6 +92,9 @@ struct SrcDesc {
 };
 
 enum OpKind { OP_CONV = 0, OP_UP = 1, OP_CLASS = 2, OP_HYPER = 3 };
+
+struct UmmaPlan;                                                 // idc_umma.cu
+struct UmmaPlanFree { void operator()(UmmaPlan* p) const; };
 
 struct ConvOp {
   std::string name;
@@ -96,7 +123,7 @@ struct ConvOp {
   __half* w_lo = nullptr;
   // wgmma launch plan (filled by umma_plan_op)
   int bn_tile = 0, hbox = 0, wbox = 0;
-  void* umma_plan = nullptr;
+  std::unique_ptr<UmmaPlan, UmmaPlanFree> umma_plan;
   double flops_per_image = 0;
 };
 
@@ -127,8 +154,31 @@ struct HostTensor {
   std::vector<int64_t> dims;
 };
 
+// Resources a context creates at first use, one group at a time.  A group is built into a local and moved into the
+// context only when every allocation in it succeeded, so the context holds it whole or not at all.
+struct HostStaging {   // idc_forward_host / idc_set_image: [L | ab | mask | glob] in, [out_ab | out_dist] out
+  DevMem<float> d_in, d_out; HostMem<float> h_in, h_out;
+  DevMem<uint8_t> d_rgb; HostMem<uint8_t> h_rgb;
+  DevMem<char> d_small; HostMem<char> h_small;   // compact [ab | rgb | quantised ab] block of the batch <= 4 graph path
+};
+struct AbqStaging { DevMem<double> d_abq; HostMem<double> h_abq; };   // quantised ab (row a11) of the large-batch path
+// idc_set_hints: [kHintHdrBytes header (int count) | IDC_MAX_HINTS x idc_hint], pinned host + device copy
+struct HintBlock { HostMem<char> h_hints; DevMem<char> d_hints; };
+// idc_set_click: the clicked pixel's pmf + K colour suggestions ride on a side branch of the click graph
+struct ClickBlock {
+  HostMem<int> h_click; int* d_click = nullptr;   // {img, y4, x4, K, seq} in mapped host memory, read when the graph runs
+  DevMem<char> d_clickout; HostMem<char> h_clickout;   // [8-int header | 544 floats pmf | n_init x (3K+2) doubles]
+};
+// dist head off the critical path: class + softmax run on s_side next to decoder levels 9-10; the announced click's
+// pmf + suggestions run on s_click, next to the full-map softmax
+struct SideBranch { Stream s_side, s_click; Event ev_fork, ev_join, ev_click[2]; };
+// idc_forward_host pipeline (large batches): H2D of image chunk k+1 overlaps conv1_1 of chunk k, D2H of ab
+// chunk k overlaps the last op of chunk k+1
+struct HostPipeStreams { Stream s_in, s_out; Event ev_in[8], ev_out[8]; };
+
 struct Ctx {
   int dev = 0;
+  int num_sms = 0;                           // of dev, read once by idc_create
   int max_n = 0, H = 0, W = 0;
   unsigned flags = 0;
   Options opt;
@@ -138,14 +188,15 @@ struct Ctx {
   std::map<std::string, int> buf_index;
   std::vector<ConvOp> ops;
   // weight arena
-  char* arena = nullptr;
+  DevMem<char> arena;
   size_t arena_bytes = 0;
-  bool weights_ready = false;
+  bool weights_ready = false;     // adopted and planned: forwards may run
+  bool weights_adopted = false;   // idc_adopt_weights succeeded and no tensor was loaded since: option changes re-plan
   // conv1_1 (4->64) + regression head + misc small weights (device fp32)
   float* w11 = nullptr;   // [36][64]  k = tap*4 + cin
   float* b11 = nullptr;   // [64]
   Conv11Weights h_w11;    // host copy passed by value to conv1_1_kernel
-  uint8_t* w11_umma = nullptr;   // conv1_1_umma_kernel: swizzled hi/lo weight tile + bias' / scale' (device, derived)
+  DevMem<uint8_t> w11_umma;   // conv1_1_umma_kernel: swizzled hi/lo weight tile + bias' / scale' (device, derived)
   float* wout = nullptr;  // [2][128]
   float* bout = nullptr;  // [2]
   // global hints MLP (device fp32)
@@ -153,43 +204,31 @@ struct Ctx {
   float* gb[4] = {nullptr, nullptr, nullptr, nullptr};
   float* gscale[4] = {nullptr, nullptr, nullptr, nullptr};
   float* gshift[4] = {nullptr, nullptr, nullptr, nullptr};
-  float* gvec = nullptr;   // [max_n][512]
-  float* gtmp = nullptr;   // [2][max_n][512]
+  DevMem<float> gvec;   // [max_n][512]
+  DevMem<float> gtmp;   // [2][max_n][512]
   // workspace
-  float* logits = nullptr;     // [max_n*(H/4)*(W/4)][cout_pad(529)]
-  float* logits313 = nullptr;  // Caffe-spec head: [max_n*(H/4)*(W/4)][320]
+  DevMem<float> logits;      // [max_n*(H/4)*(W/4)][cout_pad(529)]
+  DevMem<float> logits313;   // Caffe-spec head: [max_n*(H/4)*(W/4)][320]
   bool caffe313 = false;
-  float* pts313 = nullptr;     // [313][2] ab bin centres (device)
+  DevMem<float> pts313;      // [313][2] ab bin centres (device)
   // split-K workspace of the wgmma engine (sized by umma_plan_op, allocated after planning)
-  float* splitk_ws = nullptr; size_t splitk_ws_floats = 0;
-  int* splitk_counters = nullptr; int splitk_max_tiles = 0;
+  DevMem<float> splitk_ws; size_t splitk_ws_floats = 0;
+  DevMem<int> splitk_counters; int splitk_max_tiles = 0;
   bool dbg_graph_timing = false; // experiments: events around the click graph launch (idc_debug_graph_timing)
-  cudaEvent_t dbg_ev[2] = {nullptr, nullptr};
+  Event dbg_ev[2];
   float dbg_graph_ms = 0.f;
-  int* d_err = nullptr;        // watchdog flag (mapped pinned host memory: survives a device trap)
-  int* h_err = nullptr;
-  // staging for idc_forward_host
-  float* h_in = nullptr;  float* d_in = nullptr;   size_t in_floats = 0;
-  float* h_out = nullptr; float* d_out = nullptr;  size_t out_floats = 0;
-  uint8_t* h_rgb = nullptr; uint8_t* d_rgb = nullptr;
-  char* h_small = nullptr; char* d_small = nullptr;   // compact [ab | rgb | quantised ab] block of the batch <= 4 graph path
-  double* h_abq = nullptr; double* d_abq = nullptr;   // quantised ab (row a11) of the large-batch path
-  cudaStream_t own_stream = nullptr;
-  // idc_forward_host pipeline (large batches): H2D of image chunk k+1 overlaps conv1_1 of chunk k, D2H of ab
-  // chunk k overlaps the last op of chunk k+1
-  cudaStream_t s_in = nullptr, s_out = nullptr;
-  // dist head off the critical path: class + softmax run on a side stream next to decoder levels 9-10
-  cudaStream_t s_side = nullptr;
-  cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
-  cudaStream_t s_click = nullptr;            // announced click: pmf + suggestions next to the full-map softmax
-  cudaEvent_t ev_click[2] = {nullptr, nullptr};
+  HostMem<int> h_err;          // watchdog flag (mapped pinned host memory: survives a device trap)
+  int* d_err = nullptr;
+  std::unique_ptr<HostStaging> stage;
+  std::unique_ptr<AbqStaging> abq;
+  Stream own_stream;
+  std::unique_ptr<HostPipeStreams> pipe;
+  std::unique_ptr<SideBranch> side;
   int image_n = 0;                           // idc_set_image: this many L planes are resident at the head of d_in
-  // idc_set_hints: [kHintHdrBytes header (int count) | IDC_MAX_HINTS x idc_hint], pinned host + device copy
-  char* h_hints = nullptr; char* d_hints = nullptr;
+  std::unique_ptr<HintBlock> hints;
   int graph_captures = 0;                    // click-graph instantiations (idc_graph_captures)
-  cudaEvent_t ev_in[8] = {}, ev_out[8] = {};
   // CUDA graph cache for the batch-1 latency path
-  cudaGraphExec_t graph_exec = nullptr;
+  GraphExec graph_exec;
   const void* graph_ptrs[8] = {nullptr};
   float graph_maskcent = 0.f;
   int launch_count = 0;
@@ -197,26 +236,24 @@ struct Ctx {
   bool chain = false;           // the previous operation on the forward's stream was a kernel of this forward (PDL)
   bool gadd_active = false;     // a global-hints vector was supplied to this forward
   int last_n = 0;
-  double* d_reccs = nullptr;    // idc_ab_reccs scratch (results of every restart, then the 529x2 gamut points)
-  float* d_negent = nullptr;    // idc_dist_negentropy result, (H/4)*(W/4) floats
+  DevMem<double> d_reccs;       // idc_ab_reccs scratch (results of every restart, then the 529x2 gamut points)
+  DevMem<float> d_negent;       // idc_dist_negentropy result, (H/4)*(W/4) floats
+  DevMem<float> d_dist313;      // idc_caffe313_dist_pixel result, 320 floats
   bool dist_resident = false;   // keep the dist of the last forward_host on the device (idc_fetch_dist)
   int dist_valid_n = 0;
-  // idc_set_click: the clicked pixel's pmf + K colour suggestions ride on a side branch of the click graph
   bool click_mode = false;
-  int* h_click = nullptr; int* d_click = nullptr;   // {img, y4, x4, K, seq} in mapped host memory, read when the graph runs
-  char* d_clickout = nullptr; char* h_clickout = nullptr;   // [8-int header | 544 floats pmf | n_init x (3K+2) doubles]
+  std::unique_ptr<ClickBlock> click;
   bool click_served = false;    // h_clickout holds the answer for the click in its header
   // per-op profiling
   bool profiling = false;
-  std::vector<std::vector<cudaEvent_t>> prof_runs;   // one event list per profiled forward
-  std::vector<cudaEvent_t> prof_pool;
+  std::vector<std::vector<Event>> prof_runs;   // one event list per profiled forward
+  std::vector<Event> prof_pool;
   std::string err;
 };
 
 // ---- engine entry points (idc_simt.cu / idc_umma.cu / idc_heads.cu) ----
 cudaError_t simt_run_op(Ctx* c, ConvOp& op, int n, cudaStream_t st);
 int umma_plan_op(Ctx* c, ConvOp& op);              // builds tensor maps; returns IDC_* code
-void umma_free_op(ConvOp& op);
 cudaError_t umma_run_op(Ctx* c, ConvOp& op, int n, float* out_ab_fused, float out_mult, cudaStream_t st, int img0 = 0,
                         int max_ctas = 0);   // max_ctas > 0: cap the persistent grid (side-branch launches)
 bool umma_op_uses_split_k(const ConvOp& op);

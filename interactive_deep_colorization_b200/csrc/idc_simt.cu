@@ -121,7 +121,7 @@ cudaError_t simt_run_op(Ctx* c, ConvOp& op, int n, cudaStream_t st) {
     SimtParams p{};
     for (int s = 0; s < op.nsrc; ++s) {
       const ActBuf& b = c->bufs[op.src[s].buf];
-      p.src[s] = static_cast<const float*>(b.p0);
+      p.src[s] = static_cast<const float*>(b.p0.get());
       p.sH[s] = b.H; p.sW[s] = b.W; p.sC[s] = b.C; p.ss[s] = op.src[s].s;
     }
     p.ntaps = op.ntaps;
@@ -139,11 +139,11 @@ cudaError_t simt_run_op(Ctx* c, ConvOp& op, int n, cudaStream_t st) {
       p.out_ld = op.cout_pad;
     } else {
       const ActBuf& ob = c->bufs[op.out_buf];
-      p.out = static_cast<float*>(ob.p0); p.Hout = ob.H; p.Wout = ob.W; p.os = op.os;
+      p.out = static_cast<float*>(ob.p0.get()); p.Hout = ob.H; p.Wout = ob.W; p.os = op.os;
       p.oy0 = cls >> 1; p.ox0 = cls & 1; p.out_ld = ob.C;
     }
     p.bias = op.epi.bias; p.scale = op.epi.scale; p.shift = op.epi.shift;
-    p.gadd = (op.epi.gadd && c->gadd_active) ? c->gvec : nullptr;
+    p.gadd = (op.epi.gadd && c->gadd_active) ? c->gvec.get() : nullptr;
     p.act = op.epi.act;
     const int M = n * op.Hl * op.Wl;
     dim3 grid(ceil_div(M, BM), op.cout_pad / BN);

@@ -866,11 +866,11 @@ conv1_1_umma_kernel(const uint8_t* __restrict__ pack, const float* __restrict__ 
 }
 
 cudaError_t conv1_1_umma_pack(Ctx* c) {
-  if (!c->w11_umma) {
-    cudaError_t e = cudaMalloc(&c->w11_umma, kC11PackBytes);
+  if (!c->w11_umma.get()) {
+    cudaError_t e = cudaMalloc(c->w11_umma.put(), kC11PackBytes);
     if (e != cudaSuccess) return e;
   }
-  conv1_1_pack_kernel<<<1, 64>>>(c->w11, c->b11, c->w11_umma);
+  conv1_1_pack_kernel<<<1, 64>>>(c->w11, c->b11, c->w11_umma.get());
   cudaError_t e = cudaGetLastError();
   return e != cudaSuccess ? e : cudaDeviceSynchronize();
 }
@@ -880,10 +880,7 @@ cudaError_t launch_conv1_1_umma(Ctx* c, int n, const float* L, const float* ab, 
   const ActBuf& o = c->bufs[c->buf_index.at("a1_1")];
   const size_t HW = (size_t)o.H * o.W, npix = (size_t)n * HW, ooff = (size_t)img0 * HW * o.C;
   const int ntiles = (int)((npix + 127) / 128);
-  static int sms[64] = {};
-  int& nsm = sms[c->dev < 64 ? c->dev : 0];
-  if (!nsm) { cudaDeviceProp prop; cudaGetDeviceProperties(&prop, c->dev); nsm = prop.multiProcessorCount; }
-  const int grid = ntiles < 4 * nsm ? ntiles : 4 * nsm;
+  const int grid = ntiles < 4 * c->num_sms ? ntiles : 4 * c->num_sms;
   L += img0 * HW; ab += img0 * 2 * HW; mask += img0 * HW;
   static unsigned long long attr_devs = 0;
   if (c->dev >= 64 || !(attr_devs & (1ull << c->dev))) {
@@ -892,11 +889,11 @@ cudaError_t launch_conv1_1_umma(Ctx* c, int n, const float* L, const float* ab, 
     if (e != cudaSuccess) return e;
     if (c->dev < 64) attr_devs |= 1ull << c->dev;
   }
-  __half* hi = static_cast<__half*>(o.p0) + ooff;
-  __half* lo = o.p1 ? static_cast<__half*>(o.p1) + ooff : nullptr;
-  cudaError_t e = lo ? launch_k(c, conv1_1_umma_kernel<true>, dim3(grid), dim3(128), (size_t)kC11Smem, st, c->w11_umma, L, ab, mask,
+  __half* hi = static_cast<__half*>(o.p0.get()) + ooff;
+  __half* lo = o.p1.get() ? static_cast<__half*>(o.p1.get()) + ooff : nullptr;
+  cudaError_t e = lo ? launch_k(c, conv1_1_umma_kernel<true>, dim3(grid), dim3(128), (size_t)kC11Smem, st, c->w11_umma.get(), L, ab, mask,
                                 maskcent, n, o.H, o.W, hi, lo)
-                     : launch_k(c, conv1_1_umma_kernel<false>, dim3(grid), dim3(128), (size_t)kC11Smem, st, c->w11_umma, L, ab, mask,
+                     : launch_k(c, conv1_1_umma_kernel<false>, dim3(grid), dim3(128), (size_t)kC11Smem, st, c->w11_umma.get(), L, ab, mask,
                                 maskcent, n, o.H, o.W, hi, lo);
   c->launch_count++;
   return e;
@@ -922,8 +919,8 @@ static PFN_encodeTiled get_encode() {
 }
 
 struct UmmaPlan {
-  CUtensorMap* d_amaps = nullptr;
-  int4* d_kblk = nullptr;
+  DevMem<CUtensorMap> d_amaps;
+  DevMem<int4> d_kblk;
   CUtensorMap bmap_hi, bmap_lo;
   UmmaParams prm{};
   int num_sms = 132;
@@ -981,12 +978,9 @@ static cudaError_t launch_inst(const UmmaPlan& pl, const UmmaParams& prm, cudaSt
 int umma_plan_op(Ctx* c, ConvOp& op) {
   PFN_encodeTiled enc = get_encode();
   if (!enc) { c->err = "cuTensorMapEncodeTiled entry point not available"; return IDC_ERR_CUDA; }
-  umma_free_op(op);
-  UmmaPlan* pl = new UmmaPlan();
-  op.umma_plan = pl;
-  cudaDeviceProp prop;
-  cudaGetDeviceProperties(&prop, c->dev);
-  pl->num_sms = prop.multiProcessorCount;
+  op.umma_plan.reset();
+  std::unique_ptr<UmmaPlan, UmmaPlanFree> pl(new UmmaPlan());   // installed on the op once complete
+  pl->num_sms = c->num_sms;
   pl->dev = c->dev;
   // tile geometry: 128 output columns where the layer allows it (the chunk and tile accumulators of a 128 x 128 tile
   // take 128 of a math thread's 232 registers; 256 columns would not fit), 64 otherwise
@@ -1108,7 +1102,7 @@ int umma_plan_op(Ctx* c, ConvOp& op) {
     const ActBuf& b = c->bufs[op.src[vk.src].buf];
     const int Hv = (b.H - vk.qy + vk.s - 1) / vk.s, Wv = (b.W - vk.qx + vk.s - 1) / vk.s;
     for (int part = 0; part < 2; ++part) {
-      char* base = (char*)(part == 0 ? b.p0 : b.p1);
+      char* base = (char*)(part == 0 ? b.p0.get() : b.p1.get());
       if (!base) { amaps[i * 2 + part] = amaps[i * 2]; continue; }  // fast mode: lo unused
       base += ((size_t)vk.qy * b.W + vk.qx) * b.C * sizeof(__half);
       cuuint64_t dims[4] = {(cuuint64_t)b.C, (cuuint64_t)Wv, (cuuint64_t)Hv, (cuuint64_t)c->max_n};
@@ -1145,16 +1139,16 @@ int umma_plan_op(Ctx* c, ConvOp& op) {
       return IDC_ERR_CUDA;
     }
   }
-  if (cudaMalloc(&pl->d_amaps, amaps.size() * sizeof(CUtensorMap)) != cudaSuccess ||
-      cudaMalloc(&pl->d_kblk, kblk.size() * sizeof(int4)) != cudaSuccess) {
-    c->err = "cudaMalloc failed in umma_plan_op";
+  if (cudaMalloc(pl->d_amaps.put(), amaps.size() * sizeof(CUtensorMap)) != cudaSuccess ||
+      cudaMalloc(pl->d_kblk.put(), kblk.size() * sizeof(int4)) != cudaSuccess ||
+      cudaMemcpy(pl->d_amaps.get(), amaps.data(), amaps.size() * sizeof(CUtensorMap), cudaMemcpyHostToDevice) != cudaSuccess ||
+      cudaMemcpy(pl->d_kblk.get(), kblk.data(), kblk.size() * sizeof(int4), cudaMemcpyHostToDevice) != cudaSuccess) {
+    c->err = "uploading the launch plan failed in umma_plan_op: " + op.name;
     return IDC_ERR_CUDA;
   }
-  cudaMemcpy(pl->d_amaps, amaps.data(), amaps.size() * sizeof(CUtensorMap), cudaMemcpyHostToDevice);
-  cudaMemcpy(pl->d_kblk, kblk.data(), kblk.size() * sizeof(int4), cudaMemcpyHostToDevice);
 
   UmmaParams& q = pl->prm;
-  q.amaps = pl->d_amaps; q.n_amaps = (int)amaps.size(); q.kblk = pl->d_kblk; q.nkb = nkb; q.ncls = op.ncls;
+  q.amaps = pl->d_amaps.get(); q.n_amaps = (int)amaps.size(); q.kblk = pl->d_kblk.get(); q.nkb = nkb; q.ncls = op.ncls;
   {
     // chunk_kb: k-blocks summed inside the tensor core before the FP32 round-to-nearest add.  1 is the most
     // accurate; the Cout <= 128 layers have short K (few chunks per tile to amortise the tile epilogue) and use 2.
@@ -1176,32 +1170,25 @@ int umma_plan_op(Ctx* c, ConvOp& op) {
     q.out_f32 = op.out_f32_ptr; q.out_ld = op.cout_pad;
   } else if (op.out_buf >= 0) {
     const ActBuf& ob = c->bufs[op.out_buf];
-    q.out_hi = (__half*)ob.p0; q.out_lo = (__half*)ob.p1;
+    q.out_hi = (__half*)ob.p0.get(); q.out_lo = (__half*)ob.p1.get();
     q.Hout = ob.H; q.Wout = ob.W; q.Cout = ob.C; q.os = op.os;
   }
   if (op.fuse_out_head) { q.wout = c->wout; q.bout = c->bout; }
   q.err = c->d_err;
   q.img0 = 0;
+  op.umma_plan = std::move(pl);
   return IDC_OK;
 }
 
-void umma_free_op(ConvOp& op) {
-  UmmaPlan* pl = static_cast<UmmaPlan*>(op.umma_plan);
-  if (!pl) return;
-  if (pl->d_amaps) cudaFree(pl->d_amaps);
-  if (pl->d_kblk) cudaFree(pl->d_kblk);
-  delete pl;
-  op.umma_plan = nullptr;
-}
+void UmmaPlanFree::operator()(UmmaPlan* p) const { delete p; }
 
 bool umma_op_uses_split_k(const ConvOp& op) {
-  const UmmaPlan* pl = static_cast<const UmmaPlan*>(op.umma_plan);
-  return pl && pl->split_k > 1;
+  return op.umma_plan && op.umma_plan->split_k > 1;
 }
 
 cudaError_t umma_run_op(Ctx* c, ConvOp& op, int n, float* out_ab_fused, float out_mult, cudaStream_t st, int img0,
                         int max_ctas) {
-  UmmaPlan* pl = static_cast<UmmaPlan*>(op.umma_plan);
+  const UmmaPlan* pl = op.umma_plan.get();
   if (!pl) return cudaErrorInvalidValue;
   UmmaParams prm = pl->prm;
   prm.max_ctas = (max_ctas > 0 && pl->split_k == 1) ? (max_ctas / pl->cg) * pl->cg : 0;   // split-K needs all items co-resident
@@ -1210,11 +1197,11 @@ cudaError_t umma_run_op(Ctx* c, ConvOp& op, int n, float* out_ab_fused, float ou
   if (img0 && pl->split_k > 1) return cudaErrorInvalidValue;   // image chunks are a large-batch feature
   const int m_tiles = n * prm.tiles_y * prm.tiles_x;
   prm.total_tiles = op.ncls * (pl->cg == 2 ? (m_tiles + 1) / 2 : m_tiles) * prm.n_tiles_n;
-  prm.gadd = (op.epi.gadd && c->gadd_active) ? c->gvec : nullptr;
+  prm.gadd = (op.epi.gadd && c->gadd_active) ? c->gvec.get() : nullptr;
   prm.out_ab = out_ab_fused;
   prm.split_k = pl->split_k;
-  prm.ws = c->splitk_ws;
-  prm.counters = c->splitk_counters;
+  prm.ws = c->splitk_ws.get();
+  prm.counters = c->splitk_counters.get();
   if (pl->split_k > 1 && (!prm.ws || !prm.counters)) return cudaErrorInvalidValue;
   prm.out_mult = out_mult;
   if (op.fuse_out_head && !out_ab_fused) return cudaErrorInvalidValue;

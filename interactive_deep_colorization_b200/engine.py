@@ -200,14 +200,7 @@ class LhnContext(object):
                     "out_abq": blocks[1][b_ab + b_rgb:].view(np.float64).reshape(n, 2, self.H, self.W)}
         n_in = n * 4 * HW + (n * 316 if glob else 0)
         b_ab, b_rgb, b_q = n * 2 * HW * 4, n * 3 * HW, n * 2 * HW * 8
-        sizes = (n_in * 4, b_ab + b_rgb + b_q)
-        blocks = []
-        for nbytes in sizes:
-            p = self.lib.idc_host_alloc(nbytes)
-            if not p:
-                raise _lib.IdcError(-2, "idc_host_alloc(%d) failed" % nbytes)
-            self._pinned.append(p)
-            blocks.append(np.frombuffer((ctypes.c_char * nbytes).from_address(p), dtype=np.uint8))
+        blocks = [self._host_block(nbytes) for nbytes in (n_in * 4, b_ab + b_rgb + b_q)]
         fin = blocks[0].view(np.float32)
         out = {"L_mc": fin[:n * HW].reshape(n, 1, self.H, self.W),
                "ab": fin[n * HW:3 * n * HW].reshape(n, 2, self.H, self.W),

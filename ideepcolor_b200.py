@@ -9,6 +9,13 @@ result folder, plus the K colour suggestions per hint that the GUI shows in its 
     python ideepcolor_b200.py --image_file test_imgs/mortar_pestle.jpg --color_model caffemodel.pth \\
         --hints hints.json --out result_dir [--suggest 9] [--pytorch_maskcent] [--gpu 0] [--load_size 256]
 
+Automatic colorization of a folder of photos, in batches on the device (photos.PhotoColorizer):
+
+    python ideepcolor_b200.py --color_model caffemodel.pth --image_dir scans/ --out scans_color/ [--batch 32] [--psnr]
+
+writes <out>/<stem>.png per photo (the full-resolution result, get_img_fullres) and, with --psnr, <out>/psnr.csv
+(get_result_PSNR of each photo).
+
 hints.json: [{"loc": [row, col], "size": 3, "ab": [23, -69]}, {"loc": [100, 160], "rgb": [255, 255, 255]}, ...]
 (`loc` in load_size x load_size network coordinates, `size` = p of the notebook's put_point: a (2p+1)^2 patch.)
 """
@@ -32,6 +39,9 @@ def parse_args(argv=None):
     ap.add_argument("--load_size", type=int, default=256, help="network resolution")
     ap.add_argument("--pytorch_maskcent", action="store_true", help="centre the mask (siggraph_pretrained weights)")
     ap.add_argument("--suggest", type=int, default=0, help="K colour suggestions per hint (0 = off)")
+    ap.add_argument("--image_dir", default="", help="colorize every photo of this folder automatically (needs --out)")
+    ap.add_argument("--batch", type=int, default=32, help="photos per device pass (--image_dir)")
+    ap.add_argument("--psnr", action="store_true", help="also write psnr.csv (--image_dir)")
     return ap.parse_args(argv)
 
 
@@ -46,8 +56,48 @@ def hint_ab(h):
     return [float(lab[0, 0, 1]), float(lab[0, 0, 2])]
 
 
+IMAGE_EXTS = (".jpg", ".jpeg", ".png", ".bmp", ".tif", ".tiff", ".webp")
+
+
+def colorize_dir(args):
+    """--image_dir: every photo of the folder (sorted by name) through PhotoColorizer -> OUT/<stem>.png (+ psnr.csv)."""
+    import cv2
+    import torch
+    from interactive_deep_colorization_b200.photos import PhotoColorizer
+    if not args.out:
+        print("--image_dir needs --out")
+        return 2
+    names = sorted(f for f in os.listdir(args.image_dir) if os.path.splitext(f)[1].lower() in IMAGE_EXTS)
+    stems = {}
+    for f in names:
+        stems.setdefault(os.path.splitext(f)[0], []).append(f)
+    clash = [" / ".join(v) for v in stems.values() if len(v) > 1]
+    if clash:             # OUT/<stem>.png would hold only one of them
+        print("photos share a name and would overwrite each other's result: %s" % ", ".join(clash))
+        return 2
+    paths = [os.path.join(args.image_dir, f) for f in names]
+    if not os.path.isdir(args.out):
+        os.makedirs(args.out)
+    sd = torch.load(args.color_model, map_location="cpu")
+    pc = PhotoColorizer(sd, Xd=args.load_size, batch=args.batch, device=args.gpu, maskcent=args.pytorch_maskcent)
+    rows = []
+    for name, r in zip(names, pc.colorize(paths, psnr=args.psnr)):
+        stem = os.path.splitext(name)[0]
+        cv2.imwrite(os.path.join(args.out, stem + ".png"), np.ascontiguousarray(r.fullres[:, :, ::-1]))
+        if args.psnr:
+            rows.append("%s,%.17g" % (name, r.psnr))
+    pc.close()
+    if args.psnr:
+        with open(os.path.join(args.out, "psnr.csv"), "w") as f:
+            f.write("image,psnr\n" + "".join(row + "\n" for row in rows))
+    print("colorized %d photos into <%s>" % (len(names), args.out))
+    return 0
+
+
 def main(argv=None):
     args = parse_args(argv)
+    if args.image_dir:
+        return colorize_dir(args)
     import cv2
     import torch
     from interactive_deep_colorization_b200 import colorize_image as CI

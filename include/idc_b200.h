@@ -289,6 +289,42 @@ int idc_cubic_lab2rgb_u8(int device, int h_in, int w_in, const double* ab, int h
  * and rgb = 255 where mask is 0 (`masked_rgb`).  float64 like the reference; rgb [A][B][3], mask [A][B] DEVICE ptrs. */
 int idc_gamut_ab(int device, double L, int gamut_size, int D, uint8_t* rgb, uint8_t* mask, void* stream);
 
+/* Batched photos (automatic colorization of many photos; reference: load_image + net_forward + get_img_fullres +
+ * get_result_PSNR per photo, data/colorize_image.py:52-66, :98-109, :123-131, :249-267).  A batch is n <= IDC_MAX_PHOTOS
+ * photos of any sizes packed back to back in ONE device buffer of uint8 RGB; the table (HOST memory, checked before
+ * any device call and passed to the kernels by value) gives each photo's first pixel and size.  Photos must not
+ * overlap: off[i] + h[i] * w[i] <= off[i + 1].  X is the network size (a multiple of 8).  DEVICE data pointers,
+ * asynchronous on `stream`.  IDC_ERR_ARG, before any device call, for n outside [1, IDC_MAX_PHOTOS], a NULL pointer
+ * that is not optional, h or w outside [1, IDC_MAX_PHOTO_SIDE], overlapping photos, X outside [8, IDC_MAX_PHOTO_X] or
+ * not a multiple of 8, and a hint count above IDC_MAX_HINTS. */
+typedef struct { int64_t off; int32_t h, w; } idc_photo;   /* off = first pixel, in pixels */
+#define IDC_MAX_PHOTOS 128
+#define IDC_MAX_PHOTO_SIDE 16777216   /* 2^24: pixel and byte indices within one photo row stay in 32 bits */
+#define IDC_MAX_PHOTO_X 16384         /* X * X * 3 stays in 32 bits */
+/* load_image (:52-66) + the mean-centring of set_image (:68-77, :172-178) for every photo: cv2.resize(photo, (X, X))
+ * with OpenCV's 8-bit INTER_LINEAR (the same arithmetic as idc_resize_u8_linear, exact-2x area shortcut included),
+ * skimage rgb2lab, L_mc = (float)(L - 50) -> L_mc [n,1,X,X] float32 (idc_forward's input); rgb [n,X,X,3] uint8 = the
+ * network-size photo (`img_rgb`), or NULL. */
+int idc_photo_prep(int device, int n, const idc_photo* photos, const uint8_t* src, int X, float* L_mc, uint8_t* rgb,
+                   void* stream);
+/* get_img_fullres (:123-131) for every photo: L of each full-resolution pixel from its own source pixel (skimage
+ * rgb2lab, no Lab plane is stored), ab = scipy.ndimage.zoom(order=1) of the photo's quantised output_ab (planes 1-2 of
+ * lab [n,3,X,X] float64, as idc_rgb2lab_f64 writes them from idc_forward's out_rgb) with idc_render_planes_u8's edge
+ * rule, then lab2rgb_transpose -> out, uint8 RGB in the layout of src.  Each pixel reads only its own source pixel,
+ * so out may be src (in place). */
+int idc_photo_render(int device, int n, const idc_photo* photos, const uint8_t* src, int X, const double* lab,
+                     uint8_t* out, void* stream);
+/* The hint raster of idc_set_hints on caller planes: block = [16-byte header {count, 0, 0, 0} | count idc_hint] in
+ * DEVICE memory (the kernel reads the count from the header); count (HOST) is the same count, checked against
+ * IDC_MAX_HINTS.  Pixel (y, x) of image i in [0, n) takes the last hint with img == i that covers it -> ab [n,2,h,w],
+ * mask [n,1,h,w] float32, exactly the planes idc_forward_host's hint mode feeds the network.  n <= 65535 and
+ * h * w < 2^31 - 256. */
+int idc_hint_raster(int device, int n, int h, int w, int count, const void* block, float* ab, float* mask, void* stream);
+/* get_result_PSNR (:98-109) before its float64 tail: sse[i] = sum over the h*w*3 values of image i of (a - b)^2, exact in
+ * int64, for uint8 images a, b [n,h,w,3] (img_rgb, output_rgb), n <= 65535.  20 * log10(255 / sqrt(sse / (h*w*3))) on the host then
+ * equals numpy's result bit for bit. */
+int idc_rgb_sse(int device, int n, int h, int w, const uint8_t* a, const uint8_t* b, int64_t* sse, void* stream);
+
 /* ---- introspection / test hooks (used by tests/, never by the product path) ---- */
 /* Copy a named activation ("conv1_2", "a8_1", ... see DESIGN.md) of the LAST forward to
  * out [n,C,H,W] FP32 device memory; *c,*h,*w receive its shape. */

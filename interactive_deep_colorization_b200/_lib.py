@@ -24,6 +24,12 @@ FLAG_KEEP_CONV10 = 1 << 5
 FLAG_CAFFE313 = 1 << 6
 F32, F64, I64 = 0, 1, 2
 MAX_HINTS = 1024                      # IDC_MAX_HINTS
+MAX_PHOTOS = 128                      # IDC_MAX_PHOTOS
+MAX_PHOTO_SIDE = 1 << 24               # IDC_MAX_PHOTO_SIDE
+MAX_PHOTO_X = 16384                   # IDC_MAX_PHOTO_X
+HINT_HDR_BYTES = 16                   # header {count, 0, 0, 0} of an idc_hint_raster block
+# idc_photo: a photo of a packed batch, its first pixel and its size
+PHOTO_DTYPE = np.dtype([("off", "<i8"), ("h", "<i4"), ("w", "<i4")])
 RENDER_L_PLANE, RENDER_L_MASK, RENDER_L_SUP = 0, 1, 2     # idc_render_planes_u8 l_mode
 # idc_hint: inclusive pixel rectangle of image `img` painted with one ab colour (28 bytes, no padding)
 HINT_DTYPE = np.dtype([("img", "<i4"), ("y0", "<i4"), ("x0", "<i4"), ("y1", "<i4"), ("x1", "<i4"),
@@ -68,6 +74,10 @@ SYMBOLS = [
                                         _P, _c.c_int, _c.c_int, _P, _P]),
     ("idc_resize_u8_linear", _c.c_int, [_c.c_int, _c.c_int, _c.c_int, _P, _c.c_int, _c.c_int, _P, _P]),
     ("idc_cubic_lab2rgb_u8", _c.c_int, [_c.c_int, _c.c_int, _c.c_int, _P, _c.c_int, _c.c_int, _P, _P, _P]),
+    ("idc_photo_prep", _c.c_int, [_c.c_int, _c.c_int, _P, _P, _c.c_int, _P, _P, _P]),
+    ("idc_photo_render", _c.c_int, [_c.c_int, _c.c_int, _P, _P, _c.c_int, _P, _P, _P]),
+    ("idc_hint_raster", _c.c_int, [_c.c_int, _c.c_int, _c.c_int, _c.c_int, _c.c_int, _P, _P, _P, _P]),
+    ("idc_rgb_sse", _c.c_int, [_c.c_int, _c.c_int, _c.c_int, _c.c_int, _P, _P, _P, _P]),
     ("idc_get_activation", _c.c_int, [_P, _c.c_char_p, _P, _c.c_size_t, _c.POINTER(_c.c_int),
                                       _c.POINTER(_c.c_int), _c.POINTER(_c.c_int)]),
     ("idc_set_activation", _c.c_int, [_P, _c.c_char_p, _c.c_int, _P]),

@@ -564,7 +564,7 @@ int run_forward(Ctx* c, int n, const float* L, const float* ab, const float* mas
   const size_t HW = (size_t)c->H * c->W;
   const bool c11_umma = c->opt.conv1_1_umma && !c->simt && c->w11_umma.get();
   // hint mode: the ab / mask planes conv1_1 reads are rasterised here from the hint block (already on the device)
-  if (hints_dev) CUDA_TRY(c, launch_hint_raster(c, n, hints_dev, const_cast<float*>(ab), const_cast<float*>(mask), st));
+  if (hints_dev) CUDA_TRY(c, launch_hint_raster(c, n, c->H, c->W, hints_dev, const_cast<float*>(ab), const_cast<float*>(mask), st));
   if (hp) {
     for (int k = 0; k < hp->nchunks; ++k) {
       CUDA_TRY(c, cudaStreamWaitEvent(st, c->pipe->ev_in[k].get(), 0));
@@ -1401,6 +1401,48 @@ int idc_gamut_ab(int device, double L, int gamut_size, int D, uint8_t* rgb, uint
   const int A = (2 * gamut_size + D - 1) / D + 1;        // len(np.arange(-g, g + D, D))
   if (cudaSetDevice(device) != cudaSuccess) return IDC_ERR_CUDA;
   return launch_gamut(L, gamut_size, D, A, rgb, mask, (cudaStream_t)stream) == cudaSuccess ? IDC_OK : IDC_ERR_CUDA;
+}
+
+// the photo table of a batch: 1 <= n <= IDC_MAX_PHOTOS, every photo at least 1 x 1, in ascending non-overlapping order
+// X and the photo sides are bounded so that the kernels' 32-bit pixel and byte indices within one image cannot overflow
+static bool photos_ok(int n, const idc_photo* t, int X) {
+  if (n < 1 || n > IDC_MAX_PHOTOS || !t || X < 8 || X > IDC_MAX_PHOTO_X || (X % 8)) return false;
+  int64_t end = 0;
+  for (int i = 0; i < n; ++i) {
+    if (t[i].h < 1 || t[i].w < 1 || t[i].h > IDC_MAX_PHOTO_SIDE || t[i].w > IDC_MAX_PHOTO_SIDE || t[i].off < end)
+      return false;
+    end = t[i].off + (int64_t)t[i].h * t[i].w;
+  }
+  return end <= (int64_t)0x7fffffff * 256;              // grid.x limit of the render at 256 threads per block
+}
+
+int idc_photo_prep(int device, int n, const idc_photo* photos, const uint8_t* src, int X, float* L_mc, uint8_t* rgb,
+                   void* stream) {
+  if (!photos_ok(n, photos, X) || !src || !L_mc) return IDC_ERR_ARG;
+  if (cudaSetDevice(device) != cudaSuccess) return IDC_ERR_CUDA;
+  return launch_photo_prep(n, photos, src, X, L_mc, rgb, (cudaStream_t)stream) == cudaSuccess ? IDC_OK : IDC_ERR_CUDA;
+}
+
+int idc_photo_render(int device, int n, const idc_photo* photos, const uint8_t* src, int X, const double* lab,
+                     uint8_t* out, void* stream) {
+  if (!photos_ok(n, photos, X) || !src || !lab || !out) return IDC_ERR_ARG;
+  if (cudaSetDevice(device) != cudaSuccess) return IDC_ERR_CUDA;
+  return launch_photo_render(n, photos, src, X, lab, out, (cudaStream_t)stream) == cudaSuccess ? IDC_OK : IDC_ERR_CUDA;
+}
+
+int idc_hint_raster(int device, int n, int h, int w, int count, const void* block, float* ab, float* mask, void* stream) {
+  if (n < 1 || n > 65535 || h < 1 || w < 1 || count < 0 || count > IDC_MAX_HINTS || !block || !ab || !mask)
+    return IDC_ERR_ARG;
+  if ((size_t)h * w > (size_t)0x7fffffff - 256) return IDC_ERR_ARG;   // the kernel's int pixel index + one CTA
+  if (cudaSetDevice(device) != cudaSuccess) return IDC_ERR_CUDA;
+  return launch_hint_raster(nullptr, n, h, w, static_cast<const char*>(block), ab, mask, (cudaStream_t)stream) == cudaSuccess
+             ? IDC_OK : IDC_ERR_CUDA;
+}
+
+int idc_rgb_sse(int device, int n, int h, int w, const uint8_t* a, const uint8_t* b, int64_t* sse, void* stream) {
+  if (n < 1 || n > 65535 || h < 1 || w < 1 || !a || !b || !sse) return IDC_ERR_ARG;
+  if (cudaSetDevice(device) != cudaSuccess) return IDC_ERR_CUDA;
+  return launch_rgb_sse(n, (size_t)h * w * 3, a, b, sse, (cudaStream_t)stream) == cudaSuccess ? IDC_OK : IDC_ERR_CUDA;
 }
 
 int idc_get_activation(idc_ctx* c, const char* name, float* out, size_t out_floats, int* ch, int* h, int* w) {

@@ -267,8 +267,10 @@ cudaError_t conv1_1_umma_pack(Ctx* c);                                       // 
 // travels whole, so the copy is the same graph node whatever the count.
 constexpr size_t kHintHdrBytes = 16;
 constexpr size_t kHintBlockBytes = kHintHdrBytes + (size_t)IDC_MAX_HINTS * sizeof(idc_hint);
-// rasterise the hint block (device) into the ab [n,2,H,W] / mask [n,1,H,W] planes conv1_1 reads
-cudaError_t launch_hint_raster(Ctx* c, int n, const char* hints_dev, float* ab, float* mask, cudaStream_t st);
+// rasterise the hint block (device) into the ab [n,2,H,W] / mask [n,1,H,W] planes conv1_1 reads (c may be null:
+// idc_hint_raster, outside a forward)
+cudaError_t launch_hint_raster(Ctx* c, int n, int H, int W, const char* hints_dev, float* ab, float* mask,
+                               cudaStream_t st);
 cudaError_t launch_gamut(double L, int gamut_size, int D, int A, uint8_t* rgb, uint8_t* mask, cudaStream_t st);
 cudaError_t launch_out_head(Ctx* c, int n, float* out_ab, cudaStream_t st);   // SIMT / KEEP_CONV10 path
 cudaError_t launch_softmax529(Ctx* c, int n, float* out_dist, cudaStream_t st);
@@ -288,6 +290,12 @@ cudaError_t launch_render_planes(const double* ab, int ab_order, int ab_f32, con
 cudaError_t launch_resize_linear_u8(const uint8_t* src, int hs, int ws, uint8_t* dst, int hd, int wd, cudaStream_t st);
 cudaError_t launch_cubic_lab2rgb(const double* ab, int hin, int win, const double* L, int H, int W, uint8_t* rgb,
                                  cudaStream_t st);
+// batched photos (idc_photos.cu); table: n <= IDC_MAX_PHOTOS entries, checked by the caller
+cudaError_t launch_photo_prep(int n, const idc_photo* table, const uint8_t* src, int X, float* L_mc, uint8_t* rgb,
+                              cudaStream_t st);
+cudaError_t launch_photo_render(int n, const idc_photo* table, const uint8_t* src, int X, const double* lab, uint8_t* out,
+                                cudaStream_t st);
+cudaError_t launch_rgb_sse(int n, size_t hw3, const uint8_t* a, const uint8_t* b, int64_t* sse, cudaStream_t st);
 cudaError_t launch_global_mlp(Ctx* c, int n, const float* glob, cudaStream_t st);
 cudaError_t launch_act_to_nchw(Ctx* c, const ActBuf& b, int n, float* out, cudaStream_t st);
 cudaError_t launch_nchw_to_act(Ctx* c, const ActBuf& b, int n, const float* in, cudaStream_t st);
@@ -327,6 +335,122 @@ __device__ __forceinline__ void lab_to_rgb_u8(double l, double a, double b, uint
   out[0] = (uint8_t)(fmin(fmax(R, 0.0), 1.0) * 255.0);
   out[1] = (uint8_t)(fmin(fmax(G, 0.0), 1.0) * 255.0);
   out[2] = (uint8_t)(fmin(fmax(B, 0.0), 1.0) * 255.0);
+}
+
+// sRGB uint8 -> Lab, float64 like skimage 0.13 color.rgb2lab (data/colorize_image.py:31-36): rgb2lab_kernel, the gamut
+// map and the batched photo prep / render read a pixel through this one sequence.
+__device__ __forceinline__ double srgb_inv_gamma(double c) {
+  return c > 0.04045 ? pow((c + 0.055) / 1.055, 2.4) : c / 12.92;
+}
+__device__ __forceinline__ double lab_f(double t) { return t > 0.008856 ? cbrt(t) : 7.787 * t + 16.0 / 116.0; }
+__device__ __forceinline__ void rgb_u8_to_lab(const uint8_t* px, double& l, double& a, double& b) {
+  const double R = srgb_inv_gamma(px[0] / 255.0), G = srgb_inv_gamma(px[1] / 255.0), B = srgb_inv_gamma(px[2] / 255.0);
+  const double X = (0.412453 * R + 0.357580 * G + 0.180423 * B) / 0.95047;
+  const double Y = (0.212671 * R + 0.715160 * G + 0.072169 * B) / 1.0;
+  const double Z = (0.019334 * R + 0.119193 * G + 0.950227 * B) / 1.08883;
+  const double fx = lab_f(X), fy = lab_f(Y), fz = lab_f(Z);
+  l = 116.0 * fy - 16.0;
+  a = 500.0 * (fx - fy);
+  b = 200.0 * (fy - fz);
+}
+
+// OpenCV's source coordinate of output d, (float)((d + 0.5) * scale - 0.5) (modules/imgproc/src/resize.cpp), with the
+// multiply and the subtract rounded separately as on the host (nvcc would fuse them).
+__device__ __forceinline__ float cv_src_coord(int d, double scale) {
+  return __double2float_rn(__dsub_rn(__dmul_rn(__dadd_rn((double)d, 0.5), scale), 0.5));
+}
+
+// OpenCV resize, INTER_LINEAR, CV_8U (modules/imgproc/src/resize.cpp: resizeGeneric_ with HResizeLinear / VResizeLinear,
+// INTER_RESIZE_COEF_BITS = 11).  x axis: fx is zeroed when the 2-tap window leaves the image; y axis: the coefficients
+// are kept and the ROW INDICES are clipped instead.
+__device__ __forceinline__ void cv_lin_coef(int d, double scale, int ssize, bool clamp_f, int& s, int& c0, int& c1) {
+  float f = cv_src_coord(d, scale);
+  s = (int)floorf(f);
+  f = __fsub_rn(f, (float)s);
+  if (clamp_f) {
+    if (s < 0) { f = 0.f; s = 0; }
+    if (s >= ssize - 1) { f = 0.f; s = ssize - 1; }
+  }
+  c0 = __float2int_rn(__fmul_rn(__fsub_rn(1.f, f), 2048.f));
+  c1 = __float2int_rn(__fmul_rn(f, 2048.f));
+}
+
+// cv::resize's scale of one axis, 1 / (dsize / ssize) as it computes it
+__host__ __device__ __forceinline__ double cv_scale(int ssize, int dsize) { return 1.0 / ((double)dsize / (double)ssize); }
+
+// One output pixel (dy, dx) of that resize from the uint8 RGB image src [hs,ws,3]: the exact-2x decimation (area2) is
+// routed to the 2x2 area average as cv::resize does; otherwise the 11-bit fixed-point bilinear sum.
+__device__ __forceinline__ void cv_resize_linear_px(const uint8_t* __restrict__ src, int hs, int ws, int dy, int dx,
+                                                    double scale_y, double scale_x, bool area2, uint8_t* o) {
+  if (area2) {
+    const uint8_t* p = src + ((size_t)(2 * dy) * ws + 2 * dx) * 3;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) o[c] = (uint8_t)((p[c] + p[3 + c] + p[(size_t)ws * 3 + c] + p[(size_t)ws * 3 + 3 + c] + 2) >> 2);
+    return;
+  }
+  int sx, a0, a1, sy, b0, b1;
+  cv_lin_coef(dx, scale_x, ws, true, sx, a0, a1);
+  cv_lin_coef(dy, scale_y, hs, false, sy, b0, b1);
+  const int x1 = sx + 1 < ws ? sx + 1 : ws - 1;
+  const int y0 = sy < 0 ? 0 : (sy > hs - 1 ? hs - 1 : sy);
+  const int y1 = sy + 1 < 0 ? 0 : (sy + 1 > hs - 1 ? hs - 1 : sy + 1);
+  const uint8_t* r0 = src + (size_t)y0 * ws * 3;
+  const uint8_t* r1 = src + (size_t)y1 * ws * 3;
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    const int S0 = r0[sx * 3 + c] * a0 + r0[x1 * 3 + c] * a1;
+    const int S1 = r1[sx * 3 + c] * a0 + r1[x1 * 3 + c] * a1;
+    const int v = (((b0 * (S0 >> 4)) >> 16) + ((b1 * (S1 >> 4)) >> 16) + 2) >> 2;
+    o[c] = (uint8_t)(v < 0 ? 0 : (v > 255 ? 255 : v));
+  }
+}
+
+// One axis of scipy.ndimage.zoom(order 0 / 1, mode='constant', cval=0, grid_mode=False) as scipy 1.18 evaluates it
+// (ni_interpolation.c NI_ZoomShift): output o samples c = o * ratio, ratio = (n_in-1)/(n_out-1) rounded to float64
+// first; c > n_in-1 (the ratio rounded up) is outside the input and reads cval.  Order 0 takes floor(c + 0.5); order 1
+// blends floor(c) and the next sample with w0 = 1 - t, w1 = 1 - w0 (scipy's weights; w1 = 0 at c = n_in-1).
+// The ratio of one axis: np.divide(n_in - 1, n_out - 1), and 1 where n_out == 1 (scipy's zoom factor for a length-1
+// output axis).
+__host__ __device__ __forceinline__ double zoom_ratio(int n_in, int n_out) {
+  return n_out > 1 ? (double)(n_in - 1) / (double)(n_out - 1) : 1.0;
+}
+struct ZoomTap {
+  int i0, i1;
+  double w0, w1;
+  bool inside;
+};
+__device__ __forceinline__ ZoomTap zoom_tap(int o, double ratio, int n_in, int order) {
+  ZoomTap t;
+  const double c = __dmul_rn((double)o, ratio);
+  t.inside = c <= (double)(n_in - 1);
+  if (order == 0) {
+    t.i0 = t.i1 = min((int)floor(__dadd_rn(c, 0.5)), n_in - 1);
+    t.w0 = 1.0;
+    t.w1 = 0.0;
+  } else {
+    const double f = floor(c);
+    t.i0 = min((int)f, n_in - 1);
+    t.i1 = min(t.i0 + 1, n_in - 1);
+    t.w0 = __dsub_rn(1.0, __dsub_rn(c, f));
+    t.w1 = __dsub_rn(1.0, t.w0);
+  }
+  return t;
+}
+
+// One plane zoomed at (ty, tx).  Order 1 adds the four taps in scipy's order, (v * wy) * wx each, no FMA, so the value
+// equals scipy's bit for bit; order 0 is the sample itself.
+__device__ __forceinline__ double zoom_sample(const double* __restrict__ p, int win, const ZoomTap& ty, const ZoomTap& tx,
+                                              int order) {
+  if (!(ty.inside && tx.inside)) return 0.0;
+  const double v00 = __ldg(p + (size_t)ty.i0 * win + tx.i0);
+  if (order == 0) return v00;
+  const double v01 = __ldg(p + (size_t)ty.i0 * win + tx.i1);
+  const double v10 = __ldg(p + (size_t)ty.i1 * win + tx.i0);
+  const double v11 = __ldg(p + (size_t)ty.i1 * win + tx.i1);
+  double s = __dmul_rn(__dmul_rn(v00, ty.w0), tx.w0);
+  s = __dadd_rn(s, __dmul_rn(__dmul_rn(v01, ty.w0), tx.w1));
+  s = __dadd_rn(s, __dmul_rn(__dmul_rn(v10, ty.w1), tx.w0));
+  return __dadd_rn(s, __dmul_rn(__dmul_rn(v11, ty.w1), tx.w1));
 }
 
 __device__ __forceinline__ void pdl_prologue_done() {   // small kernels: let the successor start, then wait for the predecessor

@@ -11,59 +11,17 @@
 
 namespace idc {
 
-// OpenCV's source coordinate of output d, (float)((d + 0.5) * scale - 0.5) (modules/imgproc/src/resize.cpp), with the
-// multiply and the subtract rounded separately as on the host (nvcc would fuse them).
-__device__ __forceinline__ float cv_src_coord(int d, double scale) {
-  return __double2float_rn(__dsub_rn(__dmul_rn(__dadd_rn((double)d, 0.5), scale), 0.5));
-}
-
-// OpenCV resize, INTER_LINEAR, CV_8U (modules/imgproc/src/resize.cpp: resizeGeneric_ with HResizeLinear / VResizeLinear,
-// INTER_RESIZE_COEF_BITS = 11).  x axis: fx is zeroed when the 2-tap window leaves the image; y axis: the coefficients
-// are kept and the ROW INDICES are clipped instead.
-__device__ __forceinline__ void cv_lin_coef(int d, double scale, int ssize, bool clamp_f, int& s, int& c0, int& c1) {
-  float f = cv_src_coord(d, scale);
-  s = (int)floorf(f);
-  f = __fsub_rn(f, (float)s);
-  if (clamp_f) {
-    if (s < 0) { f = 0.f; s = 0; }
-    if (s >= ssize - 1) { f = 0.f; s = ssize - 1; }
-  }
-  c0 = __float2int_rn(__fmul_rn(__fsub_rn(1.f, f), 2048.f));
-  c1 = __float2int_rn(__fmul_rn(f, 2048.f));
-}
-
+// cv_src_coord, cv_lin_coef and cv_resize_linear_px live in idc_internal.h, shared with the batched photo prep.
 __global__ void resize_linear_u8_kernel(const uint8_t* __restrict__ src, int hs, int ws, uint8_t* __restrict__ dst,
                                         int hd, int wd, double scale_y, double scale_x, int area2) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (size_t)hd * wd) return;
   const int dy = (int)(i / wd), dx = (int)(i - (size_t)dy * wd);
-  uint8_t* o = dst + i * 3;
-  if (area2) {   // exact 2x decimation: INTER_LINEAR is routed to the 2x2 area average
-    const uint8_t* p = src + ((size_t)(2 * dy) * ws + 2 * dx) * 3;
-#pragma unroll
-    for (int c = 0; c < 3; ++c) o[c] = (uint8_t)((p[c] + p[3 + c] + p[(size_t)ws * 3 + c] + p[(size_t)ws * 3 + 3 + c] + 2) >> 2);
-    return;
-  }
-  int sx, a0, a1, sy, b0, b1;
-  cv_lin_coef(dx, scale_x, ws, true, sx, a0, a1);
-  cv_lin_coef(dy, scale_y, hs, false, sy, b0, b1);
-  const int x1 = sx + 1 < ws ? sx + 1 : ws - 1;
-  const int y0 = sy < 0 ? 0 : (sy > hs - 1 ? hs - 1 : sy);
-  const int y1 = sy + 1 < 0 ? 0 : (sy + 1 > hs - 1 ? hs - 1 : sy + 1);
-  const uint8_t* r0 = src + (size_t)y0 * ws * 3;
-  const uint8_t* r1 = src + (size_t)y1 * ws * 3;
-#pragma unroll
-  for (int c = 0; c < 3; ++c) {
-    const int S0 = r0[sx * 3 + c] * a0 + r0[x1 * 3 + c] * a1;
-    const int S1 = r1[sx * 3 + c] * a0 + r1[x1 * 3 + c] * a1;
-    const int v = (((b0 * (S0 >> 4)) >> 16) + ((b1 * (S1 >> 4)) >> 16) + 2) >> 2;
-    o[c] = (uint8_t)(v < 0 ? 0 : (v > 255 ? 255 : v));
-  }
+  cv_resize_linear_px(src, hs, ws, dy, dx, scale_y, scale_x, area2 != 0, dst + i * 3);
 }
 
 cudaError_t launch_resize_linear_u8(const uint8_t* src, int hs, int ws, uint8_t* dst, int hd, int wd, cudaStream_t st) {
-  const double inv_x = (double)wd / ws, inv_y = (double)hd / hs;
-  const double scale_x = 1.0 / inv_x, scale_y = 1.0 / inv_y;       // as cv::resize computes them
+  const double scale_x = cv_scale(ws, wd), scale_y = cv_scale(hs, hd);
   const int area2 = (ws == 2 * wd && hs == 2 * hd) ? 1 : 0;
   const size_t tot = (size_t)hd * wd;
   resize_linear_u8_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(src, hs, ws, dst, hd, wd, scale_y, scale_x, area2);

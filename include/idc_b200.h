@@ -84,6 +84,9 @@ int idc_create(int device, int max_n, int h, int w, unsigned flags, idc_ctx** ou
  *   "side_dist"     0 / 1       batches <= 4: run the dist head (class + softmax) on a side stream / graph branch
  *   "tanh_scale"    110 / 100   regression head scale: tanh * 110 (model.py:175) or the Caffe nets' 100
  *                               (models/reference_model/deploy_nodist.prototxt:812-822, SURVEY q4)
+ *   "act_exp.<buffer>"  [-24, 24]  wgmma engine: the storage exponent of one activation buffer ("conv4_3", "a8_1", ...;
+ *                               idc_act_exponent), replacing the one chosen from the weights.  Only before
+ *                               idc_finalize_weights: IDC_ERR_STATE once the weights are packed.
  * Unknown names return IDC_ERR_KEY.  A re-plan that fails returns its error and leaves the context refusing forwards
  * with IDC_ERR_STATE until a later re-plan (idc_set_option or idc_adopt_weights) succeeds. */
 int idc_set_option(idc_ctx* ctx, const char* name, int value);
@@ -326,6 +329,10 @@ int idc_hint_raster(int device, int n, int h, int w, int count, const void* bloc
 int idc_rgb_sse(int device, int n, int h, int w, const uint8_t* a, const uint8_t* b, int64_t* sse, void* stream);
 
 /* ---- introspection / test hooks (used by tests/, never by the product path) ---- */
+/* wgmma engine: the exponent S with which activation `name` is stored (FP16 hi/lo planes of value * 2^S), chosen per
+ * buffer from the weights by idc_finalize_weights (DESIGN.md §3); 0 on the SIMT engine.  IDC_ERR_KEY for an unknown
+ * name, IDC_ERR_STATE before the weights are packed. */
+int idc_act_exponent(idc_ctx* ctx, const char* name, int* exp_out);
 /* Copy a named activation ("conv1_2", "a8_1", ... see DESIGN.md) of the LAST forward to
  * out [n,C,H,W] FP32 device memory; *c,*h,*w receive its shape. */
 int idc_get_activation(idc_ctx* ctx, const char* name, float* out_nchw, size_t out_floats,

@@ -81,6 +81,7 @@ SYMBOLS = [
     ("idc_get_activation", _c.c_int, [_P, _c.c_char_p, _P, _c.c_size_t, _c.POINTER(_c.c_int),
                                       _c.POINTER(_c.c_int), _c.POINTER(_c.c_int)]),
     ("idc_set_activation", _c.c_int, [_P, _c.c_char_p, _c.c_int, _P]),
+    ("idc_act_exponent", _c.c_int, [_P, _c.c_char_p, _c.POINTER(_c.c_int)]),
     ("idc_run_op", _c.c_int, [_P, _c.c_char_p, _c.c_int, _P]),
     ("idc_num_ops", _c.c_int, [_P]),
     ("idc_op_name", _c.c_char_p, [_P, _c.c_int]),

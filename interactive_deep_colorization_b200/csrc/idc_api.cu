@@ -8,6 +8,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <cmath>
 
 #include "idc_internal.h"
 
@@ -251,6 +252,7 @@ size_t layout_arena(Ctx* c, char* base) {
   c->b11 = (float*)P(L.take<float>(64));
   c->wout = (float*)P(L.take<float>(256));
   c->bout = (float*)P(L.take<float>(4));
+  c->act_exp = (int*)P(L.take<int>(c->bufs.size()));
   for (auto& op : c->ops) {
     op.epi.bias = (float*)P(L.take<float>(op.cout_pad));
     op.epi.scale = (float*)P(L.take<float>(op.cout_pad));
@@ -303,9 +305,46 @@ void fold_bn(const HostTensor& g, const HostTensor& b, const HostTensor& m, cons
   }
 }
 
+// Storage exponent of buffer b from its magnitude estimate (DESIGN §3): S_b = kActExpRef - ceil(log2 est_b), or the
+// act_exp.<name> override.  Writes it to the arena table and the buffer; fails, naming the buffer, outside the range.
+int set_act_exp(Ctx* c, int* table, int b, double est) {
+  ActBuf& buf = c->bufs[b];
+  int s = 0;
+  if (!c->simt) {
+    if (!std::isfinite(est)) return fail(c, IDC_ERR_ARG, "activation %s: magnitude estimate %g is not finite", buf.name.c_str(), est);
+    s = kActExpRef;
+    if (est > 0.0) {
+      int ex = 0;
+      const double f = frexp(est, &ex);          // est = f * 2^ex, f in [0.5, 1): ceil(log2 est) = ex, or ex - 1 at f = 0.5
+      s = kActExpRef - (f == 0.5 ? ex - 1 : ex);
+    }
+    auto ov = c->act_exp_override.find(buf.name);
+    if (ov != c->act_exp_override.end()) s = ov->second;
+    if (s < kActExpMin || s > kActExpMax)
+      return fail(c, IDC_ERR_UNSUPPORTED,
+                  "activation %s: storage exponent %d (magnitude estimate %g) is outside the supported range [%d, %d]",
+                  buf.name.c_str(), s, est, kActExpMin, kActExpMax);
+  }
+  table[b] = s;
+  buf.exp = s;
+  return IDC_OK;
+}
+
+double sumsq(const float* p, size_t n) {
+  double a = 0.0;
+  for (size_t i = 0; i < n; ++i) a += (double)p[i] * (double)p[i];
+  return a;
+}
+
 int pack_weights(Ctx* c, char* host) {
   // translate device pointers (already laid out relative to c->arena) to host staging pointers
   auto H = [&](void* dev) { return host + ((char*)dev - c->arena.get()); };
+  // magnitude estimates of the buffers, in plan order (FP64): conv output channel co of an op reading sources s is
+  // sum_s ||W_s[co]||_2 * est(s) + |bias_co|; a BatchNorm output restarts from its statistics,
+  // |gamma| * sqrt(var + mean^2) / sqrt(var + eps) + |beta|; the buffer's estimate is the max over its channels.  Every
+  // power-of-two rescaling of the network that computes the same function scales the estimate by the same power.
+  int* act_exp = (int*)H(c->act_exp);
+  std::vector<double> est(c->bufs.size(), 0.0);
   // conv1_1: [36][64], k = (ky*3+kx)*4 + cin                                       model.py:13
   {
     const HostTensor* w = find(c, "model1.0.weight");
@@ -316,6 +355,11 @@ int pack_weights(Ctx* c, char* host) {
       for (int ci = 0; ci < 4; ++ci)
         for (int t = 0; t < 9; ++t) dst[(t * 4 + ci) * 64 + co] = w->data[((size_t)co * 4 + ci) * 9 + t];
     memcpy(H(c->b11), b->data.data(), 64 * sizeof(float));
+    const int a11 = c->buf_index.at("a1_1");
+    for (int co = 0; co < 64; ++co)      // the packed input planes count as magnitude 1
+      est[a11] = std::max(est[a11], sqrt(sumsq(w->data.data() + (size_t)co * 36, 36)) + fabs((double)b->data[co]));
+    const int rc = set_act_exp(c, act_exp, a11, est[a11]);
+    if (rc != IDC_OK) return rc;
   }
   {
     const HostTensor* w = find(c, "model_out.0.weight");
@@ -349,6 +393,34 @@ int pack_weights(Ctx* c, char* host) {
         return fail(c, IDC_ERR_KEY, "missing/bad %s.*", op.bnkey.c_str());
       fold_bn(*g, *b, *m, *v, op.cout, scale, shift);
     }
+    if (op.out_buf >= 0 && c->bufs[op.out_buf].H > 0) {
+      double& e_out = est[op.out_buf];
+      for (int co = 0; co < op.cout; ++co) {
+        double v = 0.0;
+        if (op.epi.has_bn) {
+          auto t = [&](const char* sfx) { return (double)find(c, op.bnkey + sfx)->data[co]; };
+          const double var = t(".running_var"), mean = t(".running_mean");
+          v = fabs(t(".weight")) * sqrt(var + mean * mean) / sqrt(var + (double)kBnEps) + fabs(t(".bias"));
+        } else {
+          double bsum = 0.0;
+          for (int s = 0; s < op.nsrc; ++s) {
+            const int cin = op.src[s].cin, kk = op.src_k[s] * op.src_k[s];
+            const float* wd = w[s]->data.data();
+            double n2 = 0.0;
+            if (op.src_deconv[s])   // [cin][cout][k][k]
+              for (int ci = 0; ci < cin; ++ci) n2 += sumsq(wd + ((size_t)ci * op.cout + co) * kk, kk);
+            else
+              n2 = sumsq(wd + (size_t)co * cin * kk, (size_t)cin * kk);
+            v += sqrt(n2) * est[op.src[s].buf];
+            bsum += (double)find(c, op.wkey[s] + ".bias")->data[co];
+          }
+          v += fabs(bsum);
+        }
+        e_out = std::max(e_out, v);
+      }
+      const int rc = set_act_exp(c, act_exp, op.out_buf, e_out);
+      if (rc != IDC_OK) return rc;
+    }
     // weight value of (class, tap, ci, co)
     auto wval = [&](int cls, int t, int ci, int co) -> float {
       const Tap& tp = op.taps[cls][t];
@@ -374,6 +446,13 @@ int pack_weights(Ctx* c, char* host) {
     } else {
       // K-major FP16 hi/lo rows, one row per (class, cout); per-output-channel power-of-two scale so
       // the lo term stays in FP16's normal range; the epilogue multiplies by 1/scale (exact).
+      // Sources stored at different exponents share one accumulator at source 0's: source s's weights are
+      // pre-multiplied by 2^(S_0 - S_s) (exact), so every product carries 2^(S_0 + e).
+      const int s_in = c->bufs[op.src[0].buf].exp;
+      const int s_out = (op.out_f32 || op.fuse_out_head) ? 0 : c->bufs[op.out_buf].exp;
+      float srcmul[kMaxSrc];
+      for (int s = 0; s < op.nsrc; ++s) srcmul[s] = ldexpf(1.f, s_in - c->bufs[op.src[s].buf].exp);
+      auto wq = [&](int cls, int t, int ci, int co) { return wval(cls, t, ci, co) * srcmul[op.taps[cls][t].src]; };
       __half* hi = (__half*)H(op.w_hi);
       __half* lo = (__half*)H(op.w_lo);
       memset(hi, 0, sizeof(__half) * (size_t)op.ncls * op.K * op.cout_pad);
@@ -383,7 +462,7 @@ int pack_weights(Ctx* c, char* host) {
         for (int cls = 0; cls < op.ncls; ++cls)
           for (int t = 0; t < op.ntaps; ++t) {
             const int cin = op.src[op.taps[cls][t].src].cin;
-            for (int ci = 0; ci < cin; ++ci) mx = fmaxf(mx, fabsf(wval(cls, t, ci, co)));
+            for (int ci = 0; ci < cin; ++ci) mx = fmaxf(mx, fabsf(wq(cls, t, ci, co)));
           }
         int e = 0;
         if (mx > 0.f) {
@@ -392,18 +471,17 @@ int pack_weights(Ctx* c, char* host) {
           e = std::max(-24, std::min(24, e));
         }
         const float sc = ldexpf(1.f, e);
-        // acc = sum (a * 2^S)(w * 2^e); stored output = v * 2^Sout  (all exact powers of two)
-        const int sout = (op.out_f32 || op.fuse_out_head) ? 0 : kActScaleLog2;
-        bias[co] = ldexpf(bias[co], e + kActScaleLog2);
-        scale[co] = ldexpf(scale[co], -(e + kActScaleLog2) + sout);
-        shift[co] = ldexpf(shift[co], sout);
+        // acc = sum (a * 2^S_in)(w * 2^e); stored output = v * 2^S_out  (all exact powers of two)
+        bias[co] = ldexpf(bias[co], e + s_in);
+        scale[co] = ldexpf(scale[co], -(e + s_in) + s_out);
+        shift[co] = ldexpf(shift[co], s_out);
         for (int cls = 0; cls < op.ncls; ++cls) {
           int k0 = 0;
           for (int t = 0; t < op.ntaps; ++t) {
             const int cin = op.src[op.taps[cls][t].src].cin;
             for (int ci = 0; ci < cin; ++ci) {
               const size_t idx = ((size_t)cls * op.cout_pad + co) * op.K + k0 + ci;
-              split_f16(wval(cls, t, ci, co) * sc, hi[idx], lo[idx]);
+              split_f16(wq(cls, t, ci, co) * sc, hi[idx], lo[idx]);
             }
             k0 += cin;
           }
@@ -710,6 +788,16 @@ int idc_create(int device, int max_n, int h, int w, unsigned flags, idc_ctx** ou
 
 int idc_set_option(idc_ctx* c, const char* name, int value) {
   if (!c || !name) return IDC_ERR_ARG;
+  if (!strncmp(name, "act_exp.", 8)) {     // storage exponent of one buffer: baked into the packed weights
+    auto it = c->buf_index.find(name + 8);
+    if (it == c->buf_index.end() || c->bufs[it->second].H == 0) return fail(c, IDC_ERR_KEY, "no activation '%s'", name + 8);
+    if (value < kActExpMin || value > kActExpMax)
+      return fail(c, IDC_ERR_ARG, "%s = %d outside [%d, %d]", name, value, kActExpMin, kActExpMax);
+    if (c->weights_adopted)
+      return fail(c, IDC_ERR_STATE, "%s must be set before the weights are packed (idc_finalize_weights)", name);
+    c->act_exp_override[name + 8] = value;
+    return IDC_OK;
+  }
   struct { const char* n; int* v; } tab[] = {
       {"halo", &c->opt.halo}, {"pairs", &c->opt.pairs}, {"mt", &c->opt.mt},
       {"chunk_kb", &c->opt.chunk_kb}, {"split_k", &c->opt.split_k}, {"host_pipe", &c->opt.host_pipe},
@@ -784,6 +872,9 @@ int idc_adopt_weights(idc_ctx* c) {
   // conv1_1 takes its weights as a kernel parameter: read them back from the (possibly received) arena
   CUDA_TRY(c, cudaMemcpy(c->h_w11.w, c->w11, sizeof(c->h_w11.w), cudaMemcpyDeviceToHost));
   CUDA_TRY(c, cudaMemcpy(c->h_w11.b, c->b11, sizeof(c->h_w11.b), cudaMemcpyDeviceToHost));
+  std::vector<int> exps(c->bufs.size());
+  CUDA_TRY(c, cudaMemcpy(exps.data(), c->act_exp, exps.size() * sizeof(int), cudaMemcpyDeviceToHost));
+  for (size_t i = 0; i < exps.size(); ++i) c->bufs[i].exp = exps[i];
   if (!c->simt) CUDA_TRY(c, conv1_1_umma_pack(c));      // tensor-core conv1_1: derived on the device, so ranks != 0 need nothing extra
   int rc = plan_engines(c);                             // sets weights_ready
   if (rc != IDC_OK) return rc;
@@ -1443,6 +1534,15 @@ int idc_rgb_sse(int device, int n, int h, int w, const uint8_t* a, const uint8_t
   if (n < 1 || n > 65535 || h < 1 || w < 1 || !a || !b || !sse) return IDC_ERR_ARG;
   if (cudaSetDevice(device) != cudaSuccess) return IDC_ERR_CUDA;
   return launch_rgb_sse(n, (size_t)h * w * 3, a, b, sse, (cudaStream_t)stream) == cudaSuccess ? IDC_OK : IDC_ERR_CUDA;
+}
+
+int idc_act_exponent(idc_ctx* c, const char* name, int* exp_out) {
+  if (!c || !name || !exp_out) return IDC_ERR_ARG;
+  auto it = c->buf_index.find(name);
+  if (it == c->buf_index.end() || c->bufs[it->second].H == 0) return fail(c, IDC_ERR_KEY, "no activation '%s'", name);
+  if (!c->weights_ready) return fail(c, IDC_ERR_STATE, "idc_act_exponent before idc_finalize_weights");
+  *exp_out = c->bufs[it->second].exp;
+  return IDC_OK;
 }
 
 int idc_get_activation(idc_ctx* c, const char* name, float* out, size_t out_floats, int* ch, int* h, int* w) {

@@ -46,13 +46,17 @@ constexpr int kMaxCls = 4;    // output parity classes of a stride-2 transposed 
 
 enum Act { ACT_NONE = 0, ACT_RELU = 1, ACT_LEAKY02 = 2 };
 
-// wgmma engine: activations are stored as FP16 hi/lo planes of (value * 2^kActScaleLog2).
-// The scale keeps the lo plane out of the FP16 subnormal range (tensor cores may flush subnormal
-// operands to zero, which would drop the low half of every small activation): scaling by 64 keeps
-// lo normal down to |a| = 0.002; FP16 range then covers |a| < 1023.
-constexpr int kActScaleLog2 = 6;
-constexpr float kActScale = 64.0f;
-constexpr float kActInvScale = 1.0f / 64.0f;
+// wgmma engine: buffer b is stored as FP16 hi/lo planes of (value * 2^S_b), one exponent per buffer (ActBuf::exp),
+// chosen from the weights when they are packed (DESIGN §3): S_b = kActExpRef - ceil(log2 est_b), where est_b is a
+// magnitude estimate of the buffer propagated through the plan from the weights alone.  It puts the estimate in
+// (2^(kActExpRef-1), 2^kActExpRef], far below FP16's 65504 and far above the range where the lo plane goes subnormal.
+// A network whose exponents fall outside [kActExpMin, kActExpMax] is refused (the per-channel weight exponent, clamped
+// to +-24, could not absorb the shift exactly any more).
+constexpr int kActExpRef = 7;
+constexpr int kActExpMin = -24, kActExpMax = 24;
+// conv1_1's packed input (L/100, ab/110, mask - maskcent: |x| <= ~1 by construction) is split at this fixed exponent
+constexpr int kInExp = 6;
+constexpr float kInScale = 64.0f;   // 2^kInExp
 
 // One filter tap of a gather-GEMM convolution.  For logical output pixel (y, x) the tap reads
 // source pixel (y*s + ty, x*s + tx) of source `src`; out-of-range pixels read zero
@@ -64,10 +68,11 @@ struct Tap {
 };
 
 // Activation buffer.  SIMT engine: p0 = float [N,H,W,C].  wgmma engine: p0/p1 = __half
-// hi/lo planes, each [N,H,W,C]; value = hi + lo.
+// hi/lo planes, each [N,H,W,C]; value = (hi + lo) * 2^-exp.
 struct ActBuf {
   std::string name;
   int H = 0, W = 0, C = 0;
+  int exp = 0;   // wgmma engine: storage exponent S_b (0 on the SIMT engine, whose planes are FP32 values)
   DevMem<void> p0, p1;
 };
 
@@ -190,6 +195,8 @@ struct Ctx {
   // weight arena
   DevMem<char> arena;
   size_t arena_bytes = 0;
+  int* act_exp = nullptr;         // [bufs.size()] storage exponents, in the arena so that adopting ranks read them too
+  std::map<std::string, int> act_exp_override;   // idc_set_option("act_exp.<buffer>"): applied at the next pack
   bool weights_ready = false;     // adopted and planned: forwards may run
   bool weights_adopted = false;   // idc_adopt_weights succeeded and no tensor was loaded since: option changes re-plan
   // conv1_1 (4->64) + regression head + misc small weights (device fp32)

@@ -50,7 +50,7 @@ struct UmmaParams {
   const float* shift;
   const float* gadd;   // [n_img][gadd_ld] or null
   int gadd_ld;
-  float gadd_mult;     // output activation scale (2^kActScaleLog2) applied to the global-hints vector
+  float gadd_mult;     // output buffer's storage scale 2^S_out, applied to the global-hints vector
   int act;
   __half* out_hi;
   __half* out_lo;
@@ -686,7 +686,7 @@ umma_conv_kernel(const __grid_constant__ CUtensorMap bmap_hi, const __grid_const
 // (4 -> 64, 3x3, ReLU; model.py:13-14) as ONE padded k-block.  K = 9 taps x 4 channels = 36 -> 48 (three K=16 steps).
 // There is no 16-byte granule to aim a TMA box at (a tap contributes 4 channels = 8 bytes), so the 128 threads of a CTA
 // (one warpgroup) gather and normalise their pixel's 36 inputs themselves, split them into FP16 hi / lo (x 2^6, like
-// every activation) and write their row of the two K-major SWIZZLE_128B operand tiles directly; the 64 x 48 weight tile
+// kInExp) and write their row of the two K-major SWIZZLE_128B operand tiles directly; the 64 x 48 weight tile
 // (hi / lo, pre-swizzled by conv1_1_pack_kernel) stays in shared memory for the life of the CTA.  9 wgmmas per 64-row
 // half (lo*hi, hi*lo, hi*hi per K step) replace 2304 FFMAs per pixel.  4 CTAs per SM hide each other's gather / MMA /
 // epilogue phases (no intra-CTA pipeline).
@@ -700,8 +700,10 @@ __device__ __forceinline__ uint32_t sw128_off(int row, int chunk) {   // byte of
 }
 
 // one thread per output channel: power-of-two scale so the largest weight lands in [256, 512), hi/lo split, swizzled
-// smem image of the [64 cout][48 k] tile (k = tap * 4 + cin, zero beyond 36), bias' = bias * 2^6 * 2^e, scale' = 2^-e
-__global__ void conv1_1_pack_kernel(const float* __restrict__ w36x64, const float* __restrict__ bias, uint8_t* __restrict__ out) {
+// smem image of the [64 cout][48 k] tile (k = tap * 4 + cin, zero beyond 36), bias' = bias * 2^kInExp * 2^e,
+// scale' = 2^(s_out - kInExp - e) (s_out: a1_1's storage exponent)
+__global__ void conv1_1_pack_kernel(const float* __restrict__ w36x64, const float* __restrict__ bias, int s_out,
+                                    uint8_t* __restrict__ out) {
   const int co = threadIdx.x;
   if (co >= 64) return;
   float mx = 0.f;
@@ -719,8 +721,8 @@ __global__ void conv1_1_pack_kernel(const float* __restrict__ w36x64, const floa
     bh[o] = hi; bl[o] = lo;
   }
   float* vec = reinterpret_cast<float*>(out + 16384);
-  vec[co] = bias[co] * kActScale * sc;
-  vec[64 + co] = ldexpf(1.f, -e);
+  vec[co] = bias[co] * kInScale * sc;
+  vec[64 + co] = ldexpf(1.f, s_out - kInExp - e);
 }
 
 template <bool SPLIT>
@@ -784,7 +786,7 @@ conv1_1_umma_kernel(const uint8_t* __restrict__ pack, const float* __restrict__ 
       uint32_t hw[4], lw[4];
 #pragma unroll
       for (int q = 0; q < 4; ++q) {
-        const float v0 = in[8 * j + 2 * q] * kActScale, v1 = in[8 * j + 2 * q + 1] * kActScale;
+        const float v0 = in[8 * j + 2 * q] * kInScale, v1 = in[8 * j + 2 * q + 1] * kInScale;
         hw[q] = pack_f16x2_sat(v0, v1);
         lw[q] = lo_f16x2(v0, v1, hw[q]);
       }
@@ -829,7 +831,7 @@ conv1_1_umma_kernel(const uint8_t* __restrict__ pack, const float* __restrict__ 
     wgmma_wait<0>();
     wgmma_reg_fence(acc[0]);
     wgmma_reg_fence(acc[1]);
-    // ---- epilogue: relu(acc + bias') * scale' = 2^6 * relu(conv + b) -> hi / lo -> coalesced stores ----
+    // ---- epilogue: relu(acc + bias') * scale' = 2^S(a1_1) * relu(conv + b) -> hi / lo -> coalesced stores ----
 #pragma unroll
     for (int m = 0; m < 2; ++m)
 #pragma unroll
@@ -870,7 +872,7 @@ cudaError_t conv1_1_umma_pack(Ctx* c) {
     cudaError_t e = cudaMalloc(c->w11_umma.put(), kC11PackBytes);
     if (e != cudaSuccess) return e;
   }
-  conv1_1_pack_kernel<<<1, 64>>>(c->w11, c->b11, c->w11_umma.get());
+  conv1_1_pack_kernel<<<1, 64>>>(c->w11, c->b11, c->bufs[c->buf_index.at("a1_1")].exp, c->w11_umma.get());
   cudaError_t e = cudaGetLastError();
   return e != cudaSuccess ? e : cudaDeviceSynchronize();
 }
@@ -1164,7 +1166,7 @@ int umma_plan_op(Ctx* c, ConvOp& op) {
   while ((1 << q.wshift) < op.wbox) q.wshift++;
   q.Hl = op.Hl; q.Wl = op.Wl; q.cout_pad = op.cout_pad;
   q.bias = op.epi.bias; q.scale = op.epi.scale; q.shift = op.epi.shift;
-  q.gadd = nullptr; q.gadd_ld = 512; q.gadd_mult = kActScale;
+  q.gadd = nullptr; q.gadd_ld = 512; q.gadd_mult = op.out_buf >= 0 ? ldexpf(1.f, c->bufs[op.out_buf].exp) : 1.f;
   q.act = op.epi.act;
   if (op.out_f32) {
     q.out_f32 = op.out_f32_ptr; q.out_ld = op.cout_pad;

@@ -33,7 +33,7 @@ class LhnContext(object):
                  global_hints=False, use_graph=True, keep_conv10=False, caffe313=False, options=None):
         """engine: "wgmma" (tensor cores; "tcgen05" is accepted as the name earlier releases used) or "simt"
         (exact FP32 CUDA cores).  options: {name: int} plan-time switches, see include/idc_b200.h: idc_set_option
-        (halo, pairs, mt, chunk_kb, split_k, host_pipe, pdl, side_dist, conv1_1_umma, tanh_scale)."""
+        (halo, pairs, mt, chunk_kb, split_k, host_pipe, pdl, side_dist, conv1_1_umma, tanh_scale, act_exp.<buffer>)."""
         self.lib = _lib.load()
         flags = 0
         if dist:
@@ -290,6 +290,12 @@ class LhnContext(object):
         _lib.check(self.h, self.lib.idc_get_activation(self.h, name.encode(), None, 0, ctypes.byref(c),
                                                        ctypes.byref(h), ctypes.byref(w)))
         return c.value, h.value, w.value
+
+    def act_exponent(self, name):
+        """The exponent S with which the wgmma engine stores activation `name` (value * 2^S in FP16 hi/lo)."""
+        e = ctypes.c_int()
+        _lib.check(self.h, self.lib.idc_act_exponent(self.h, name.encode(), ctypes.byref(e)))
+        return e.value
 
     def get_activation(self, name, n):
         import torch

@@ -34,11 +34,11 @@ def synthetic_glob_state_dict(seed=4321):
     return sd
 
 
-def global_hints_vector(gsd, glob316):
+def global_hints_vector(gsd, glob316, dtype=torch.float32):
     """glob316 [N,316] = [313 histogram, indicator, mean saturation, indicator] -> [N,512]."""
-    x = torch.as_tensor(np.asarray(glob316), dtype=torch.float32)
+    x = torch.as_tensor(np.asarray(glob316), dtype=dtype)
     for l in range(4):
-        t = lambda k: torch.as_tensor(np.asarray(gsd["glob.%d.%s" % (l, k)]), dtype=torch.float32)
+        t = lambda k: torch.as_tensor(np.asarray(gsd["glob.%d.%s" % (l, k)]), dtype=dtype)
         x = F.relu(F.linear(x, t("weight"), t("bias")))
         x = F.batch_norm(x, t("bn.running_mean"), t("bn.running_var"), t("bn.weight"), t("bn.bias"), False, 0.0, BN_EPS)
     return x

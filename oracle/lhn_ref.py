@@ -12,41 +12,42 @@ import torch.nn.functional as F
 BN_EPS = 1e-5  # torch BatchNorm2d default (SURVEY q7)
 
 
-def _t(x):
+def _t(x, dtype=torch.float32):
     if isinstance(x, np.ndarray):
-        return torch.from_numpy(np.ascontiguousarray(x)).float()
-    return x.float()
+        return torch.from_numpy(np.ascontiguousarray(x)).to(dtype)
+    return x.to(dtype)
 
 
 def _conv(sd, key, x, dilation=1):
     # nn.Conv2d(k=3, stride 1, padding=dilation) model.py:13-101 ; 1x1 heads :105,:108
-    w = _t(sd[key + ".weight"])
+    w = _t(sd[key + ".weight"], x.dtype)
     pad = dilation * (w.shape[-1] // 2)
-    return F.conv2d(x, w, _t(sd[key + ".bias"]), stride=1, padding=pad, dilation=dilation)
+    return F.conv2d(x, w, _t(sd[key + ".bias"], x.dtype), stride=1, padding=pad, dilation=dilation)
 
 
 def _deconv(sd, key, x):
     # nn.ConvTranspose2d(k=4, stride 2, padding 1) model.py:75,86,96
-    return F.conv_transpose2d(x, _t(sd[key + ".weight"]), _t(sd[key + ".bias"]), stride=2, padding=1)
+    return F.conv_transpose2d(x, _t(sd[key + ".weight"], x.dtype), _t(sd[key + ".bias"], x.dtype), stride=2, padding=1)
 
 
 def _bn(sd, key, x):
     # eval-mode BatchNorm2d (data/colorize_image.py:232 net.eval()) model.py:17...93
-    return F.batch_norm(x, _t(sd[key + ".running_mean"]), _t(sd[key + ".running_var"]),
-                        _t(sd[key + ".weight"]), _t(sd[key + ".bias"]), False, 0.0, BN_EPS)
+    t = lambda s: _t(sd[key + s], x.dtype)
+    return F.batch_norm(x, t(".running_mean"), t(".running_var"), t(".weight"), t(".bias"), False, 0.0, BN_EPS)
 
 
 def lhn_forward(sd, L_mc, ab, mask, maskcent=0.0, dist=False, glob_add=None, ref_quirks=True,
-                return_intermediates=False):
+                return_intermediates=False, dtype=torch.float32):
     """L_mc [N,1,H,W] in [-50,50]; ab [N,2,H,W] in [-110,110]; mask [N,1,H,W] in [0,1].
     Returns out_reg [N,2,H,W] (dist=False) or (out_reg_quirk, dist[N,529,H/4,W/4]) -- the
     nearest x4 upsample (model.py:160 upsample4) is NOT materialised here; use
     `upsample4()` below.  glob_add [N,512] is broadcast-added to conv4_3 (row a15).
-    With ref_quirks the dist=True regression output is tanh*110*110 (model.py:166-168, q1)."""
+    With ref_quirks the dist=True regression output is tanh*110*110 (model.py:166-168, q1).
+    dtype=torch.float64 evaluates the same network in double precision (inputs and weights converted)."""
     inter = {}
-    A = _t(L_mc)
-    B = _t(ab)
-    M = _t(mask) - maskcent                                              # model.py:142
+    A = _t(L_mc, dtype)
+    B = _t(ab, dtype)
+    M = _t(mask, dtype) - maskcent                                              # model.py:142
     x = torch.cat((A / 100.0, B / 110.0, M), dim=1)                      # model.py:148
     # model1 (:13-17)
     h = F.relu(_conv(sd, "model1.0", x)); inter["a1_1"] = h
@@ -68,7 +69,7 @@ def lhn_forward(sd, L_mc, ab, mask, maskcent=0.0, dist=False, glob_add=None, ref
     conv4_3 = _bn(sd, "model4.6", h)
     if glob_add is not None:
         # models/global_model/deploy_nodist.prototxt:501-527: SpatialRep + Eltwise SUM on conv4_3norm
-        conv4_3 = conv4_3 + _t(glob_add)[:, :, None, None]
+        conv4_3 = conv4_3 + _t(glob_add, dtype)[:, :, None, None]
     inter["conv4_3"] = conv4_3
     # model5, model6 dilation 2 (:48-63), model7 (:66-72)
     h = conv4_3

@@ -45,7 +45,12 @@ enum {
   IDC_ERR_STATE = -3,        /* wrong call order (e.g. forward before finalize)     */
   IDC_ERR_KEY = -4,          /* unknown / missing state_dict key                    */
   IDC_ERR_UNSUPPORTED = -5,  /* e.g. not an sm_90 device                            */
-  IDC_ERR_WATCHDOG = -6      /* a device-side pipeline wait timed out               */
+  IDC_ERR_WATCHDOG = -6,     /* a device-side pipeline wait timed out               */
+  IDC_ERR_RANGE = -7         /* an activation reached 65504, FP16's largest value, at its storage exponent
+                                (wgmma engine; |v| >= 65488, and values above 65504 saturated).  idc_last_error
+                                names the buffers.  idc_forward_host(_q) return it from the forward that saturated;
+                                after an idc_forward, the next forward call on the context returns it (before
+                                running). */
 };
 
 /* idc_create flags */

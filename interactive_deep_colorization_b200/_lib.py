@@ -15,6 +15,8 @@ if os.environ.get("IDC_B200_LIB"):            # tools only: a build elsewhere (m
     LIB_PATH = os.environ["IDC_B200_LIB"]
 
 IDC_OK = 0
+# error codes (include/idc_b200.h)
+ERR_ARG, ERR_CUDA, ERR_STATE, ERR_KEY, ERR_UNSUPPORTED, ERR_WATCHDOG, ERR_RANGE = -1, -2, -3, -4, -5, -6, -7
 FLAG_DIST = 1 << 0
 FLAG_ENGINE_SIMT = 1 << 1
 FLAG_FAST_FP16 = 1 << 2

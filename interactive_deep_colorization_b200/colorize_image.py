@@ -908,14 +908,20 @@ class ColorizeImageB200CaffeDist(_DistPlots, ColorizeImageB200Caffe):
         dA, dB, dM = (torch.from_numpy(a).to(dev) for a in (A, B, M))
         self._ctx.forward_device(dA, dB, dM, 0.0)                      # trunk + hyper-column + pred_313 logits
         pred = self._ctx.caffe313_pred_ab(1, T=2.6)                    # annealed-mean `pred_ab` [1,2,X,X] (device)
-        rgb = torch.empty((1, self.Xd, self.Xd, 3), dtype=torch.uint8, device=dev)
-        L = (dA + 50.0).contiguous()
+        # lab2rgb_transpose(self.img_l, pred_ab) (data/colorize_image.py:20-28) on the float64 L plane the reference
+        # converts, not on the FP32 L - 50 the network reads (an FP32 ulp of L can flip a truncating cast): an order-0
+        # render at the net size samples pred_ab exactly
+        Xd = self.Xd
+        d_L = torch.from_numpy(np.ascontiguousarray(self.img_l, dtype=np.float64).reshape(Xd, Xd)).to(dev)
+        d_ab = pred[0].double().contiguous()
+        rgb = torch.empty((Xd, Xd, 3), dtype=torch.uint8, device=dev)
         st = torch.cuda.current_stream(self._ctx.device).cuda_stream
-        rc = _lib.load().idc_lab2rgb_u8(self._ctx.device, 1, self.Xd, self.Xd, L.data_ptr(), pred.data_ptr(), rgb.data_ptr(), st)
+        rc = _lib.load().idc_render_planes_u8(self._ctx.device, Xd, Xd, d_ab.data_ptr(), 0, 0, None, 0,
+                                              _lib.RENDER_L_PLANE, d_L.data_ptr(), Xd, Xd, rgb.data_ptr(), st)
         if rc != _lib.IDC_OK:
-            raise _lib.IdcError(rc, "idc_lab2rgb_u8 failed")
+            raise _lib.IdcError(rc, "idc_render_planes_u8 failed")
         self.output_ab_raw = pred[0].cpu().numpy()
-        self.output_rgb = rgb[0].cpu().numpy()
+        self.output_rgb = rgb.cpu().numpy()
         self._set_out_ab_()
         self.dist_ab = _LazyDist313(self._ctx, self.Xd, self.S)
         self.dist_ab_set = True

@@ -305,25 +305,31 @@ void fold_bn(const HostTensor& g, const HostTensor& b, const HostTensor& m, cons
   }
 }
 
-// Storage exponent of buffer b from its magnitude estimate (DESIGN §3): S_b = kActExpRef - ceil(log2 est_b), or the
-// act_exp.<name> override.  Writes it to the arena table and the buffer; fails, naming the buffer, outside the range.
-int set_act_exp(Ctx* c, int* table, int b, double est) {
+// ref - ceil(log2 est), or ref for est = 0
+int exp_below(int ref, double est) {
+  if (!(est > 0.0)) return ref;
+  int ex = 0;
+  const double f = frexp(est, &ex);          // est = f * 2^ex, f in [0.5, 1): ceil(log2 est) = ex, or ex - 1 at f = 0.5
+  return ref - (f == 0.5 ? ex - 1 : ex);
+}
+
+// Storage exponent of buffer b from its magnitude estimate est and, for the outputs of convs without a BatchNorm, its
+// bound (DESIGN §3): S_b = min(kActExpRef - ceil(log2 est_b), kActExpBound - ceil(log2 bound_b)), or the act_exp.<name>
+// override.  bound < 0: none.  Writes it to the arena table and the buffer; fails, naming the buffer, outside the range.
+int set_act_exp(Ctx* c, int* table, int b, double est, double bound) {
   ActBuf& buf = c->bufs[b];
   int s = 0;
   if (!c->simt) {
-    if (!std::isfinite(est)) return fail(c, IDC_ERR_ARG, "activation %s: magnitude estimate %g is not finite", buf.name.c_str(), est);
-    s = kActExpRef;
-    if (est > 0.0) {
-      int ex = 0;
-      const double f = frexp(est, &ex);          // est = f * 2^ex, f in [0.5, 1): ceil(log2 est) = ex, or ex - 1 at f = 0.5
-      s = kActExpRef - (f == 0.5 ? ex - 1 : ex);
-    }
+    if (!std::isfinite(est) || !std::isfinite(bound))
+      return fail(c, IDC_ERR_ARG, "activation %s: magnitude estimate %g / bound %g is not finite", buf.name.c_str(), est, bound);
+    s = exp_below(kActExpRef, est);
+    if (bound >= 0.0) s = std::min(s, exp_below(kActExpBound, bound));
     auto ov = c->act_exp_override.find(buf.name);
     if (ov != c->act_exp_override.end()) s = ov->second;
     if (s < kActExpMin || s > kActExpMax)
       return fail(c, IDC_ERR_UNSUPPORTED,
-                  "activation %s: storage exponent %d (magnitude estimate %g) is outside the supported range [%d, %d]",
-                  buf.name.c_str(), s, est, kActExpMin, kActExpMax);
+                  "activation %s: storage exponent %d (magnitude estimate %g, bound %g) is outside the supported range [%d, %d]",
+                  buf.name.c_str(), s, est, bound, kActExpMin, kActExpMax);
   }
   table[b] = s;
   buf.exp = s;
@@ -336,15 +342,24 @@ double sumsq(const float* p, size_t n) {
   return a;
 }
 
+double sumabs(const float* p, size_t n) {
+  double a = 0.0;
+  for (size_t i = 0; i < n; ++i) a += fabs((double)p[i]);
+  return a;
+}
+
 int pack_weights(Ctx* c, char* host) {
   // translate device pointers (already laid out relative to c->arena) to host staging pointers
   auto H = [&](void* dev) { return host + ((char*)dev - c->arena.get()); };
   // magnitude estimates of the buffers, in plan order (FP64): conv output channel co of an op reading sources s is
   // sum_s ||W_s[co]||_2 * est(s) + |bias_co|; a BatchNorm output restarts from its statistics,
-  // |gamma| * sqrt(var + mean^2) / sqrt(var + eps) + |beta|; the buffer's estimate is the max over its channels.  Every
-  // power-of-two rescaling of the network that computes the same function scales the estimate by the same power.
+  // |gamma| * sqrt(var + mean^2) / sqrt(var + eps) + |beta|; the buffer's estimate is the max over its channels.
+  // Outputs of convs without a BatchNorm also get a bound: the max over channels and output-parity classes of
+  // sum_s ||W_s[co, class]||_1 * bound(s) + |bias_co|, with bound = est at a BatchNorm output and 1 for the packed
+  // conv1_1 input; it holds whenever the BatchNorm outputs stay within their estimates.  Every power-of-two rescaling of
+  // the network that computes the same function scales estimate and bound by the same power.
   int* act_exp = (int*)H(c->act_exp);
-  std::vector<double> est(c->bufs.size(), 0.0);
+  std::vector<double> est(c->bufs.size(), 0.0), bound(c->bufs.size(), 0.0);
   // conv1_1: [36][64], k = (ky*3+kx)*4 + cin                                       model.py:13
   {
     const HostTensor* w = find(c, "model1.0.weight");
@@ -356,9 +371,12 @@ int pack_weights(Ctx* c, char* host) {
         for (int t = 0; t < 9; ++t) dst[(t * 4 + ci) * 64 + co] = w->data[((size_t)co * 4 + ci) * 9 + t];
     memcpy(H(c->b11), b->data.data(), 64 * sizeof(float));
     const int a11 = c->buf_index.at("a1_1");
-    for (int co = 0; co < 64; ++co)      // the packed input planes count as magnitude 1
-      est[a11] = std::max(est[a11], sqrt(sumsq(w->data.data() + (size_t)co * 36, 36)) + fabs((double)b->data[co]));
-    const int rc = set_act_exp(c, act_exp, a11, est[a11]);
+    for (int co = 0; co < 64; ++co) {    // the packed input planes count as magnitude 1
+      const float* wc = w->data.data() + (size_t)co * 36;
+      est[a11] = std::max(est[a11], sqrt(sumsq(wc, 36)) + fabs((double)b->data[co]));
+      bound[a11] = std::max(bound[a11], sumabs(wc, 36) + fabs((double)b->data[co]));
+    }
+    const int rc = set_act_exp(c, act_exp, a11, est[a11], bound[a11]);
     if (rc != IDC_OK) return rc;
   }
   {
@@ -393,8 +411,18 @@ int pack_weights(Ctx* c, char* host) {
         return fail(c, IDC_ERR_KEY, "missing/bad %s.*", op.bnkey.c_str());
       fold_bn(*g, *b, *m, *v, op.cout, scale, shift);
     }
+    // weight value of (class, tap, ci, co)
+    auto wval = [&](int cls, int t, int ci, int co) -> float {
+      const Tap& tp = op.taps[cls][t];
+      const HostTensor* ww = w[tp.src];
+      const int cin = op.src[tp.src].cin, k = op.src_k[tp.src];
+      if (op.src_deconv[tp.src])  // ConvTranspose2d / Caffe Deconvolution weight is [Cin][Cout][k][k]
+        return ww->data[(((size_t)ci * op.cout + co) * k + tp.ky) * k + tp.kx];
+      return ww->data[(((size_t)co * cin + ci) * k + tp.ky) * k + tp.kx];
+    };
     if (op.out_buf >= 0 && c->bufs[op.out_buf].H > 0) {
       double& e_out = est[op.out_buf];
+      double& b_out = bound[op.out_buf];
       for (int co = 0; co < op.cout; ++co) {
         double v = 0.0;
         if (op.epi.has_bn) {
@@ -415,21 +443,23 @@ int pack_weights(Ctx* c, char* host) {
             bsum += (double)find(c, op.wkey[s] + ".bias")->data[co];
           }
           v += fabs(bsum);
+          for (int cls = 0; cls < op.ncls; ++cls) {   // the taps of one output-parity class reach one output pixel
+            double l1 = 0.0;
+            for (int t = 0; t < op.ntaps; ++t) {
+              const int s = op.taps[cls][t].src;
+              double a = 0.0;
+              for (int ci = 0; ci < op.src[s].cin; ++ci) a += fabs((double)wval(cls, t, ci, co));
+              l1 += a * bound[op.src[s].buf];
+            }
+            b_out = std::max(b_out, l1 + fabs(bsum));
+          }
         }
         e_out = std::max(e_out, v);
       }
-      const int rc = set_act_exp(c, act_exp, op.out_buf, e_out);
+      if (op.epi.has_bn) b_out = e_out;
+      const int rc = set_act_exp(c, act_exp, op.out_buf, e_out, op.epi.has_bn ? -1.0 : b_out);
       if (rc != IDC_OK) return rc;
     }
-    // weight value of (class, tap, ci, co)
-    auto wval = [&](int cls, int t, int ci, int co) -> float {
-      const Tap& tp = op.taps[cls][t];
-      const HostTensor* ww = w[tp.src];
-      const int cin = op.src[tp.src].cin, k = op.src_k[tp.src];
-      if (op.src_deconv[tp.src])  // ConvTranspose2d / Caffe Deconvolution weight is [Cin][Cout][k][k]
-        return ww->data[(((size_t)ci * op.cout + co) * k + tp.ky) * k + tp.kx];
-      return ww->data[(((size_t)co * cin + ci) * k + tp.ky) * k + tp.kx];
-    };
     if (c->simt) {
       float* dst = (float*)H(op.w_simt);
       memset(dst, 0, sizeof(float) * (size_t)op.ncls * op.K * op.cout_pad);
@@ -511,6 +541,7 @@ int pack_weights(Ctx* c, char* host) {
 }
 
 int alloc_workspace(Ctx* c) {
+  if (c->bufs.size() > kRangeInputBit) return fail(c, IDC_ERR_STATE, "%zu buffers: the range word has 31 bits", c->bufs.size());
   for (auto& b : c->bufs) {
     if (b.H == 0) continue;
     const size_t elems = (size_t)c->max_n * b.H * b.W * b.C;
@@ -535,6 +566,7 @@ int alloc_workspace(Ctx* c) {
   CUDA_TRY(c, cudaHostAlloc(c->h_err.put(), 64, cudaHostAllocMapped));
   memset(c->h_err.get(), 0, 64);
   CUDA_TRY(c, cudaHostGetDevicePointer(&c->d_err, c->h_err.get(), 0));
+  c->d_range = reinterpret_cast<unsigned*>(c->d_err + 1);
   CUDA_TRY(c, cudaStreamCreateWithFlags(c->own_stream.put(), cudaStreamNonBlocking));
   return IDC_OK;
 }
@@ -560,13 +592,28 @@ int plan_engines(Ctx* c) {
   return IDC_OK;
 }
 
-// a code the device watchdog left in the mapped flag: clear it and fail with msg (which formats the code)
-int take_watchdog(Ctx* c, const char* msg) {
+// a code the device watchdog left in the mapped flag: clear it and fail with msg (which formats the code); then the
+// buffers whose FP16 stores saturated since the last check: clear the word and fail with IDC_ERR_RANGE, naming them
+int take_device_flags(Ctx* c, const char* msg) {
   volatile int* flag = c->h_err.get();
-  const int werr = *flag;
-  if (!werr) return IDC_OK;
-  *flag = 0;
-  return fail(c, IDC_ERR_WATCHDOG, msg, werr);
+  const int werr = flag[0];
+  if (werr) {
+    flag[0] = 0;
+    return fail(c, IDC_ERR_WATCHDOG, msg, werr);
+  }
+  const unsigned range = (unsigned)flag[1];
+  if (!range) return IDC_OK;
+  flag[1] = 0;
+  std::string names;
+  for (unsigned b = 0; b < 32; ++b) {
+    if (!(range & (1u << b))) continue;
+    if (!names.empty()) names += ", ";
+    if (b == kRangeInputBit) names += "conv1_1 input";
+    else if (b < c->bufs.size()) names += c->bufs[b].name + " (S = " + std::to_string(c->bufs[b].exp) + ")";
+  }
+  return fail(c, IDC_ERR_RANGE,
+              "activation values reached 65504, FP16's largest value, at their storage exponent in: %s (values above it "
+              "saturated; lower the exponent with act_exp.<buffer>)", names.c_str());
 }
 
 // idc_forward_host's copy/compute overlap: the batch is cut into image chunks; conv1_1 of chunk k waits for the
@@ -897,7 +944,7 @@ int idc_forward(idc_ctx* c, int n, int h, int w, const float* L, const float* ab
   int rc = check_forward_args(c, n, h, w, L, ab, mask, glob, out_ab, out_dist);
   if (rc != IDC_OK) return rc;
   CUDA_TRY(c, cudaSetDevice(c->dev));
-  rc = take_watchdog(c, "device pipeline watchdog fired earlier (code %d)");   // left by an earlier (asynchronous) forward
+  rc = take_device_flags(c, "device pipeline watchdog fired earlier (code %d)");   // left by an earlier (asynchronous) forward
   if (rc != IDC_OK) return rc;
   return run_forward(c, n, L, ab, mask, maskcent, glob, out_ab, out_dist, out_rgb, (cudaStream_t)stream);
 }
@@ -1122,7 +1169,7 @@ int idc_forward_host_q(idc_ctx* c, int n, int h, int w, const float* L, const fl
       if (hs[i].img < 0 || hs[i].img >= n) return fail(c, IDC_ERR_ARG, "hint %d: img=%d outside [0,%d)", i, hs[i].img, n);
   }
   CUDA_TRY(c, cudaSetDevice(c->dev));
-  rc = take_watchdog(c, "device pipeline watchdog fired earlier (code %d)");   // left over from an asynchronous idc_forward
+  rc = take_device_flags(c, "device pipeline watchdog fired earlier (code %d)");   // left over from an asynchronous idc_forward
   if (rc != IDC_OK) return rc;
   const size_t HW = (size_t)c->H * c->W, HW4 = (size_t)(c->H / 4) * (c->W / 4);
   rc = ensure_host_staging(c);
@@ -1132,7 +1179,7 @@ int idc_forward_host_q(idc_ctx* c, int n, int h, int w, const float* L, const fl
   const bool use_graph = !(c->flags & IDC_FLAG_NO_GRAPH) && n <= 4;
   if (use_graph) {
     rc = forward_host_small(c, n, L, ab, mask, maskcent, glob, out_ab, out_dist, out_rgb, out_abq, hint_mode);
-    return rc != IDC_OK ? rc : take_watchdog(c, "device pipeline watchdog fired (code %d)");
+    return rc != IDC_OK ? rc : take_device_flags(c, "device pipeline watchdog fired (code %d)");
   }
   if (out_abq && !c->abq) {
     auto g = std::make_unique<AbqStaging>();
@@ -1226,7 +1273,7 @@ int idc_forward_host_q(idc_ctx* c, int n, int h, int w, const float* L, const fl
   c->dist_valid_n = want_dist ? n : 0;
   if (want_rgb && !is_pinned(out_rgb)) memcpy(out_rgb, sg.h_rgb.get(), n * HW * 3);
   if (out_abq && !is_pinned(out_abq)) memcpy(out_abq, c->abq->h_abq.get(), n * 2 * HW * sizeof(double));
-  return take_watchdog(c, "device pipeline watchdog fired (code %d)");
+  return take_device_flags(c, "device pipeline watchdog fired (code %d)");
 }
 
 void* idc_host_alloc(size_t bytes) {
@@ -1601,7 +1648,7 @@ int idc_get_profile(idc_ctx* c, float* ms, int max_slots) {
   if (max_slots < slots) return fail(c, IDC_ERR_ARG, "need %d slots", slots);
   CUDA_TRY(c, cudaSetDevice(c->dev));
   CUDA_TRY(c, cudaDeviceSynchronize());
-  const int rc = take_watchdog(c, "device pipeline watchdog fired (code %d)");
+  const int rc = take_device_flags(c, "device pipeline watchdog fired (code %d)");
   if (rc != IDC_OK) return rc;
   for (int i = 0; i < slots; ++i) ms[i] = 0.f;
   int runs = 0;

@@ -50,10 +50,18 @@ enum Act { ACT_NONE = 0, ACT_RELU = 1, ACT_LEAKY02 = 2 };
 // chosen from the weights when they are packed (DESIGN §3): S_b = kActExpRef - ceil(log2 est_b), where est_b is a
 // magnitude estimate of the buffer propagated through the plan from the weights alone.  It puts the estimate in
 // (2^(kActExpRef-1), 2^kActExpRef], far below FP16's 65504 and far above the range where the lo plane goes subnormal.
+// The output of a conv without a BatchNorm also has a bound (1-norms instead of 2-norms); S_b is lowered where needed
+// to keep the bound at or below 2^kActExpBound.
 // A network whose exponents fall outside [kActExpMin, kActExpMax] is refused (the per-channel weight exponent, clamped
 // to +-24, could not absorb the shift exactly any more).
 constexpr int kActExpRef = 7;
+constexpr int kActExpBound = 11;
 constexpr int kActExpMin = -24, kActExpMax = 24;
+// Every FP16 activation store whose hi part reaches 65504, FP16's largest value (|v| >= 65488; above 65504 the value
+// saturates there), sets bit `buffer index` of the context's range word; the packed conv1_1 input uses bit
+// kRangeInputBit.
+constexpr unsigned kRangeInputBit = 31;
+constexpr unsigned kF16MaxBits = 0x7BFFu;   // 65504
 // conv1_1's packed input (L/100, ab/110, mask - maskcent: |x| <= ~1 by construction) is split at this fixed exponent
 constexpr int kInExp = 6;
 constexpr float kInScale = 64.0f;   // 2^kInExp
@@ -224,8 +232,9 @@ struct Ctx {
   bool dbg_graph_timing = false; // experiments: events around the click graph launch (idc_debug_graph_timing)
   Event dbg_ev[2];
   float dbg_graph_ms = 0.f;
-  HostMem<int> h_err;          // watchdog flag (mapped pinned host memory: survives a device trap)
+  HostMem<int> h_err;          // [0] watchdog flag, [1] range word (mapped pinned host memory: survives a device trap)
   int* d_err = nullptr;
+  unsigned* d_range = nullptr; // device alias of h_err[1]: bit b = a store into buffer b saturated
   std::unique_ptr<HostStaging> stage;
   std::unique_ptr<AbqStaging> abq;
   Stream own_stream;

@@ -62,6 +62,8 @@ struct UmmaParams {
   float* out_ab;
   float out_mult;
   int* err;
+  unsigned* range;     // the context's range word: range_bit is set when a stored value exceeds FP16's 65504
+  unsigned range_bit;
   int n_amaps;         // entries of `amaps` (prefetched in the prologue)
   int max_ctas;        // host side only: grid cap for side-branch launches
   int img0;            // first image of this launch (n_img = img0 + images of the launch): idc_forward_host
@@ -243,6 +245,15 @@ __device__ __forceinline__ uint32_t pack_f16x2_sat(float a, float b) {
 __device__ __forceinline__ uint32_t lo_f16x2(float a, float b, uint32_t hw) {
   const float2 hf = __half22float2(*reinterpret_cast<const __half2*>(&hw));
   return pack_f16x2_sat(a - hf.x, b - hf.y);
+}
+// Range check of the FP16 stores: a running max of |h| over packed pairs (two calls fuse into one VHMNMX), and whether
+// it reached 65504, FP16's largest value: the value rounded to it (|v| >= 65488) or saturated there (|v| > 65504).
+__device__ __forceinline__ uint32_t habs_max2(uint32_t m, uint32_t w) {
+  const __half2 r = __hmax2(*reinterpret_cast<const __half2*>(&m), __habs2(*reinterpret_cast<const __half2*>(&w)));
+  return *reinterpret_cast<const uint32_t*>(&r);
+}
+__device__ __forceinline__ bool f16_top(uint32_t m) {     // m: a habs_max2 result (sign bits clear)
+  return ((m & 0xFFFFu) >= kF16MaxBits) | ((m >> 16) >= kF16MaxBits);
 }
 
 __device__ __forceinline__ void split_h(float v, __half& hi, __half& lo) {
@@ -432,6 +443,7 @@ umma_conv_kernel(const __grid_constant__ CUtensorMap bmap_hi, const __grid_const
     uint32_t phase = 0;
     uint32_t hcount = 0;                              // HALO: halo tiles consumed
     int staged_key = -1;
+    bool sat = false;                                 // a value this thread stored reached FP16's largest value
     for (int w = w0; w < n_items; w += wstep) {
       const int tile = w / S, ks = w - tile * S;
       const int kbeg = (ks * p.nkb) / S, kend = ((ks + 1) * p.nkb) / S;
@@ -576,6 +588,12 @@ umma_conv_kernel(const __grid_constant__ CUtensorMap bmap_hi, const __grid_const
 
       // ---- epilogue: v = act(acc + bias) * scale + shift on the register fragment, one 64-row block at a time ----
       const float neg_slope = p.act == ACT_RELU ? 0.f : (p.act == ACT_LEAKY02 ? 0.2f : 1.f);
+      unsigned own = ~0u;                               // the 32-column pieces this work item stores (split-K: 1 in S)
+      if (S > 1) {
+        own = 0u;
+#pragma unroll
+        for (int pc = 0; pc < BN / 32; ++pc) own |= (pc % S == ks ? 1u : 0u) << pc;
+      }
 #pragma unroll
       for (int m = 0; m < MT; ++m) {
         const int blk = (wg * MT + m) * 64;             // first tile row of this 64-row block
@@ -643,6 +661,9 @@ umma_conv_kernel(const __grid_constant__ CUtensorMap bmap_hi, const __grid_const
                          : nullptr;
           }
           const ptrdiff_t lo_delta = SPLIT ? p.out_lo - p.out_hi : 0;
+          // range check: max |hi| per row half and 32-column piece over the packed hi words (one VHMNMX per four
+          // values); only the rows and pieces this CTA stores count
+          uint32_t hmax[2][BN / 32] = {};
 #pragma unroll
           for (int sl = 0; sl < BN / 64; ++sl) {              // 64-column slabs = registers 32*sl .. 32*sl+31
             if (S > 1 && ((2 * sl) % S != ks) && ((2 * sl + 1) % S != ks)) continue;
@@ -651,6 +672,7 @@ umma_conv_kernel(const __grid_constant__ CUtensorMap bmap_hi, const __grid_const
 #pragma unroll
               for (int i = 32 * sl; i < 32 * sl + 32; i += 2) {
                 const uint32_t hw = pack_f16x2_sat(acc[m][i], acc[m][i + 1]);
+                if (plane == 0) hmax[(i >> 1) & 1][i >> 4] = habs_max2(hmax[(i >> 1) & 1][i >> 4], hw);
                 const uint32_t v = plane == 0 ? hw : lo_f16x2(acc[m][i], acc[m][i + 1], hw);
                 const int rl = (lane >> 2) + 8 * ((i >> 1) & 1), cl = frag_col(i, lane) - 64 * sl;
                 st_shared_u32(wbuf + rl * SP::kOutRow + cl * 2, v);
@@ -666,6 +688,14 @@ umma_conv_kernel(const __grid_constant__ CUtensorMap bmap_hi, const __grid_const
               __syncwarp();
             }
           }
+          uint32_t top = 0u;                               // over the rows and pieces this thread stores
+#pragma unroll
+          for (int pc = 0; pc < BN / 32; ++pc) {
+            const bool mine = (own >> pc) & 1u;
+            top = habs_max2(top, (mine & ok[0]) ? hmax[0][pc] : 0u);
+            top = habs_max2(top, (mine & ok[1]) ? hmax[1][pc] : 0u);
+          }
+          sat |= f16_top(top);
         }
       }
       if (S > 1) {
@@ -676,6 +706,7 @@ umma_conv_kernel(const __grid_constant__ CUtensorMap bmap_hi, const __grid_const
         }
       }
     }
+    if (__any_sync(0xffffffffu, sat) && lane == 0) atomicOr(p.range, p.range_bit);   // saturation is never silent
   }
   // pairs: the peer may still multicast into / arrive on this CTA's shared memory until it has consumed its last stage
   if (PAIR) cluster_sync_all();
@@ -729,7 +760,7 @@ template <bool SPLIT>
 __global__ void __launch_bounds__(128, 4)
 conv1_1_umma_kernel(const uint8_t* __restrict__ pack, const float* __restrict__ L, const float* __restrict__ ab,
                     const float* __restrict__ mask, float maskcent, int N, int H, int Wd, __half* __restrict__ ohi,
-                    __half* __restrict__ olo) {
+                    __half* __restrict__ olo, unsigned* range, unsigned out_bit) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* s_ahi = smem;                       // [128 px][64 k] FP16, K-major SW128 (16 KB); reused as the store staging
@@ -781,6 +812,9 @@ conv1_1_umma_kernel(const uint8_t* __restrict__ pack, const float* __restrict__ 
       }
 #pragma unroll
     for (int k = 36; k < kC11K; ++k) in[k] = 0.f;
+    // an input (|ab| > 110 * 1023, say) saturates the packed operand; every input pixel is the centre tap (k = 16..19)
+    // of exactly one output pixel, its own, so checking the centre taps checks every input once
+    uint32_t hin = 0u;
 #pragma unroll
     for (int j = 0; j < kC11K / 8; ++j) {
       uint32_t hw[4], lw[4];
@@ -788,6 +822,7 @@ conv1_1_umma_kernel(const uint8_t* __restrict__ pack, const float* __restrict__ 
       for (int q = 0; q < 4; ++q) {
         const float v0 = in[8 * j + 2 * q] * kInScale, v1 = in[8 * j + 2 * q + 1] * kInScale;
         hw[q] = pack_f16x2_sat(v0, v1);
+        if (8 * j + 2 * q >= 16 && 8 * j + 2 * q < 20) hin = habs_max2(hin, hw[q]);
         lw[q] = lo_f16x2(v0, v1, hw[q]);
       }
       const uint32_t o = sw128_off(threadIdx.x, j);
@@ -841,6 +876,7 @@ conv1_1_umma_kernel(const uint8_t* __restrict__ pack, const float* __restrict__ 
       }
     __syncthreads();        // every warpgroup MMA has read the operand tiles: reuse them as per-warp staging
     const uint32_t wbuf = smem_u32(s_ahi) + warp * (2 * 16 * kRow);   // rows 16*warp (+64 for m = 1) of the tile
+    uint32_t hmax[2][2] = {};                         // [m][row half]: max |hi| of the stored values
 #pragma unroll
     for (int plane = 0; plane < (SPLIT ? 2 : 1); ++plane) {
 #pragma unroll
@@ -848,6 +884,7 @@ conv1_1_umma_kernel(const uint8_t* __restrict__ pack, const float* __restrict__ 
 #pragma unroll
         for (int i = 0; i < 32; i += 2) {
           const uint32_t hw = pack_f16x2_sat(acc[m][i], acc[m][i + 1]);
+          if (plane == 0) hmax[m][(i >> 1) & 1] = habs_max2(hmax[m][(i >> 1) & 1], hw);
           const uint32_t v = plane == 0 ? hw : lo_f16x2(acc[m][i], acc[m][i + 1], hw);
           const int rl = m * 16 + (lane >> 2) + 8 * ((i >> 1) & 1);
           st_shared_u32(wbuf + rl * kRow + frag_col(i, lane) * 2, v);
@@ -862,6 +899,18 @@ conv1_1_umma_kernel(const uint8_t* __restrict__ pack, const float* __restrict__ 
         if (px < total) *reinterpret_cast<uint4*>(gbase + px * 64 + c * 8) = v;
       }
       __syncwarp();
+    }
+    {                                                 // saturation is never silent
+      // rows of the tile that hold pixels, relative to this thread's first fragment row
+      const int rows_left = (int)min(total - (size_t)tile * 128, (size_t)128) - (warp * 16 + (lane >> 2));
+      uint32_t top = 0u;
+#pragma unroll
+      for (int m = 0; m < 2; ++m)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) top = habs_max2(top, m * 64 + 8 * h < rows_left ? hmax[m][h] : 0u);
+      const unsigned bits = (__any_sync(0xffffffffu, live & f16_top(hin)) ? 1u << kRangeInputBit : 0u) |
+                            (__any_sync(0xffffffffu, f16_top(top)) ? out_bit : 0u);
+      if (bits && lane == 0) atomicOr(range, bits);
     }
     __syncthreads();        // staging read by every warp before the next tile's operand rows overwrite it
   }
@@ -893,10 +942,11 @@ cudaError_t launch_conv1_1_umma(Ctx* c, int n, const float* L, const float* ab, 
   }
   __half* hi = static_cast<__half*>(o.p0.get()) + ooff;
   __half* lo = o.p1.get() ? static_cast<__half*>(o.p1.get()) + ooff : nullptr;
+  const unsigned out_bit = 1u << c->buf_index.at("a1_1");
   cudaError_t e = lo ? launch_k(c, conv1_1_umma_kernel<true>, dim3(grid), dim3(128), (size_t)kC11Smem, st, c->w11_umma.get(), L, ab, mask,
-                                maskcent, n, o.H, o.W, hi, lo)
+                                maskcent, n, o.H, o.W, hi, lo, c->d_range, out_bit)
                      : launch_k(c, conv1_1_umma_kernel<false>, dim3(grid), dim3(128), (size_t)kC11Smem, st, c->w11_umma.get(), L, ab, mask,
-                                maskcent, n, o.H, o.W, hi, lo);
+                                maskcent, n, o.H, o.W, hi, lo, c->d_range, out_bit);
   c->launch_count++;
   return e;
 }
@@ -1177,6 +1227,7 @@ int umma_plan_op(Ctx* c, ConvOp& op) {
   }
   if (op.fuse_out_head) { q.wout = c->wout; q.bout = c->bout; }
   q.err = c->d_err;
+  q.range = c->d_range; q.range_bit = op.out_buf >= 0 ? 1u << op.out_buf : 0u;
   q.img0 = 0;
   op.umma_plan = std::move(pl);
   return IDC_OK;

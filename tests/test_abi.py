@@ -28,6 +28,14 @@ def test_library_exports_every_declared_symbol():
     assert b"sm_90a" in lib.idc_version()
 
 
+def test_error_codes_match_header():
+    """Every IDC_ERR_* of the header, IDC_ERR_RANGE included, has the same value in _lib."""
+    src = open(os.path.join(ROOT, "include", "idc_b200.h")).read()
+    codes = {m.group(1): int(m.group(2)) for m in re.finditer(r"\bIDC_ERR_([A-Z]+)\s*=\s*(-?\d+)", src)}
+    assert codes["RANGE"] == -7
+    assert codes == {k[4:]: v for k, v in vars(_lib).items() if k.startswith("ERR_")}
+
+
 def test_argument_validation_without_gpu():
     lib = _lib.load()
     h = ctypes.c_void_p()

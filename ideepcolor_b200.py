@@ -8,6 +8,7 @@ result folder, plus the K colour suggestions per hint that the GUI shows in its 
 
     python ideepcolor_b200.py --image_file test_imgs/mortar_pestle.jpg --color_model caffemodel.pth \\
         --hints hints.json --out result_dir [--suggest 9] [--pytorch_maskcent] [--gpu 0] [--load_size 256]
+        [--calibrate photos/ | ranges.json] [--save_act_ranges ranges.json]
 
 Automatic colorization of a folder of photos, in batches on the device (photos.PhotoColorizer):
 
@@ -42,7 +43,27 @@ def parse_args(argv=None):
     ap.add_argument("--image_dir", default="", help="colorize every photo of this folder automatically (needs --out)")
     ap.add_argument("--batch", type=int, default=32, help="photos per device pass (--image_dir)")
     ap.add_argument("--psnr", action="store_true", help="also write psnr.csv (--image_dir)")
-    return ap.parse_args(argv)
+    ap.add_argument("--calibrate", default="", metavar="DIR_OR_JSON",
+                    help="set the activation storage exponents from measured ranges instead of the weights: a folder of "
+                         "colour photos to measure on (a seeded sample of at most 16), or a JSON file saved earlier")
+    ap.add_argument("--save_act_ranges", default="", metavar="FILE", help="write the ranges --calibrate used as JSON")
+    args = ap.parse_args(argv)
+    args.calibrate_source = None
+    if args.calibrate:
+        from interactive_deep_colorization_b200 import engine
+        try:
+            args.calibrate_source = engine.calibration_source(args.calibrate)
+        except ValueError as e:
+            ap.error(str(e))
+    elif args.save_act_ranges:
+        ap.error("--save_act_ranges needs --calibrate")
+    return args
+
+
+def save_ranges(args, ranges):
+    if args.save_act_ranges:
+        from interactive_deep_colorization_b200 import engine
+        engine.save_act_ranges(args.save_act_ranges, ranges)
 
 
 def hint_ab(h):
@@ -79,7 +100,9 @@ def colorize_dir(args):
     if not os.path.isdir(args.out):
         os.makedirs(args.out)
     sd = torch.load(args.color_model, map_location="cpu")
-    pc = PhotoColorizer(sd, Xd=args.load_size, batch=args.batch, device=args.gpu, maskcent=args.pytorch_maskcent)
+    pc = PhotoColorizer(sd, Xd=args.load_size, batch=args.batch, device=args.gpu, maskcent=args.pytorch_maskcent,
+                        calibrate=args.calibrate_source)
+    save_ranges(args, pc.act_ranges)
     rows = []
     for name, r in zip(names, pc.colorize(paths, psnr=args.psnr)):
         stem = os.path.splitext(name)[0]
@@ -107,7 +130,8 @@ def main(argv=None):
     color_model = CI.ColorizeImageB200(Xd=X, maskcent=args.pytorch_maskcent)
     # one checkpoint, one trunk (ideepcolor.py:34-38 "same model used for both"): with suggestions on, the colour model
     # carries the distribution head and the distribution model below shares its context -> ONE forward for both
-    color_model.prep_net(gpu_id=args.gpu, state_dict=sd, dist=args.suggest > 0)
+    color_model.prep_net(gpu_id=args.gpu, state_dict=sd, dist=args.suggest > 0, calibrate=args.calibrate_source)
+    save_ranges(args, color_model.act_ranges)
     color_model.load_image(args.image_file)
     dist_model = None
     if args.suggest > 0:

@@ -338,6 +338,32 @@ int idc_rgb_sse(int device, int n, int h, int w, const uint8_t* a, const uint8_t
  * buffer from the weights by idc_finalize_weights (DESIGN.md §3); 0 on the SIMT engine.  IDC_ERR_KEY for an unknown
  * name, IDC_ERR_STATE before the weights are packed. */
 int idc_act_exponent(idc_ctx* ctx, const char* name, int* exp_out);
+/* The activation buffers this context stores, in plan order (like idc_num_ops / idc_op_name): "a1_1", "conv1_2", ...;
+ * "conv10_2" only on the SIMT engine or with IDC_FLAG_KEEP_CONV10, "hyper" only with IDC_FLAG_CAFFE313.  NULL outside
+ * [0, idc_num_acts). */
+int idc_num_acts(idc_ctx* ctx);
+const char* idc_act_name(idc_ctx* ctx, int i);
+/* *out_host = the largest |a| over images [0, n) of activation `name` as the last forward / idc_run_op /
+ * idc_set_activation left it, i.e. the maximum of what idc_get_activation returns, bit for bit, on both engines (wgmma:
+ * |hi + lo| * 2^-S).  A NaN anywhere in the buffer comes back as NaN, an infinity as infinity.  One bandwidth-bound
+ * pass over the buffer; synchronises the device.  On the wgmma engine this says how close a checkpoint comes to FP16's
+ * limit on an image (stored value = result * 2^S against 65504); on the SIMT engine, whose FP32 planes cannot
+ * saturate, it is the measurement idc_set_act_range wants.  IDC_ERR_KEY unknown buffer, IDC_ERR_ARG for n outside
+ * [1, max_n] or a NULL argument, IDC_ERR_STATE before the weights are packed. */
+int idc_act_absmax(idc_ctx* ctx, const char* name, int n, float* out_host);
+/* Calibration: "the largest |a| activation `name` takes on representative inputs is max_abs".  The wgmma engine then
+ * stores that buffer with S = 10 - ceil(log2 max_abs), which puts the measured maximum in (512, 1024] and leaves 64x
+ * of headroom below 65504 for inputs outside the sample, in place of the exponent estimated from the weights
+ * (DESIGN.md §3).  "act_exp.<buffer>" still wins over a range; a buffer without a range keeps the weight-derived
+ * exponent, so a partial set of ranges is well defined.  An exponent outside [-24, 24] fails idc_finalize_weights,
+ * naming the buffer, as for the estimate.  Same life cycle as "act_exp.<buffer>": only before idc_finalize_weights
+ * (IDC_ERR_STATE once the weights are packed); IDC_ERR_KEY unknown buffer; IDC_ERR_ARG unless max_abs is finite and
+ * > 0.  No effect on the SIMT engine.  A range stays with the context, like an "act_exp.<buffer>" override: weights
+ * loaded and packed again later are packed with it, so a context that moves to another checkpoint needs that
+ * checkpoint's ranges set again (or a new context).  The resulting exponents live in the weight arena like any others, so a context
+ * that receives the arena (idc_reserve_weights + copy + idc_adopt_weights, ranks != 0) stores its activations exactly
+ * as the context that packed it, with no call of its own. */
+int idc_set_act_range(idc_ctx* ctx, const char* name, double max_abs);
 /* Copy a named activation ("conv1_2", "a8_1", ... see DESIGN.md) of the LAST forward to
  * out [n,C,H,W] FP32 device memory; *c,*h,*w receive its shape. */
 int idc_get_activation(idc_ctx* ctx, const char* name, float* out_nchw, size_t out_floats,

@@ -84,6 +84,10 @@ SYMBOLS = [
                                       _c.POINTER(_c.c_int), _c.POINTER(_c.c_int)]),
     ("idc_set_activation", _c.c_int, [_P, _c.c_char_p, _c.c_int, _P]),
     ("idc_act_exponent", _c.c_int, [_P, _c.c_char_p, _c.POINTER(_c.c_int)]),
+    ("idc_num_acts", _c.c_int, [_P]),
+    ("idc_act_name", _c.c_char_p, [_P, _c.c_int]),
+    ("idc_act_absmax", _c.c_int, [_P, _c.c_char_p, _c.c_int, _c.POINTER(_c.c_float)]),
+    ("idc_set_act_range", _c.c_int, [_P, _c.c_char_p, _c.c_double]),
     ("idc_run_op", _c.c_int, [_P, _c.c_char_p, _c.c_int, _P]),
     ("idc_num_ops", _c.c_int, [_P]),
     ("idc_op_name", _c.c_char_p, [_P, _c.c_int]),

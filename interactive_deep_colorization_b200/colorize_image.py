@@ -265,7 +265,19 @@ class ColorizeImageB200(ColorizeImageBase):
         # torch-path bin grid (reference :213; (b,a)-ordered meshgrid, SURVEY q3)
         self.pts_in_hull = np.array(np.meshgrid(np.arange(-110, 120, 10), np.arange(-110, 120, 10))).reshape((2, 529)).T
 
-    def prep_net(self, gpu_id=None, path='', dist=False, state_dict=None):
+    def _calibrate(self, calibrate, sd, device, **flags):
+        """prep_net's calibrate= argument -> self.act_ranges, {buffer: max_abs} or None.  calibrate: None (exponents
+        from the weights); a list of colour photos (paths or uint8 RGB arrays) to measure the activation ranges of
+        this checkpoint on now (engine.calibration_batch + engine.measure_act_ranges); or such a measurement, as a dict
+        or the path of a JSON file written by engine.save_act_ranges."""
+        from . import engine
+        X = self.Xd
+        self.act_ranges = engine.resolve_calibration(calibrate, lambda photos: engine.measure_act_ranges(
+            sd, engine.calibration_batch(photos, X, device=device, global_hints=flags.get("global_hints", False)),
+            X, X, device=device, maskcent=float(self.mask_cent), **flags))
+        return self.act_ranges
+
+    def prep_net(self, gpu_id=None, path='', dist=False, state_dict=None, calibrate=None):
         import torch
         from .model import SIGGRAPHGeneratorB200
         print('path = %s' % path)
@@ -279,6 +291,7 @@ class ColorizeImageB200(ColorizeImageBase):
         self.net.load_state_dict(state_dict)
         self.net.cuda()
         self.net.eval()
+        self.net.set_act_ranges(self._calibrate(calibrate, self.net.state_dict(), self.net.b200_device))
         self.net_set = True
 
     def net_forward(self, input_ab, input_mask):
@@ -589,8 +602,8 @@ class ColorizeImageB200Dist(_DistPlots, ColorizeImageB200):
         self.dist_entropy = np.zeros((self.Xd, self.Xd))
         self.mask_cent = .5 if maskcent else 0
 
-    def prep_net(self, gpu_id=None, path='', dist=True, S=.2, state_dict=None):
-        ColorizeImageB200.prep_net(self, gpu_id=gpu_id, path=path, dist=dist, state_dict=state_dict)
+    def prep_net(self, gpu_id=None, path='', dist=True, S=.2, state_dict=None, calibrate=None):
+        ColorizeImageB200.prep_net(self, gpu_id=gpu_id, path=path, dist=dist, state_dict=state_dict, calibrate=calibrate)
 
     def share_trunk(self, color_model):
         """ONE forward per click instead of two.  The PyTorch backend loads the same checkpoint into both models
@@ -711,14 +724,15 @@ class ColorizeImageB200GlobDist(ColorizeImageB200):
         ColorizeImageB200.__init__(self, Xd, maskcent=maskcent, engine=engine)
         self.glob_mask_mult = 1.
 
-    def prep_net(self, gpu_id=None, path='', state_dict=None):
+    def prep_net(self, gpu_id=None, path='', state_dict=None, calibrate=None):
         import torch
         from .engine import LhnContext
         if state_dict is None:
             state_dict = torch.load(path, map_location='cpu')
-        self._ctx = LhnContext(device=0 if gpu_id is None else int(gpu_id), max_n=1, H=self.Xd, W=self.Xd,
-                               engine=self.engine, global_hints=True)
-        self._ctx.load_state_dict(state_dict)
+        device = 0 if gpu_id is None else int(gpu_id)
+        ranges = self._calibrate(calibrate, state_dict, device, global_hints=True)
+        self._ctx = LhnContext(device=device, max_n=1, H=self.Xd, W=self.Xd, engine=self.engine, global_hints=True)
+        self._ctx.load_state_dict(state_dict, act_ranges=ranges)
         self.net_set = True
 
     def get_global_histogram(self, ref_rgb_u8):
@@ -780,7 +794,7 @@ class ColorizeImageB200Caffe(ColorizeImageB200):
         from . import prepost
         self.pts_in_hull = prepost.pts_in_hull().astype(np.float64)       # 313 x 2, in-gamut (reference :388-389)
 
-    def prep_net(self, gpu_id=0, prototxt_path='', caffemodel_path='', state_dict=None):
+    def prep_net(self, gpu_id=0, prototxt_path='', caffemodel_path='', state_dict=None, calibrate=None):
         import torch
         from .engine import LhnContext
         print('gpu_id = %d, net_path = %s, model_path = %s' % (-1 if gpu_id is None else gpu_id, prototxt_path, caffemodel_path))
@@ -790,10 +804,11 @@ class ColorizeImageB200Caffe(ColorizeImageB200):
         sd = caffe_scaled_state_dict(state_dict)
         if self._caffe313:
             sd["caffe.pts_in_hull"] = torch.from_numpy(self.pts_in_hull.astype(np.float32))   # reference :405-407
-        self._ctx = LhnContext(device=0 if gpu_id in (None, -1) else int(gpu_id), max_n=1, H=self.Xd, W=self.Xd,
-                               engine=self.engine, global_hints=self._global_hints, caffe313=self._caffe313,
-                               options={"tanh_scale": 100})
-        self._ctx.load_state_dict(sd)
+        device = 0 if gpu_id in (None, -1) else int(gpu_id)
+        flags = dict(global_hints=self._global_hints, caffe313=self._caffe313, options={"tanh_scale": 100})
+        ranges = self._calibrate(calibrate, sd, device, **flags)
+        self._ctx = LhnContext(device=device, max_n=1, H=self.Xd, W=self.Xd, engine=self.engine, **flags)
+        self._ctx.load_state_dict(sd, act_ranges=ranges)
         self.net_set = True
 
     def _engine_inputs(self):
@@ -893,9 +908,9 @@ class ColorizeImageB200CaffeDist(_DistPlots, ColorizeImageB200Caffe):
         self.A = self.B = int(np.sqrt(self.AB))
         self.dist_entropy = np.zeros((self.Xd, self.Xd))
 
-    def prep_net(self, gpu_id=0, prototxt_path='', caffemodel_path='', S=.2, state_dict=None):
+    def prep_net(self, gpu_id=0, prototxt_path='', caffemodel_path='', S=.2, state_dict=None, calibrate=None):
         ColorizeImageB200Caffe.prep_net(self, gpu_id, prototxt_path=prototxt_path, caffemodel_path=caffemodel_path,
-                                        state_dict=state_dict)
+                                        state_dict=state_dict, calibrate=calibrate)
         self.S = S
 
     def net_forward(self, input_ab, input_mask):

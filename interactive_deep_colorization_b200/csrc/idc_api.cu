@@ -314,18 +314,25 @@ int exp_below(int ref, double est) {
 }
 
 // Storage exponent of buffer b from its magnitude estimate est and, for the outputs of convs without a BatchNorm, its
-// bound (DESIGN §3): S_b = min(kActExpRef - ceil(log2 est_b), kActExpBound - ceil(log2 bound_b)), or the act_exp.<name>
-// override.  bound < 0: none.  Writes it to the arena table and the buffer; fails, naming the buffer, outside the range.
+// bound (DESIGN §3): the act_exp.<name> override, else kActExpCal - ceil(log2 max_abs) where a range was measured
+// (idc_set_act_range), else S_b = min(kActExpRef - ceil(log2 est_b), kActExpBound - ceil(log2 bound_b)).
+// bound < 0: none.  Writes it to the arena table and the buffer; fails, naming the buffer, outside the range.
 int set_act_exp(Ctx* c, int* table, int b, double est, double bound) {
   ActBuf& buf = c->bufs[b];
   int s = 0;
   if (!c->simt) {
-    if (!std::isfinite(est) || !std::isfinite(bound))
-      return fail(c, IDC_ERR_ARG, "activation %s: magnitude estimate %g / bound %g is not finite", buf.name.c_str(), est, bound);
-    s = exp_below(kActExpRef, est);
-    if (bound >= 0.0) s = std::min(s, exp_below(kActExpBound, bound));
     auto ov = c->act_exp_override.find(buf.name);
-    if (ov != c->act_exp_override.end()) s = ov->second;
+    auto rg = c->act_range.find(buf.name);
+    if (ov != c->act_exp_override.end()) {
+      s = ov->second;
+    } else if (rg != c->act_range.end()) {
+      s = exp_below(kActExpCal, rg->second);
+    } else {     // only this branch needs the estimate: a checkpoint whose estimate overflows can still be calibrated
+      if (!std::isfinite(est) || !std::isfinite(bound))
+        return fail(c, IDC_ERR_ARG, "activation %s: magnitude estimate %g / bound %g is not finite", buf.name.c_str(), est, bound);
+      s = exp_below(kActExpRef, est);
+      if (bound >= 0.0) s = std::min(s, exp_below(kActExpBound, bound));
+    }
     if (s < kActExpMin || s > kActExpMax)
       return fail(c, IDC_ERR_UNSUPPORTED,
                   "activation %s: storage exponent %d (magnitude estimate %g, bound %g) is outside the supported range [%d, %d]",
@@ -1589,6 +1596,49 @@ int idc_act_exponent(idc_ctx* c, const char* name, int* exp_out) {
   if (it == c->buf_index.end() || c->bufs[it->second].H == 0) return fail(c, IDC_ERR_KEY, "no activation '%s'", name);
   if (!c->weights_ready) return fail(c, IDC_ERR_STATE, "idc_act_exponent before idc_finalize_weights");
   *exp_out = c->bufs[it->second].exp;
+  return IDC_OK;
+}
+
+int idc_num_acts(idc_ctx* c) {
+  int k = 0;
+  if (c) for (auto& b : c->bufs) k += b.H > 0;
+  return k;
+}
+const char* idc_act_name(idc_ctx* c, int i) {
+  if (c && i >= 0)
+    for (auto& b : c->bufs)
+      if (b.H > 0 && i-- == 0) return b.name.c_str();
+  return nullptr;
+}
+
+int idc_act_absmax(idc_ctx* c, const char* name, int n, float* out_host) {
+  if (!c || !name || !out_host || n < 1 || n > c->max_n) return fail(c, IDC_ERR_ARG, "bad idc_act_absmax args");
+  auto it = c->buf_index.find(name);
+  if (it == c->buf_index.end() || c->bufs[it->second].H == 0) return fail(c, IDC_ERR_KEY, "no activation '%s'", name);
+  if (!c->weights_ready) return fail(c, IDC_ERR_STATE, "idc_act_absmax before idc_finalize_weights");
+  const ActBuf& b = c->bufs[it->second];
+  if (b.C % 8) return fail(c, IDC_ERR_UNSUPPORTED, "activation %s: %d channels, idc_act_absmax reads 8 at a time", name, b.C);
+  CUDA_TRY(c, cudaSetDevice(c->dev));
+  if (!c->d_absmax.get()) CUDA_TRY(c, cudaMalloc(c->d_absmax.put(), sizeof(unsigned)));
+  CUDA_TRY(c, cudaDeviceSynchronize());   // the forward that wrote the buffer may be running on any stream
+  CUDA_TRY(c, launch_act_absmax(c, b, n, c->d_absmax.get(), 0));
+  unsigned bits = 0;
+  CUDA_TRY(c, cudaMemcpy(&bits, c->d_absmax.get(), sizeof(bits), cudaMemcpyDeviceToHost));
+  float v;
+  memcpy(&v, &bits, sizeof(v));
+  *out_host = v * ldexpf(1.f, -b.exp);    // stored units -> value, the multiply idc_get_activation applies per element
+  return IDC_OK;
+}
+
+int idc_set_act_range(idc_ctx* c, const char* name, double max_abs) {
+  if (!c || !name) return IDC_ERR_ARG;
+  auto it = c->buf_index.find(name);
+  if (it == c->buf_index.end() || c->bufs[it->second].H == 0) return fail(c, IDC_ERR_KEY, "no activation '%s'", name);
+  if (!std::isfinite(max_abs) || !(max_abs > 0.0))
+    return fail(c, IDC_ERR_ARG, "range of activation %s = %g: must be finite and > 0", name, max_abs);
+  if (c->weights_adopted)
+    return fail(c, IDC_ERR_STATE, "the range of %s must be set before the weights are packed (idc_finalize_weights)", name);
+  c->act_range[name] = max_abs;
   return IDC_OK;
 }
 

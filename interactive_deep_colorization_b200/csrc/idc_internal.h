@@ -52,10 +52,13 @@ enum Act { ACT_NONE = 0, ACT_RELU = 1, ACT_LEAKY02 = 2 };
 // (2^(kActExpRef-1), 2^kActExpRef], far below FP16's 65504 and far above the range where the lo plane goes subnormal.
 // The output of a conv without a BatchNorm also has a bound (1-norms instead of 2-norms); S_b is lowered where needed
 // to keep the bound at or below 2^kActExpBound.
+// A buffer whose largest |a| on sample inputs was measured (idc_set_act_range) takes S_b = kActExpCal - ceil(log2 max_abs)
+// instead: a measured maximum needs less headroom than an estimate that BatchNorm outputs exceed by orders of magnitude.
 // A network whose exponents fall outside [kActExpMin, kActExpMax] is refused (the per-channel weight exponent, clamped
 // to +-24, could not absorb the shift exactly any more).
 constexpr int kActExpRef = 7;
 constexpr int kActExpBound = 11;
+constexpr int kActExpCal = 10;
 constexpr int kActExpMin = -24, kActExpMax = 24;
 // Every FP16 activation store whose hi part reaches 65504, FP16's largest value (|v| >= 65488; above 65504 the value
 // saturates there), sets bit `buffer index` of the context's range word; the packed conv1_1 input uses bit
@@ -205,6 +208,8 @@ struct Ctx {
   size_t arena_bytes = 0;
   int* act_exp = nullptr;         // [bufs.size()] storage exponents, in the arena so that adopting ranks read them too
   std::map<std::string, int> act_exp_override;   // idc_set_option("act_exp.<buffer>"): applied at the next pack
+  std::map<std::string, double> act_range;       // idc_set_act_range: measured largest |a| per buffer, applied at the next pack
+  DevMem<unsigned> d_absmax;                     // idc_act_absmax result word (bit pattern of the maximum), made at first use
   bool weights_ready = false;     // adopted and planned: forwards may run
   bool weights_adopted = false;   // idc_adopt_weights succeeded and no tensor was loaded since: option changes re-plan
   // conv1_1 (4->64) + regression head + misc small weights (device fp32)
@@ -315,6 +320,8 @@ cudaError_t launch_rgb_sse(int n, size_t hw3, const uint8_t* a, const uint8_t* b
 cudaError_t launch_global_mlp(Ctx* c, int n, const float* glob, cudaStream_t st);
 cudaError_t launch_act_to_nchw(Ctx* c, const ActBuf& b, int n, float* out, cudaStream_t st);
 cudaError_t launch_nchw_to_act(Ctx* c, const ActBuf& b, int n, const float* in, cudaStream_t st);
+// *out_bits (device) = the bit pattern of max |a| over the first n images of b, in stored units (value * 2^b.exp)
+cudaError_t launch_act_absmax(Ctx* c, const ActBuf& b, int n, unsigned* out_bits, cudaStream_t st);
 
 inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 

@@ -4,6 +4,9 @@ Host-side plumbing only: pointer marshalling, torch tensors as device memory, st
 All arithmetic of the forward happens in libidc_b200.so.
 """
 import ctypes
+import json
+import math
+import os
 
 import numpy as np
 
@@ -23,6 +26,169 @@ def as_hints(rects):
             out[f] = rects[f]
         return out
     return np.array([tuple(r) for r in rects], dtype=_lib.HINT_DTYPE).reshape(-1)
+
+
+# every activation buffer a context can store, in plan order (idc_act_name lists the ones a given context has:
+# conv10_2 on the SIMT engine or with keep_conv10, hyper with caffe313)
+ACT_BUFFERS = ("a1_1", "conv1_2", "a2_1", "conv2_2", "a3_1", "a3_2", "conv3_3", "a4_1", "a4_2", "conv4_3",
+               "a5_1", "a5_2", "conv5_3", "a6_1", "a6_2", "conv6_3", "a7_1", "a7_2", "conv7_3",
+               "a8_1", "a8_2", "conv8_3", "hyper", "a9_1", "conv9_3", "a10_1", "conv10_2")
+CALIBRATION_MAX_N = 4        # images per forward of the temporary measuring context
+
+
+def check_act_ranges(ranges):
+    """-> {buffer: float} or ValueError naming the first entry that is not a known buffer with a finite range > 0."""
+    if not isinstance(ranges, dict):
+        raise ValueError("activation ranges: need a {buffer: max_abs} object, got %s" % type(ranges).__name__)
+    out = {}
+    for k, v in ranges.items():
+        if k not in ACT_BUFFERS:
+            raise ValueError("activation ranges: %r is not an activation buffer" % (k,))
+        if isinstance(v, bool) or not isinstance(v, (int, float, np.floating, np.integer)) \
+                or not math.isfinite(v) or not v > 0:
+            raise ValueError("activation ranges: %s = %r must be a finite number > 0" % (k, v))
+        out[k] = float(v)
+    return out
+
+
+def save_act_ranges(path, ranges):
+    """Write measured ranges as a flat JSON object {buffer: max_abs}.  Ranges belong to a checkpoint (and its input
+    scaling), not to a network size: a file measured at one Xd serves every Xd."""
+    with open(path, "w") as f:
+        json.dump(check_act_ranges(ranges), f, indent=1, sort_keys=True)
+        f.write("\n")
+
+
+def load_act_ranges(path):
+    with open(path) as f:
+        try:
+            return check_act_ranges(json.load(f))
+        except ValueError as e:
+            raise ValueError("%s: %s" % (path, e))
+
+
+def calibration_batch(images, X, hints=8, seed=0, device=0, global_hints=False):
+    """Colour photos (paths or HxWx3 uint8 RGB arrays, at most 128) -> the network's own inputs (L_mc [n,1,X,X], ab
+    [n,2,X,X], mask [n,1,X,X][, glob [n,316]]), device float32 tensors, through the same device steps as a photo batch
+    (idc_photo_prep: cv2-exact resize, rgb2lab, L - 50).  A click session is what the network will see, so every
+    second photo also carries `hints` hint rectangles, 1-9 pixels wide like the GUI's, at seeded places, painted with
+    the photo's own ab at their centres; with global_hints every second photo carries its own global-statistics vector.
+    More, and more varied, photos give safer ranges; the headroom of the exponent rule covers what they miss."""
+    import torch
+    from . import photos as P
+    lib = _lib.load()
+    imgs = [P.check_photo(P.read_photo(p) if not isinstance(p, np.ndarray) else np.ascontiguousarray(p), "photo %d" % i)
+            for i, p in enumerate(images)]
+    n = len(imgs)
+    if not 1 <= n <= _lib.MAX_PHOTOS:
+        raise ValueError("calibration needs 1 to %d photos, got %d" % (_lib.MAX_PHOTOS, n))
+    dev = torch.device("cuda:%d" % device)
+    st = torch.cuda.current_stream(dev).cuda_stream
+    table = np.zeros(n, _lib.PHOTO_DTYPE)
+    off = 0
+    for i, a in enumerate(imgs):
+        table[i] = (off, a.shape[0], a.shape[1])
+        off += a.shape[0] * a.shape[1]
+    src = torch.from_numpy(np.concatenate([a.reshape(-1) for a in imgs])).to(dev)
+    L_mc = torch.empty((n, 1, X, X), dtype=torch.float32, device=dev)
+    rgb = torch.empty((n, X, X, 3), dtype=torch.uint8, device=dev)
+    lab = torch.empty((n, 3, X, X), dtype=torch.float64, device=dev)
+    _lib.check(None, lib.idc_photo_prep(device, n, table.ctypes.data, src.data_ptr(), X, L_mc.data_ptr(), rgb.data_ptr(), st))
+    _lib.check(None, lib.idc_rgb2lab_f64(device, n, X, X, rgb.data_ptr(), lab.data_ptr(), st))
+    own_ab = lab[:, 1:].cpu().numpy()
+    rng = np.random.RandomState(seed)
+    rects = []
+    for i in range(1, n, 2):
+        for _ in range(hints):
+            y, x, p = int(rng.randint(X)), int(rng.randint(X)), int(rng.randint(5))     # (2p+1)-pixel square, p = 0..4
+            rects.append((i, max(y - p, 0), max(x - p, 0), min(y + p, X - 1), min(x + p, X - 1),
+                          own_ab[i, 0, y, x], own_ab[i, 1, y, x]))
+    if len(rects) > _lib.MAX_HINTS:
+        raise ValueError("%d calibration hints, at most %d" % (len(rects), _lib.MAX_HINTS))
+    block = np.zeros(_lib.HINT_HDR_BYTES + len(rects) * _lib.HINT_DTYPE.itemsize, np.uint8)
+    block[:4].view(np.int32)[0] = len(rects)
+    if rects:
+        block[_lib.HINT_HDR_BYTES:] = as_hints(rects).view(np.uint8)
+    d_block = torch.from_numpy(block).to(dev)
+    ab = torch.empty((n, 2, X, X), dtype=torch.float32, device=dev)
+    mask = torch.empty((n, 1, X, X), dtype=torch.float32, device=dev)
+    _lib.check(None, lib.idc_hint_raster(device, n, X, X, len(rects), d_block.data_ptr(), ab.data_ptr(), mask.data_ptr(), st))
+    if not global_hints:
+        return L_mc, ab, mask
+    from . import prepost
+    glob = torch.zeros((n, 316), dtype=torch.float32, device=dev)
+    pts = torch.from_numpy(prepost.pts_in_hull()).to(dev)
+    for i in range(1, n, 2):
+        _lib.check(None, lib.idc_global_stats(device, X, X, rgb[i].data_ptr(), pts.data_ptr(), glob[i].data_ptr(), st))
+    return L_mc, ab, mask, glob
+
+
+def measure_act_ranges(sd, batches, H, W, device=0, maskcent=0., dist=False, global_hints=False, caffe313=False,
+                       keep_conv10=False, options=None):
+    """The largest |a| of every activation buffer of checkpoint `sd` over `batches` -> {buffer: max_abs}, for
+    LhnContext.load_state_dict(sd, act_ranges=...).  batches: one (L_mc, ab, mask[, glob]) tuple or a list of them,
+    float32 device tensors or host arrays ([n,1,H,W], [n,2,H,W], [n,1,H,W], [n,316]).
+    The measurement runs on a temporary exact-FP32 context (engine="simt") of the same geometry and flags, not on the
+    wgmma engine being calibrated: FP32 planes cannot saturate, so one pass gives every buffer's true range even where
+    several buffers in a chain would saturate.  The context is closed before this returns, so its buffers are free
+    again before the caller builds its own.  A buffer that stayed 0 is left out (it keeps the weight-derived
+    exponent); a NaN or infinite range raises, naming the buffer."""
+    import torch
+    if isinstance(batches, tuple):
+        batches = [batches]
+    dev = torch.device("cuda:%d" % device)
+    ctx = LhnContext(device=device, max_n=CALIBRATION_MAX_N, H=H, W=W, dist=dist, engine="simt", global_hints=global_hints,
+                     caffe313=caffe313, keep_conv10=keep_conv10, options=options)
+    try:
+        ctx.load_state_dict(sd)
+        names = ctx.act_names()
+        top = dict.fromkeys(names, 0.0)
+        for batch in batches:
+            t = [torch.as_tensor(a, dtype=torch.float32).to(dev).contiguous() for a in batch]
+            for i in range(0, t[0].shape[0], CALIBRATION_MAX_N):
+                c = [a[i:i + CALIBRATION_MAX_N] for a in t]
+                ctx.forward_device(c[0], c[1], c[2], maskcent, glob=c[3] if len(c) > 3 else None)
+                for b in names:
+                    v = ctx.act_absmax(b, c[0].shape[0])
+                    top[b] = v if math.isnan(v) else max(top[b], v)
+    finally:
+        ctx.close()
+    for b, v in top.items():
+        if not math.isfinite(v):
+            raise ValueError("activation %s reaches %r on the calibration images: the checkpoint does not compute "
+                             "finite values" % (b, v))
+    return {b: v for b, v in top.items() if v > 0}
+
+
+def resolve_calibration(calibrate, measure):
+    """The `calibrate=` argument of the wrappers -> {buffer: max_abs} or None: None; a dict; the path of a JSON file
+    written by save_act_ranges; or a list of photos (paths / uint8 RGB arrays), measured now by measure(photos)."""
+    if calibrate is None:
+        return None
+    if isinstance(calibrate, dict):
+        return check_act_ranges(calibrate)
+    if isinstance(calibrate, (str, bytes, os.PathLike)):
+        return load_act_ranges(calibrate)
+    return check_act_ranges(measure(list(calibrate)))
+
+
+PHOTO_EXTS = (".jpg", ".jpeg", ".png", ".bmp", ".tif", ".tiff", ".webp")
+
+
+def calibration_source(path, max_photos=16, seed=0):
+    """The --calibrate argument of the command-line front ends -> a `calibrate=` value: a folder becomes a seeded
+    sample of at most max_photos of its photos (sorted by name), a file is taken as a saved JSON of ranges."""
+    if os.path.isdir(path):
+        names = sorted(f for f in os.listdir(path) if os.path.splitext(f)[1].lower() in PHOTO_EXTS)
+        if not names:
+            raise ValueError("--calibrate %s: no photos in this folder" % path)
+        if len(names) > max_photos:
+            pick = np.random.RandomState(seed).choice(len(names), max_photos, replace=False)
+            names = [names[i] for i in sorted(pick)]
+        return [os.path.join(path, f) for f in names]
+    if os.path.isfile(path):
+        return path
+    raise ValueError("--calibrate %s: neither a folder of photos nor a JSON file of ranges" % path)
 
 
 class LhnContext(object):
@@ -72,8 +238,17 @@ class LhnContext(object):
         _lib.check(self.h, self.lib.idc_set_option(self.h, name.encode(), int(value)))
 
     # ---- weights ---------------------------------------------------------------------------
-    def load_state_dict(self, sd):
-        """sd: {reference state_dict key: torch.Tensor | ndarray}.  Packs + uploads."""
+    def load_state_dict(self, sd, act_ranges=None):
+        """sd: {reference state_dict key: torch.Tensor | ndarray}.  Packs + uploads.
+        act_ranges: {buffer: max_abs} from measure_act_ranges: the wgmma engine then stores those buffers by their
+        measured range instead of the estimate from the weights (idc_set_act_range); buffers this context does not
+        store (conv10_2 with the fused head) are ignored.  Ranges stay with the context: loading another checkpoint
+        into it later without act_ranges packs it with the ranges set here."""
+        if act_ranges:
+            mine = set(self.act_names())
+            for b, v in check_act_ranges(act_ranges).items():
+                if b in mine:
+                    _lib.check(self.h, self.lib.idc_set_act_range(self.h, b.encode(), v))
         for k, v in sd.items():
             a = v.detach().cpu().numpy() if hasattr(v, "detach") else np.asarray(v)
             if a.dtype == np.float32:
@@ -296,6 +471,19 @@ class LhnContext(object):
         e = ctypes.c_int()
         _lib.check(self.h, self.lib.idc_act_exponent(self.h, name.encode(), ctypes.byref(e)))
         return e.value
+
+    def act_names(self):
+        """The activation buffers this context stores, in plan order."""
+        return [self.lib.idc_act_name(self.h, i).decode() for i in range(self.lib.idc_num_acts(self.h))]
+
+    def act_exponents(self):
+        return {b: self.act_exponent(b) for b in self.act_names()}
+
+    def act_absmax(self, name, n):
+        """max |a| over the first n images of activation `name` as the last forward left it (idc_act_absmax)."""
+        v = ctypes.c_float()
+        _lib.check(self.h, self.lib.idc_act_absmax(self.h, name.encode(), int(n), ctypes.byref(v)))
+        return v.value
 
     def get_activation(self, name, n):
         import torch

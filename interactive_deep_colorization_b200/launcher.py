@@ -49,7 +49,21 @@ def parse_args(argv=None):
     p.add_argument('--host_display', action='store_true', help='keep the numpy display step of compute_result')
     p.add_argument('--separate_models', action='store_true',
                    help='b200: two contexts (two forwards per click) like the reference, instead of one shared trunk')
-    return p.parse_args(argv)
+    p.add_argument('--calibrate', type=str, default='', metavar='DIR_OR_JSON',
+                   help='set the activation storage exponents from measured ranges: a folder of colour photos to measure '
+                        'on at start-up, or a JSON file saved by ideepcolor_b200.py --save_act_ranges (no measurement)')
+    args = p.parse_args(argv)
+    args.calibrate_source = None
+    if args.calibrate:
+        from . import engine
+        try:
+            args.calibrate_source = engine.calibration_source(args.calibrate)
+        except ValueError as e:
+            p.error(str(e))
+        if args.backend == 'b200-caffe' and isinstance(args.calibrate_source, str):
+            p.error("--calibrate %s: ranges belong to one checkpoint and b200-caffe loads two (--color_caffemodel, "
+                    "--dist_caffemodel); give a folder of photos, each checkpoint is then measured on it" % args.calibrate)
+    return args
 
 
 def build_models(args):
@@ -60,17 +74,19 @@ def build_models(args):
         # model shares the colour model's context and a click is ONE forward (ColorizeImageB200Dist.share_trunk)
         share = not getattr(args, 'separate_models', False)
         colorModel = CI.ColorizeImageB200(Xd=args.load_size, maskcent=args.pytorch_maskcent)
-        colorModel.prep_net(gpu_id=args.gpu, path=args.color_model, dist=share)
+        cal = getattr(args, 'calibrate_source', None)
+        colorModel.prep_net(gpu_id=args.gpu, path=args.color_model, dist=share, calibrate=cal)
         distModel = CI.ColorizeImageB200Dist(Xd=args.load_size, maskcent=args.pytorch_maskcent)
         if share:
             distModel.share_trunk(colorModel)
         else:
-            distModel.prep_net(gpu_id=args.gpu, path=args.color_model, dist=True)
+            distModel.prep_net(gpu_id=args.gpu, path=args.color_model, dist=True, calibrate=colorModel.act_ranges)
     elif args.backend == 'b200-caffe':
         colorModel = CI.ColorizeImageB200Caffe(Xd=args.load_size)
-        colorModel.prep_net(args.gpu, caffemodel_path=args.color_caffemodel)
+        cal = getattr(args, 'calibrate_source', None)      # a photo folder is measured once per checkpoint
+        colorModel.prep_net(args.gpu, caffemodel_path=args.color_caffemodel, calibrate=cal)
         distModel = CI.ColorizeImageB200CaffeDist(Xd=args.load_size)
-        distModel.prep_net(args.gpu, caffemodel_path=args.dist_caffemodel)
+        distModel.prep_net(args.gpu, caffemodel_path=args.dist_caffemodel, calibrate=cal)
     else:
         raise SystemExit('backend type [%s] not found! (choose from %s)' % (args.backend, ', '.join(BACKENDS)))
     return colorModel, distModel

@@ -59,6 +59,13 @@ class SIGGRAPHGeneratorB200(nn.Module):
             p.requires_grad_(False)
         self._ctx = {}                    # (H, W, max_n) -> LhnContext
         self._dirty = True
+        self.act_ranges = None            # measured activation ranges (set_act_ranges): applied to every context built
+
+    def set_act_ranges(self, ranges):
+        """{buffer: max_abs} from engine.measure_act_ranges, or None: ranges belong to the checkpoint, so every
+        context this network builds, whatever its geometry, packs its weights with them."""
+        self.act_ranges = ranges
+        self._dirty = True
 
     # --- weights: any state change re-packs lazily ---
     def load_state_dict(self, state_dict, strict=True, **kw):
@@ -87,7 +94,7 @@ class SIGGRAPHGeneratorB200(nn.Module):
                 ctx.close()
             ctx = LhnContext(device=self.b200_device, max_n=max(n, self.max_batch), H=H, W=W, dist=self.dist,
                              engine=self.engine, fast_fp16=self.fast_fp16)
-            ctx.load_state_dict(self.state_dict())
+            ctx.load_state_dict(self.state_dict(), act_ranges=self.act_ranges)
             self._ctx[key] = ctx
         return ctx
 

@@ -44,21 +44,37 @@ class ShardedColorizer(object):
     """Per-rank Local-Hints-Network context with weights received from rank 0.
 
     `state_dict` is only needed on rank 0; the other ranks allocate the (deterministically laid
-    out) arena, receive it with a single NCCL broadcast over NVLink/NVSwitch and adopt it."""
+    out) arena, receive it with a single NCCL broadcast over NVLink/NVSwitch and adopt it.
 
-    def __init__(self, H, W, per_rank_batch, state_dict=None, device=None, dist_head=False, **ctx_kw):
+    calibrate (rank 0 only; see PhotoColorizer): photos to measure the activation ranges on (H == W only: photos are
+    prepared square; calibrate_maskcent is the mask centring the forwards will use), or a saved measurement.
+    The measured storage exponents are part of the arena, so the other ranks receive them with the weights."""
+
+    def __init__(self, H, W, per_rank_batch, state_dict=None, device=None, dist_head=False, calibrate=None,
+                 calibrate_maskcent=0.0, **ctx_kw):
+        from . import engine
         from .engine import LhnContext
         self.world = dist.get_world_size() if dist.is_initialized() else 1
         self.rank = dist.get_rank() if dist.is_initialized() else 0
         self.device = torch.cuda.current_device() if device is None else device
+        ranges = None
+        if self.rank == 0 and calibrate is not None:
+            if H != W and not isinstance(calibrate, (dict, str, bytes)):
+                raise ValueError("calibrate=[photos] needs a square geometry, got %dx%d: measure at a square size with "
+                                 "engine.measure_act_ranges and pass the ranges (they do not depend on the size)" % (H, W))
+            flags = {k: v for k, v in ctx_kw.items() if k in ("global_hints", "caffe313", "keep_conv10", "options")}
+            ranges = engine.resolve_calibration(calibrate, lambda photos: engine.measure_act_ranges(
+                state_dict, engine.calibration_batch(photos, H, device=self.device,
+                                                     global_hints=flags.get("global_hints", False)),
+                H, W, device=self.device, maskcent=float(calibrate_maskcent), **flags))
         self.ctx = LhnContext(device=self.device, max_n=per_rank_batch, H=H, W=W, dist=dist_head, **ctx_kw)
         if self.world == 1:
-            self.ctx.load_state_dict(state_dict)
+            self.ctx.load_state_dict(state_dict, act_ranges=ranges)
             return
         if self.rank == 0:
             if state_dict is None:
                 raise ValueError("rank 0 needs the state_dict")
-            self.ctx.load_state_dict(state_dict)
+            self.ctx.load_state_dict(state_dict, act_ranges=ranges)
         else:
             self.ctx.reserve_weights()
         ptr, nbytes = self.ctx.weights_arena()

@@ -94,10 +94,13 @@ class PhotoColorizer(object):
     maskcent    centre the mask (siggraph_pretrained weights), as ColorizeImageTorch(maskcent=True)
     max_batch_bytes  source bytes per batch (a larger photo forms a batch by itself); two page-locked buffers of this
                 size each way hold the batches in flight
-    readahead   photos decoded ahead of the device (default 2 * batch); workers: decoding threads"""
+    readahead   photos decoded ahead of the device (default 2 * batch); workers: decoding threads
+    calibrate   None, or what sets the storage exponents of the wgmma engine's activations from measured ranges instead
+                of the weights: a list of colour photos to measure on now, a {buffer: max_abs} dict, or the path of a
+                JSON file of one (engine.save_act_ranges); the ranges used are kept in `act_ranges`"""
 
     def __init__(self, state_dict, Xd=256, batch=32, device=0, maskcent=False, global_hints=False, engine="wgmma",
-                 max_batch_bytes=96 << 20, readahead=None, workers=4):
+                 max_batch_bytes=96 << 20, readahead=None, workers=4, calibrate=None):
         if Xd < 8 or Xd % 8:
             raise ValueError("Xd must be a multiple of 8, got %d" % Xd)
         if not 1 <= batch <= _lib.MAX_PHOTOS:
@@ -107,11 +110,18 @@ class PhotoColorizer(object):
         self.max_batch_bytes = int(max_batch_bytes)
         self.readahead = int(readahead) if readahead else 2 * self.batch
         self.workers = int(workers)
+        self.act_ranges = self._calibrate(calibrate, state_dict)
         self._backend = self._make_backend(state_dict)
+
+    def _calibrate(self, calibrate, state_dict):
+        X, dev, glob = self.Xd, self.device, self.global_hints
+        return engine.resolve_calibration(calibrate, lambda photos: engine.measure_act_ranges(
+            state_dict, engine.calibration_batch(photos, X, device=dev, global_hints=glob), X, X, device=dev,
+            maskcent=0.5 if self.maskcent else 0.0, global_hints=glob))
 
     def _make_backend(self, state_dict):
         return _DeviceBatches(state_dict, self.Xd, self.batch, self.device, 0.5 if self.maskcent else 0.0,
-                              self.global_hints, self.engine, self.max_batch_bytes)
+                              self.global_hints, self.engine, self.max_batch_bytes, self.act_ranges)
 
     def colorize(self, photos, hints=None, glob=None, psnr=False):
         """photos: a sequence of paths (read as load_image reads them) or HxWx3 uint8 RGB arrays.
@@ -215,12 +225,12 @@ class _DeviceBatches(object):
     the slot's next batch that fits, or close(), returns them to max_bytes (the page-locked host memory goes back to
     the system, the device memory to torch's caching allocator)."""
 
-    def __init__(self, state_dict, X, batch, device, maskcent, global_hints, engine_name, max_bytes):
+    def __init__(self, state_dict, X, batch, device, maskcent, global_hints, engine_name, max_bytes, act_ranges=None):
         import torch
         self.torch, self.lib = torch, _lib.load()
         self.X, self.batch, self.device, self.maskcent = X, batch, device, maskcent
         self.ctx = engine.LhnContext(device=device, max_n=batch, H=X, W=X, engine=engine_name, global_hints=global_hints)
-        self.ctx.load_state_dict(state_dict)
+        self.ctx.load_state_dict(state_dict, act_ranges=act_ranges)
         dev = self.dev = torch.device("cuda:%d" % device)
         f32 = torch.float32
         # used by the compute stream only: one copy

@@ -15,7 +15,11 @@ Automatic colorization of a folder of photos, in batches on the device (photos.P
     python ideepcolor_b200.py --color_model caffemodel.pth --image_dir scans/ --out scans_color/ [--batch 32] [--psnr]
 
 writes <out>/<stem>.png per photo (the full-resolution result, get_img_fullres) and, with --psnr, <out>/psnr.csv
-(get_result_PSNR of each photo).
+(get_result_PSNR of each photo).  PSNR against the number of hint points revealed from each photo's own colours
+(photos.reveal_points), written to <out>/reveal_psnr.csv with no images:
+
+    python ideepcolor_b200.py --color_model caffemodel.pth --image_dir val/ --out sweep/ --reveal_sweep 0,1,2,5,10,20,50
+        [--reveal_seed 0] [--batch 60]
 
 hints.json: [{"loc": [row, col], "size": 3, "ab": [23, -69]}, {"loc": [100, 160], "rgb": [255, 255, 255]}, ...]
 (`loc` in load_size x load_size network coordinates, `size` = p of the notebook's put_point: a (2p+1)^2 patch.)
@@ -47,7 +51,23 @@ def parse_args(argv=None):
                     help="set the activation storage exponents from measured ranges instead of the weights: a folder of "
                          "colour photos to measure on (a seeded sample of at most 16), or a JSON file saved earlier")
     ap.add_argument("--save_act_ranges", default="", metavar="FILE", help="write the ranges --calibrate used as JSON")
+    ap.add_argument("--reveal_sweep", default="", metavar="M1,M2,...",
+                    help="with --image_dir: PSNR of every photo against the number of hint points revealed from its own "
+                         "colours, one column per level, into <out>/reveal_psnr.csv (no images are written)")
+    ap.add_argument("--reveal_seed", type=int, default=None, help="seed of the revealed points (--reveal_sweep; default 0)")
     args = ap.parse_args(argv)
+    args.reveal_levels = None
+    if args.reveal_sweep:
+        if not args.image_dir:
+            ap.error("--reveal_sweep needs --image_dir")
+        try:
+            args.reveal_levels = parse_levels(args.reveal_sweep, args.batch)
+        except ValueError as e:
+            ap.error("--reveal_sweep: %s" % e)
+    elif args.reveal_seed is not None:
+        ap.error("--reveal_seed needs --reveal_sweep")
+    if args.reveal_seed is None:
+        args.reveal_seed = 0
     args.calibrate_source = None
     if args.calibrate:
         from interactive_deep_colorization_b200 import engine
@@ -58,6 +78,16 @@ def parse_args(argv=None):
     elif args.save_act_ranges:
         ap.error("--save_act_ranges needs --calibrate")
     return args
+
+
+def parse_levels(text, batch):
+    """'0,1,2,5' -> (0, 1, 2, 5): the levels of --reveal_sweep, checked as PhotoColorizer.reveal_sweep checks them."""
+    from interactive_deep_colorization_b200 import photos
+    try:
+        levels = [int(v) for v in text.split(",")]
+    except ValueError:
+        raise ValueError("%r is not a comma-separated list of integers" % text)
+    return photos.check_levels(levels, batch)
 
 
 def save_ranges(args, ranges):
@@ -103,6 +133,8 @@ def colorize_dir(args):
     pc = PhotoColorizer(sd, Xd=args.load_size, batch=args.batch, device=args.gpu, maskcent=args.pytorch_maskcent,
                         calibrate=args.calibrate_source)
     save_ranges(args, pc.act_ranges)
+    if args.reveal_levels is not None:
+        return reveal_dir(args, pc, names, paths)
     rows = []
     for name, r in zip(names, pc.colorize(paths, psnr=args.psnr)):
         stem = os.path.splitext(name)[0]
@@ -114,6 +146,25 @@ def colorize_dir(args):
         with open(os.path.join(args.out, "psnr.csv"), "w") as f:
             f.write("image,psnr\n" + "".join(row + "\n" for row in rows))
     print("colorized %d photos into <%s>" % (len(names), args.out))
+    return 0
+
+
+def reveal_dir(args, pc, names, paths):
+    """--reveal_sweep: PhotoColorizer.reveal_sweep over the folder -> OUT/reveal_psnr.csv (a row per photo, a column per
+    level, then the mean row), and the mean curve on stdout."""
+    levels = args.reveal_levels
+    rows, curves = [], []
+    for name, r in zip(names, pc.reveal_sweep(paths, levels=levels, seed=args.reveal_seed)):
+        rows.append([name] + ["%.17g" % v for v in r.psnr])
+        curves.append(r.psnr)
+    pc.close()
+    mean = np.mean(curves, axis=0) if curves else np.full(len(levels), np.nan)
+    rows.append(["mean"] + ["%.17g" % v for v in mean])
+    with open(os.path.join(args.out, "reveal_psnr.csv"), "w") as f:
+        f.write(",".join(["image"] + [str(m) for m in levels]) + "\n" + "".join(",".join(row) + "\n" for row in rows))
+    print("reveal sweep of %d photos (seed %d), mean PSNR per number of revealed points:" % (len(names), args.reveal_seed))
+    for m, v in zip(levels, mean):
+        print("  %4d  %.3f dB" % (m, v))
     return 0
 
 

@@ -333,6 +333,19 @@ int idc_hint_raster(int device, int n, int h, int w, int count, const void* bloc
  * int64, for uint8 images a, b [n,h,w,3] (img_rgb, output_rgb), n <= 65535.  20 * log10(255 / sqrt(sse / (h*w*3))) on the host then
  * equals numpy's result bit for bit. */
 int idc_rgb_sse(int device, int n, int h, int w, const uint8_t* a, const uint8_t* b, int64_t* sse, void* stream);
+/* Hints coloured from the ground truth: the notebook's put_point(input_ab, mask, loc, p, val) (DemoInteractive-
+ * Colorization.ipynb) with val taken from the photo itself, as a simulated user who reveals points of the true colours.
+ * blocks = n_blocks hint blocks in idc_hint_raster's layout, block b at blocks + b * block_stride, DEVICE memory; block
+ * b belongs to photo b / levels of lab [*,3,X,X] float64 (as idc_rgb2lab_f64 writes it from idc_photo_prep's rgb).
+ * Every hint of a block (its count read from the header on the device, clamped to [0, IDC_MAX_HINTS] and to what
+ * block_stride holds) gets (a, b) = the mean of planes 1-2 of that photo over its rectangle clipped to X x X, summed in
+ * float64 in row-major order, divided by the pixel count and rounded once to float32; an empty rectangle gets (0, 0).
+ * The rectangles and img fields are left as they are; each block is then one idc_hint_raster block.  Deterministic.
+ * Asynchronous on `stream`.  IDC_ERR_ARG, before any device call, for n_blocks outside [1, 65535], levels < 1, X
+ * outside [1, IDC_MAX_PHOTO_X], NULL lab or blocks, and a block_stride below 16 or blocks / block_stride not a
+ * multiple of 4. */
+int idc_hint_fill_mean(int device, int n_blocks, int levels, int X, const double* lab, void* blocks, size_t block_stride,
+                       void* stream);
 
 /* ---- introspection / test hooks (used by tests/, never by the product path) ---- */
 /* wgmma engine: the exponent S with which activation `name` is stored (FP16 hi/lo planes of value * 2^S), chosen per

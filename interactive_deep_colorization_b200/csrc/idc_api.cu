@@ -1584,6 +1584,15 @@ int idc_hint_raster(int device, int n, int h, int w, int count, const void* bloc
              ? IDC_OK : IDC_ERR_CUDA;
 }
 
+int idc_hint_fill_mean(int device, int n_blocks, int levels, int X, const double* lab, void* blocks, size_t block_stride,
+                       void* stream) {
+  if (n_blocks < 1 || n_blocks > 65535 || levels < 1 || X < 1 || X > IDC_MAX_PHOTO_X || !lab || !blocks) return IDC_ERR_ARG;
+  if (block_stride < kHintHdrBytes || block_stride % 4 || (uintptr_t)blocks % 4) return IDC_ERR_ARG;   // int32 fields
+  if (cudaSetDevice(device) != cudaSuccess) return IDC_ERR_CUDA;
+  return launch_hint_fill_mean(n_blocks, levels, X, lab, static_cast<char*>(blocks), block_stride, (cudaStream_t)stream)
+             == cudaSuccess ? IDC_OK : IDC_ERR_CUDA;
+}
+
 int idc_rgb_sse(int device, int n, int h, int w, const uint8_t* a, const uint8_t* b, int64_t* sse, void* stream) {
   if (n < 1 || n > 65535 || h < 1 || w < 1 || !a || !b || !sse) return IDC_ERR_ARG;
   if (cudaSetDevice(device) != cudaSuccess) return IDC_ERR_CUDA;

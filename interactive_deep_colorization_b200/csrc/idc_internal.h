@@ -317,6 +317,9 @@ cudaError_t launch_photo_prep(int n, const idc_photo* table, const uint8_t* src,
 cudaError_t launch_photo_render(int n, const idc_photo* table, const uint8_t* src, int X, const double* lab, uint8_t* out,
                                 cudaStream_t st);
 cudaError_t launch_rgb_sse(int n, size_t hw3, const uint8_t* a, const uint8_t* b, int64_t* sse, cudaStream_t st);
+// hint blocks of `stride` bytes (>= kHintHdrBytes, a multiple of 4), checked by the caller
+cudaError_t launch_hint_fill_mean(int n_blocks, int levels, int X, const double* lab, char* blocks, size_t stride,
+                                  cudaStream_t st);
 cudaError_t launch_global_mlp(Ctx* c, int n, const float* glob, cudaStream_t st);
 cudaError_t launch_act_to_nchw(Ctx* c, const ActBuf& b, int n, float* out, cudaStream_t st);
 cudaError_t launch_nchw_to_act(Ctx* c, const ActBuf& b, int n, const float* in, cudaStream_t st);

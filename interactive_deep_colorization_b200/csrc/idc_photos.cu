@@ -5,6 +5,8 @@
 //   photo_render_kernel  one thread per full-resolution pixel of every photo: L from the pixel's own source RGB, ab
 //                        zoomed from the photo's quantised output_ab (zoom_tap / zoom_sample), lab_to_rgb_u8
 //   rgb_sse_kernel       exact int64 sum of squared differences per image (get_result_PSNR before its float64 tail)
+//   hint_fill_mean_kernel  one thread per hint of a batch of hint blocks: the mean ground-truth ab under the hint's
+//                        rectangle (a simulated user revealing points of the photo's own colours)
 // The per-pixel arithmetic is the one of resize_linear_u8_kernel, rgb2lab_kernel and render_planes_kernel (the device
 // functions in idc_internal.h), so every photo equals the single-image path bit for bit.
 #include <algorithm>
@@ -94,6 +96,40 @@ __global__ void __launch_bounds__(256) rgb_sse_kernel(size_t hw3, const uint8_t*
   }
 }
 
+// grid (chunks, n_blocks): thread i of column b sets hint i of block b to the mean of planes 1-2 of photo b / levels of
+// lab over the hint's rectangle clipped to X x X, summed in float64 in row-major order and rounded once to float32.
+// The sums start at -0.0, the identity of IEEE addition, so they equal a sequential sum from the first pixel bit for
+// bit (signed zeros included).  A hint whose clipped rectangle is empty gets (0, 0); the raster skips it anyway.
+constexpr int kFillThreads = 128;
+
+__global__ void __launch_bounds__(kFillThreads) hint_fill_mean_kernel(int levels, int X, const double* __restrict__ lab,
+                                                                      char* __restrict__ blocks, size_t stride, int cap) {
+  char* blk = blocks + (size_t)blockIdx.y * stride;
+  const int count = min(max(*reinterpret_cast<const int*>(blk), 0), cap);   // as the raster reads it, within the stride
+  const int i = blockIdx.x * kFillThreads + threadIdx.x;
+  if (i >= count) return;
+  idc_hint* h = reinterpret_cast<idc_hint*>(blk + kHintHdrBytes) + i;
+  const int y0 = max(h->y0, 0), x0 = max(h->x0, 0), y1 = min(h->y1, X - 1), x1 = min(h->x1, X - 1);
+  float a = 0.f, b = 0.f;
+  if (y0 <= y1 && x0 <= x1) {
+    const size_t XX = (size_t)X * X;
+    const double* pa = lab + ((size_t)(blockIdx.y / levels) * 3 + 1) * XX;
+    const double* pb = pa + XX;
+    double sa = -0.0, sb = -0.0;
+    for (int y = y0; y <= y1; ++y) {
+      for (int x = x0; x <= x1; ++x) {
+        sa = __dadd_rn(sa, pa[(size_t)y * X + x]);
+        sb = __dadd_rn(sb, pb[(size_t)y * X + x]);
+      }
+    }
+    const double cnt = (double)((int64_t)(y1 - y0 + 1) * (x1 - x0 + 1));
+    a = __double2float_rn(__ddiv_rn(sa, cnt));
+    b = __double2float_rn(__ddiv_rn(sb, cnt));
+  }
+  h->a = a;
+  h->b = b;
+}
+
 static PhotoTable make_table(int n, const idc_photo* table) {
   PhotoTable t{};
   for (int i = 0; i < n; ++i) t.p[i] = table[i];
@@ -119,6 +155,15 @@ cudaError_t launch_rgb_sse(int n, size_t hw3, const uint8_t* a, const uint8_t* b
   if (e != cudaSuccess) return e;
   const dim3 grid((unsigned)std::min<size_t>((hw3 + 255) / 256, 64), (unsigned)n);
   rgb_sse_kernel<<<grid, 256, 0, st>>>(hw3, a, b, reinterpret_cast<unsigned long long*>(sse));
+  return cudaGetLastError();
+}
+
+cudaError_t launch_hint_fill_mean(int n_blocks, int levels, int X, const double* lab, char* blocks, size_t stride,
+                                  cudaStream_t st) {
+  const int cap = (int)std::min<size_t>((stride - kHintHdrBytes) / sizeof(idc_hint), IDC_MAX_HINTS);
+  if (cap == 0) return cudaSuccess;                      // blocks without room for a hint: nothing to fill
+  const dim3 grid((unsigned)((cap + kFillThreads - 1) / kFillThreads), (unsigned)n_blocks);
+  hint_fill_mean_kernel<<<grid, kFillThreads, 0, st>>>(levels, X, lab, blocks, stride, cap);
   return cudaGetLastError();
 }
 

@@ -13,10 +13,17 @@ into one page-locked buffer and goes through the device as
 with two sets of buffers, so that batch k+1 is read, packed and uploaded and batch k-1 is copied back while batch k
 computes.  Every value equals the single-photo path on the same forward: prep is the cv2-exact resize + skimage Lab of
 `load_image`, the render is `get_img_fullres`'s scipy zoom of the quantised output_ab, and the PSNR is numpy's.
+
+`PhotoColorizer.reveal_sweep` measures PSNR against the number of hint points revealed from each photo's own ground
+truth (`reveal_points`), all levels of a photo in the same device pass:
+
+    H2D -> idc_photo_prep -> idc_rgb2lab_f64 (ground truth) -> idc_hint_fill_mean -> idc_hint_raster per image
+    -> L and img_rgb repeated once per level -> idc_forward -> idc_rgb_sse -> D2H of the network-size results
 """
 import collections
 import concurrent.futures
 import ctypes
+import math
 import os
 
 import numpy as np
@@ -30,7 +37,60 @@ PhotoResult.__doc__ = """One colorized photo.
     ab       float32 [2,X,X] output_ab_raw (the raw network output)
     psnr     float or None   get_result_PSNR() against the network-size photo, when asked for"""
 
+RevealResult = collections.namedtuple("RevealResult", "psnr ab rgb points")
+RevealResult.__doc__ = """One photo of a reveal sweep, over the L levels in the order given.
+    psnr    float64 [L]          get_result_PSNR() of each level's output_rgb against the network-size photo
+    ab      float32 [L,2,X,X]    output_ab_raw of each level
+    rgb     uint8 [L,X,X,3]      output_rgb of each level
+    points  int32 [max(levels),3] the revealed points (y0, x0, P) (reveal_points); level m used the first m"""
+
 XFULLRES_MAX = 10000          # the wrapper's Xfullres_max (ColorizeImageBase): larger photos are resized on the host
+REVEAL_LEVELS = (0, 1, 2, 5, 10, 20, 50, 100, 200, 500)
+
+
+def reveal_points(X, m, seed, index):
+    """The first m points a simulated user reveals on the X x X network grid of photo number `index` -> int32 [m, 3],
+    one row (y0, x0, P) per point: a P x P square with top-left corner (y0, x0), painted with the photo's mean
+    ground-truth colour under it.  Following the paper's description of its simulated user (centred Gaussian
+    locations, square patches of 1 to 9 pixels), with rng = np.random.default_rng([seed, index]), each point draws
+        P = rng.integers(1, 10);  cy, cx = rng.normal(X / 2, X / 4, 2)
+        y0 = clip(floor(cy) - (P - 1) // 2, 0, X - P),  x0 likewise from cx
+    in that order.  A photo's points depend only on (seed, index), not on how photos are batched, and the first m points
+    are a prefix of the first m + 1.  This is this package's rule, not the authors' evaluation sampling (which was not
+    published with the code), so curves from it are not comparable with the paper's figures.  X must be at least 9."""
+    if X < 9:
+        raise ValueError("reveal_points: X = %d, need at least 9 for a 9 x 9 patch" % X)
+    if m < 0:
+        raise ValueError("reveal_points: m = %d < 0" % m)
+    rng = np.random.default_rng([int(seed), int(index)])
+    integers, normal = rng.integers, rng.normal
+    out = []
+    for _ in range(m):
+        P = int(integers(1, 10))
+        cy, cx = normal(X / 2, X / 4, 2).tolist()
+        lo = (P - 1) // 2
+        out.append((min(max(math.floor(cy) - lo, 0), X - P), min(max(math.floor(cx) - lo, 0), X - P), P))
+    return np.array(out, np.int32).reshape(m, 3)
+
+
+def check_levels(levels, batch):
+    """levels of a reveal sweep -> tuple of int.  Raise ValueError unless they are distinct integers in
+    [0, IDC_MAX_HINTS] and at most `batch` of them (one device pass carries every level of a photo)."""
+    try:
+        levels = list(levels)
+    except TypeError:
+        raise ValueError("levels: need a sequence of integers, got %r" % (levels,))
+    if not levels:
+        raise ValueError("levels: need at least one level")
+    for v in levels:
+        if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, np.integer)) or not 0 <= v <= _lib.MAX_HINTS:
+            raise ValueError("levels: %r is not an integer in [0, %d]" % (v, _lib.MAX_HINTS))
+    levels = tuple(int(v) for v in levels)
+    if len(set(levels)) != len(levels):
+        raise ValueError("levels: %s repeats a level" % (levels,))
+    if len(levels) > batch:
+        raise ValueError("%d levels do not fit one device pass of batch = %d" % (len(levels), batch))
+    return levels
 
 
 def read_photo(path):
@@ -131,11 +191,7 @@ class PhotoColorizer(object):
         exceed Xfullres_max raise ValueError here, before any device work; a path is checked when it is read, before
         its batch is submitted."""
         n = len(photos)
-        for i, p in enumerate(photos):
-            if isinstance(p, np.ndarray):
-                check_photo(p, "photo %d" % i)
-            elif not isinstance(p, (str, bytes, os.PathLike)):
-                raise ValueError("photo %d: need a path or an HxWx3 uint8 array, got %s" % (i, type(p).__name__))
+        self._check_photos(photos)
         if hints is not None:
             if len(hints) != n:
                 raise ValueError("%d hint lists for %d photos" % (len(hints), n))
@@ -150,6 +206,39 @@ class PhotoColorizer(object):
                 raise ValueError("every glob vector must have 316 values")
         return self._run(photos, hints, glob, bool(psnr))
 
+    def reveal_sweep(self, photos, levels=REVEAL_LEVELS, seed=0):
+        """PSNR against the number of revealed hint points: for every photo and every level m, the network-size result
+        with the first m points of reveal_points(Xd, max(levels), seed, i) (i = the photo's position in `photos`) as
+        hints, each painted with the photo's mean ground-truth ab under it (idc_hint_fill_mean, the Lab of the
+        network-size photo).  A device pass carries batch // len(levels) photos, each as len(levels) consecutive forward
+        images; nothing is rendered at full resolution.
+        photos: as colorize.  levels: distinct integers in [0, IDC_MAX_HINTS], at most `batch` of them.
+        -> iterator of RevealResult, in input order.  Bad levels or photos raise ValueError here, before any device
+        work (paths as in colorize)."""
+        levels = check_levels(levels, self.batch)
+        if self.Xd < 9:
+            raise ValueError("reveal_sweep needs Xd >= 9 for a 9 x 9 patch, got %d" % self.Xd)
+        self._check_photos(photos)
+        seed = int(seed)
+        M = max(levels)
+
+        def items():
+            for i, a in self._read(photos):
+                yield a.nbytes, 0, (i, a, reveal_points(self.Xd, M, seed, i))
+
+        per = self.batch // len(levels)
+        return self._pipeline(cut_batches(items(), per, self.max_batch_bytes),
+                              lambda b: self._backend.submit_reveal([a for _, a, _ in b], [p for _, _, p in b], levels),
+                              self._backend.collect_reveal)
+
+    @staticmethod
+    def _check_photos(photos):
+        for i, p in enumerate(photos):
+            if isinstance(p, np.ndarray):
+                check_photo(p, "photo %d" % i)
+            elif not isinstance(p, (str, bytes, os.PathLike)):
+                raise ValueError("photo %d: need a path or an HxWx3 uint8 array, got %s" % (i, type(p).__name__))
+
     @staticmethod
     def _hint_list(h, i):
         if h is None:
@@ -159,34 +248,43 @@ class PhotoColorizer(object):
             raise ValueError("photo %d: %d hints, at most %d" % (i, h.shape[0], _lib.MAX_HINTS))
         return h
 
-    def _run(self, photos, hints, glob, psnr):
+    def _read(self, photos):
+        """(index, photo array) in input order, decoded `readahead` ahead of the consumer."""
         def load(i):
             p = photos[i]
             if isinstance(p, np.ndarray):
                 return i, np.ascontiguousarray(p)
             return i, check_photo(read_photo(p), "photo %d (%s)" % (i, p))
+        return read_ahead(range(len(photos)), load, self.readahead, self.workers)
 
+    def _run(self, photos, hints, glob, psnr):
         def items():
-            for i, a in read_ahead(range(len(photos)), load, self.readahead, self.workers):
+            for i, a in self._read(photos):
                 nh = 0 if hints is None or hints[i] is None else hints[i].shape[0]
                 yield a.nbytes, nh, (i, a)
 
+        def submit(b):
+            idx = [i for i, _ in b]
+            return self._backend.submit([a for _, a in b], None if hints is None else [hints[i] for i in idx],
+                                        None if glob is None else [glob[i] for i in idx], psnr)
+
+        return self._pipeline(cut_batches(items(), self.batch, self.max_batch_bytes), submit, self._backend.collect)
+
+    def _pipeline(self, batches, submit, collect):
         # Batch k-1 is collected after batch k is submitted, so the device always has the next batch queued.  Whatever
         # ends the iteration early (a break, an abandoned iterator, a photo that fails to read) still collects the batch
         # in flight, so no batch is left behind in a buffer slot.
         pending = None
         try:
-            for b in cut_batches(items(), self.batch, self.max_batch_bytes):
-                idx = [i for i, _ in b]
-                token = self._backend.submit([a for _, a in b], None if hints is None else [hints[i] for i in idx],
-                                             None if glob is None else [glob[i] for i in idx], psnr)
+            for b in batches:
+                token = submit(b)
                 prev, pending = pending, token
                 if prev is not None:
-                    for r in self._backend.collect(prev):
+                    for r in collect(prev):
                         yield r
             last, pending = pending, None
             if last is not None:
-                for r in self._backend.collect(last):
+                for r in collect(last):
                     yield r
         finally:
             if pending is not None:
@@ -284,14 +382,16 @@ class _DeviceBatches(object):
         s["cap"] = cap
         self._after_alloc()
 
-    def submit(self, photos, hints, glob, psnr):
-        torch, lib, X = self.torch, self.lib, self.X
-        n = len(photos)
+    def _next_slot(self):
         s = self.slots[self.k % 2]
         self.k += 1
         s["ev_out"].synchronize()          # the slot's previous batch (if any) is off the device: render, D2H, all
         s["batch"] = self.k
-        table = np.zeros(n, _lib.PHOTO_DTYPE)
+        return s
+
+    def _pack(self, s, photos):
+        """The batch's photo table; the photos packed back to back into slot s's page-locked source buffer."""
+        table = np.zeros(len(photos), _lib.PHOTO_DTYPE)
         off = 0
         for i, a in enumerate(photos):
             table[i] = (off, a.shape[0], a.shape[1])
@@ -302,6 +402,13 @@ class _DeviceBatches(object):
         for i, a in enumerate(photos):
             o = int(table[i]["off"]) * 3
             h_src[o:o + a.nbytes] = a.reshape(-1)
+        return table, nbytes
+
+    def submit(self, photos, hints, glob, psnr):
+        torch, lib, X = self.torch, self.lib, self.X
+        n = len(photos)
+        s = self._next_slot()
+        table, nbytes = self._pack(s, photos)
         count = 0
         if hints is not None:
             lists = []
@@ -371,6 +478,90 @@ class _DeviceBatches(object):
             if psnr:    # get_result_PSNR: 20 * log10(255 / sqrt(mean(err2))); the sum of err2 is exact, so is the mean
                 p = float(20 * np.log10(255. / np.sqrt(np.float64(sse[i]) / N)))
             out.append(PhotoResult(full[off * 3:(off + h * w) * 3].reshape(h, w, 3).copy(), rgb[i].copy(), ab[i].copy(), p))
+        return out
+
+    def _reveal_buffers(self):
+        """Buffers of reveal sweeps, made on the first one: the prepared photos before they are repeated per level
+        (compute stream only, one copy) and, per slot, room for `batch` hint blocks of IDC_MAX_HINTS hints each."""
+        if getattr(self, "L_photo", None) is None:
+            torch, X, n, dev = self.torch, self.X, self.batch, self.dev
+            self.L_photo = torch.empty((n, 1, X, X), dtype=torch.float32, device=dev)
+            self.rgb_photo = torch.empty((n, X, X, 3), dtype=torch.uint8, device=dev)
+            nb = n * (_lib.HINT_HDR_BYTES + _lib.MAX_HINTS * _lib.HINT_DTYPE.itemsize)
+            for s in self.slots:
+                s["blocks"] = torch.empty((nb,), dtype=torch.uint8, device=dev)
+                s["h_blocks"] = torch.empty((nb,), dtype=torch.uint8, pin_memory=True)
+            self._after_alloc()
+
+    def submit_reveal(self, photos, points, levels):
+        """One device pass of a reveal sweep: photo i of the batch is forward images i*L .. i*L+L-1 (L = len(levels)),
+        image i*L+j with the first levels[j] rows of points[i] as hints."""
+        torch, lib, X = self.torch, self.lib, self.X
+        m, L = len(photos), len(levels)
+        N = m * L
+        self._reveal_buffers()
+        s = self._next_slot()
+        table, nbytes = self._pack(s, photos)
+        # hint blocks, one per forward image, in idc_hint_raster's layout; the colours are filled on the device
+        stride = _lib.HINT_HDR_BYTES + (max(levels) * _lib.HINT_DTYPE.itemsize + 15) // 16 * 16
+        hb = s["h_blocks"].numpy()[:N * stride].reshape(N, stride)
+        for i, pts in enumerate(points):
+            rect = np.zeros(max(levels), _lib.HINT_DTYPE)
+            rect["y0"], rect["x0"] = pts[:, 0], pts[:, 1]
+            rect["y1"], rect["x1"] = pts[:, 0] + pts[:, 2] - 1, pts[:, 1] + pts[:, 2] - 1
+            raw = rect.view(np.uint8)
+            for j, c in enumerate(levels):
+                row = hb[i * L + j]
+                row[:_lib.HINT_HDR_BYTES].view(np.int32)[:] = (c, 0, 0, 0)
+                row[_lib.HINT_HDR_BYTES:_lib.HINT_HDR_BYTES + c * _lib.HINT_DTYPE.itemsize] = raw[:c * _lib.HINT_DTYPE.itemsize]
+
+        with torch.cuda.stream(self.s_in):
+            s["src"][:nbytes].copy_(s["h_src"].tensor[:nbytes], non_blocking=True)
+            s["blocks"][:N * stride].copy_(s["h_blocks"][:N * stride], non_blocking=True)
+            s["ev_in"].record(self.s_in)
+
+        st = self.s_comp
+        st.wait_event(s["ev_in"])
+        sh = st.cuda_stream
+        blocks = s["blocks"].data_ptr()
+        with torch.cuda.stream(st):
+            _lib.check(None, lib.idc_photo_prep(self.device, m, table.ctypes.data, s["src"].data_ptr(), X,
+                                                self.L_photo.data_ptr(), self.rgb_photo.data_ptr(), sh))
+            _lib.check(None, lib.idc_rgb2lab_f64(self.device, m, X, X, self.rgb_photo.data_ptr(), self.lab.data_ptr(), sh))
+            _lib.check(None, lib.idc_hint_fill_mean(self.device, N, L, X, self.lab.data_ptr(), blocks, stride, sh))
+            for b in range(N):
+                _lib.check(None, lib.idc_hint_raster(self.device, 1, X, X, levels[b % L], blocks + b * stride,
+                                                     self.ab_in[b].data_ptr(), self.mask[b].data_ptr(), sh))
+            self.L_mc[:N].view(m, L, 1, X, X).copy_(self.L_photo[:m, None].expand(m, L, 1, X, X))
+            s["img_rgb"][:N].view(m, L, X, X, 3).copy_(self.rgb_photo[:m, None].expand(m, L, X, X, 3))
+            self.ctx.forward_device(self.L_mc[:N], self.ab_in[:N], self.mask[:N], self.maskcent, want_rgb=True,
+                                    out_ab=s["ab"][:N], out_rgb=s["rgb"][:N])
+            _lib.check(None, lib.idc_rgb_sse(self.device, N, X, X, s["img_rgb"].data_ptr(), s["rgb"].data_ptr(),
+                                             s["sse"].data_ptr(), sh))
+            s["ev_comp"].record(st)
+
+        with torch.cuda.stream(self.s_out):
+            self.s_out.wait_event(s["ev_comp"])
+            s["h_ab"][:N].copy_(s["ab"][:N], non_blocking=True)
+            s["h_rgb"][:N].copy_(s["rgb"][:N], non_blocking=True)
+            s["h_sse"][:N].copy_(s["sse"][:N], non_blocking=True)
+            s["ev_out"].record(self.s_out)
+        return s, s["batch"], points, L
+
+    def collect_reveal(self, token):
+        s, batch, points, L = token
+        if s["batch"] != batch:
+            raise RuntimeError("this batch's buffers were reused by a later batch: iterate one result iterator at a "
+                               "time per PhotoColorizer")
+        s["ev_out"].synchronize()
+        ab, rgb, sse = s["h_ab"].numpy(), s["h_rgb"].numpy(), s["h_sse"].numpy()
+        N = self.X * self.X * 3
+        out = []
+        for i, pts in enumerate(points):
+            k = slice(i * L, (i + 1) * L)
+            # the formula of collect(): get_result_PSNR with an exact sum of err2
+            psnr = np.array([float(20 * np.log10(255. / np.sqrt(np.float64(e) / N))) for e in sse[k]], np.float64)
+            out.append(RevealResult(psnr, ab[k].copy(), rgb[k].copy(), pts))
         return out
 
     def discard(self, token):

@@ -21,6 +21,14 @@ writes <out>/<stem>.png per photo (the full-resolution result, get_img_fullres) 
     python ideepcolor_b200.py --color_model caffemodel.pth --image_dir val/ --out sweep/ --reveal_sweep 0,1,2,5,10,20,50
         [--reveal_seed 0] [--batch 60]
 
+With a global-hints checkpoint (--global_hints: the glob.* keys; --caffe: Caffe-scaled weights such as the global
+model's), every photo of the folder coloured with a reference photo's ab histogram (DemoGlobalHistogramTransfer.ipynb),
+or PSNR under the global-hints conditions taken from each photo itself (none, sat, hist, hist+sat) written to
+<out>/glob_psnr.csv with no images:
+
+    python ideepcolor_b200.py --color_model glob.pth --global_hints --caffe --image_dir scans/ --out o/ --glob_ref ref.jpg
+    python ideepcolor_b200.py --color_model glob.pth --global_hints --image_dir val/ --out o/ --glob_sweep [none,hist]
+
 hints.json: [{"loc": [row, col], "size": 3, "ab": [23, -69]}, {"loc": [100, 160], "rgb": [255, 255, 255]}, ...]
 (`loc` in load_size x load_size network coordinates, `size` = p of the notebook's put_point: a (2p+1)^2 patch.)
 """
@@ -55,7 +63,35 @@ def parse_args(argv=None):
                     help="with --image_dir: PSNR of every photo against the number of hint points revealed from its own "
                          "colours, one column per level, into <out>/reveal_psnr.csv (no images are written)")
     ap.add_argument("--reveal_seed", type=int, default=None, help="seed of the revealed points (--reveal_sweep; default 0)")
+    ap.add_argument("--global_hints", action="store_true",
+                    help="the checkpoint has the global-hints branch (glob.* keys; --image_dir)")
+    ap.add_argument("--caffe", action="store_true",
+                    help="Caffe-scaled weights (mask x 110 and tanh x 100, as ColorizeImageCaffe; --image_dir)")
+    ap.add_argument("--glob_ref", default="", metavar="REF",
+                    help="with --global_hints: colour every photo with the ab histogram of photo REF (histogram transfer)")
+    ap.add_argument("--glob_sweep", nargs="?", const="", default=None, metavar="C1,C2,...",
+                    help="with --global_hints: PSNR of every photo under global hints from its own statistics, one "
+                         "column per condition of none,sat,hist,hist+sat (default all four), into <out>/glob_psnr.csv "
+                         "(no images are written)")
     args = ap.parse_args(argv)
+    given = {"global_hints": args.global_hints, "caffe": args.caffe, "glob_ref": bool(args.glob_ref),
+             "glob_sweep": args.glob_sweep is not None}
+    for flag in ("global_hints", "caffe", "glob_ref", "glob_sweep"):
+        if given[flag] and not args.image_dir:
+            ap.error("--%s needs --image_dir" % flag)
+    if args.caffe and args.pytorch_maskcent:
+        ap.error("--caffe and --pytorch_maskcent exclude each other: the Caffe models do not centre the mask")
+    args.glob_conditions = None
+    if args.glob_ref or args.glob_sweep is not None:
+        if not args.global_hints:
+            ap.error("--%s needs --global_hints" % ("glob_ref" if args.glob_ref else "glob_sweep"))
+    if args.glob_sweep is not None:
+        if args.glob_ref or args.reveal_sweep:
+            ap.error("--glob_sweep excludes --%s" % ("glob_ref" if args.glob_ref else "reveal_sweep"))
+        try:
+            args.glob_conditions = parse_conditions(args.glob_sweep, args.batch)
+        except ValueError as e:
+            ap.error("--glob_sweep: %s" % e)
     args.reveal_levels = None
     if args.reveal_sweep:
         if not args.image_dir:
@@ -88,6 +124,13 @@ def parse_levels(text, batch):
     except ValueError:
         raise ValueError("%r is not a comma-separated list of integers" % text)
     return photos.check_levels(levels, batch)
+
+
+def parse_conditions(text, batch):
+    """'none,hist' -> ('none', 'hist'), '' -> all of photos.GLOBAL_CONDITIONS: the conditions of --glob_sweep, checked
+    as PhotoColorizer.global_sweep checks them."""
+    from interactive_deep_colorization_b200 import photos
+    return photos.check_conditions(text.split(",") if text else photos.GLOBAL_CONDITIONS, batch)
 
 
 def save_ranges(args, ranges):
@@ -131,12 +174,19 @@ def colorize_dir(args):
         os.makedirs(args.out)
     sd = torch.load(args.color_model, map_location="cpu")
     pc = PhotoColorizer(sd, Xd=args.load_size, batch=args.batch, device=args.gpu, maskcent=args.pytorch_maskcent,
-                        calibrate=args.calibrate_source)
+                        calibrate=args.calibrate_source, global_hints=args.global_hints, caffe=args.caffe)
     save_ranges(args, pc.act_ranges)
     if args.reveal_levels is not None:
         return reveal_dir(args, pc, names, paths)
+    if args.glob_conditions is not None:
+        return glob_sweep_dir(args, pc, names, paths)
+    glob = None
+    if args.glob_ref:         # histogram transfer: every photo with REF's histogram (DemoGlobalHistogramTransfer.ipynb)
+        from interactive_deep_colorization_b200 import photos
+        ref = next(iter(pc.global_stats([args.glob_ref])))
+        glob = [photos.glob_vector(ref, "hist")] * len(paths)
     rows = []
-    for name, r in zip(names, pc.colorize(paths, psnr=args.psnr)):
+    for name, r in zip(names, pc.colorize(paths, glob=glob, psnr=args.psnr)):
         stem = os.path.splitext(name)[0]
         cv2.imwrite(os.path.join(args.out, stem + ".png"), np.ascontiguousarray(r.fullres[:, :, ::-1]))
         if args.psnr:
@@ -165,6 +215,25 @@ def reveal_dir(args, pc, names, paths):
     print("reveal sweep of %d photos (seed %d), mean PSNR per number of revealed points:" % (len(names), args.reveal_seed))
     for m, v in zip(levels, mean):
         print("  %4d  %.3f dB" % (m, v))
+    return 0
+
+
+def glob_sweep_dir(args, pc, names, paths):
+    """--glob_sweep: PhotoColorizer.global_sweep over the folder -> OUT/glob_psnr.csv (a row per photo, a column per
+    condition, then the mean row), and the mean per condition on stdout."""
+    conds = args.glob_conditions
+    rows, curves = [], []
+    for name, r in zip(names, pc.global_sweep(paths, conditions=conds)):
+        rows.append([name] + ["%.17g" % v for v in r.psnr])
+        curves.append(r.psnr)
+    pc.close()
+    mean = np.mean(curves, axis=0) if curves else np.full(len(conds), np.nan)
+    rows.append(["mean"] + ["%.17g" % v for v in mean])
+    with open(os.path.join(args.out, "glob_psnr.csv"), "w") as f:
+        f.write(",".join(["image"] + list(conds)) + "\n" + "".join(",".join(row) + "\n" for row in rows))
+    print("global-hints sweep of %d photos, mean PSNR per condition:" % len(names))
+    for c, v in zip(conds, mean):
+        print("  %-8s  %.3f dB" % (c, v))
     return 0
 
 

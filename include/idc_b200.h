@@ -346,6 +346,18 @@ int idc_rgb_sse(int device, int n, int h, int w, const uint8_t* a, const uint8_t
  * multiple of 4. */
 int idc_hint_fill_mean(int device, int n_blocks, int levels, int X, const double* lab, void* blocks, size_t block_stride,
                        void* stream);
+/* Global-hints statistics of a batch of network-size images (global_stats.prototxt, as idc_global_stats): rgb [n,h,w,3]
+ * uint8 (the layout idc_photo_prep writes img_rgb in), pts313 [313,2] -> out [n,316] float32, row i = [313-bin
+ * histogram, 1, s_avg, 1], the `glob` layout of idc_forward.  Per 4x4 cell: the Lab of its 16 pixels (the arithmetic of
+ * idc_rgb2lab_f64), a and b summed in float64 in row-major order, / 16, rounded once to float32; the cell's bin is the
+ * first minimum of the float32 squared distance with every operation rounded separately (numpy's
+ * ((ab - pts)**2).sum(-1)).  hist[k] = float32(count_k / cells) from float64; s_avg = float32 of the float64 mean of
+ * skimage's HSV saturation over the h*w pixels, summed in a fixed order.  One CTA per image; a row is identical bit for
+ * bit whatever n, wherever the image sits in the batch, and on every run.  Reads no host memory and allocates nothing,
+ * so it can be captured in a graph.  DEVICE ptrs, asynchronous on `stream`.  IDC_ERR_ARG, before any device call, for
+ * n outside [1, 65535], h or w below 4, not a multiple of 4 or above IDC_MAX_PHOTO_X, and a NULL pointer. */
+int idc_global_stats_batch(int device, int n, int h, int w, const uint8_t* rgb, const float* pts313, float* out,
+                           void* stream);
 
 /* ---- introspection / test hooks (used by tests/, never by the product path) ---- */
 /* wgmma engine: the exponent S with which activation `name` is stored (FP16 hi/lo planes of value * 2^S), chosen per

@@ -81,6 +81,7 @@ SYMBOLS = [
     ("idc_hint_raster", _c.c_int, [_c.c_int, _c.c_int, _c.c_int, _c.c_int, _c.c_int, _P, _P, _P, _P]),
     ("idc_rgb_sse", _c.c_int, [_c.c_int, _c.c_int, _c.c_int, _c.c_int, _P, _P, _P, _P]),
     ("idc_hint_fill_mean", _c.c_int, [_c.c_int, _c.c_int, _c.c_int, _c.c_int, _P, _P, _c.c_size_t, _P]),
+    ("idc_global_stats_batch", _c.c_int, [_c.c_int, _c.c_int, _c.c_int, _c.c_int, _P, _P, _P, _P]),
     ("idc_get_activation", _c.c_int, [_P, _c.c_char_p, _P, _c.c_size_t, _c.POINTER(_c.c_int),
                                       _c.POINTER(_c.c_int), _c.POINTER(_c.c_int)]),
     ("idc_set_activation", _c.c_int, [_P, _c.c_char_p, _c.c_int, _P]),

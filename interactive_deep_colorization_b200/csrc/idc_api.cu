@@ -1593,6 +1593,14 @@ int idc_hint_fill_mean(int device, int n_blocks, int levels, int X, const double
              == cudaSuccess ? IDC_OK : IDC_ERR_CUDA;
 }
 
+int idc_global_stats_batch(int device, int n, int h, int w, const uint8_t* rgb, const float* pts313, float* out,
+                           void* stream) {
+  if (n < 1 || n > 65535 || h < 4 || w < 4 || (h % 4) || (w % 4) || h > IDC_MAX_PHOTO_X || w > IDC_MAX_PHOTO_X) return IDC_ERR_ARG;
+  if (!rgb || !pts313 || !out) return IDC_ERR_ARG;
+  if (cudaSetDevice(device) != cudaSuccess) return IDC_ERR_CUDA;
+  return launch_global_stats_batch(n, h, w, rgb, pts313, out, (cudaStream_t)stream) == cudaSuccess ? IDC_OK : IDC_ERR_CUDA;
+}
+
 int idc_rgb_sse(int device, int n, int h, int w, const uint8_t* a, const uint8_t* b, int64_t* sse, void* stream) {
   if (n < 1 || n > 65535 || h < 1 || w < 1 || !a || !b || !sse) return IDC_ERR_ARG;
   if (cudaSetDevice(device) != cudaSuccess) return IDC_ERR_CUDA;

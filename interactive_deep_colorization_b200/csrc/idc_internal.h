@@ -320,6 +320,9 @@ cudaError_t launch_rgb_sse(int n, size_t hw3, const uint8_t* a, const uint8_t* b
 // hint blocks of `stride` bytes (>= kHintHdrBytes, a multiple of 4), checked by the caller
 cudaError_t launch_hint_fill_mean(int n_blocks, int levels, int X, const double* lab, char* blocks, size_t stride,
                                   cudaStream_t st);
+// n in [1, 65535], h and w multiples of 4 in [4, IDC_MAX_PHOTO_X], checked by the caller
+cudaError_t launch_global_stats_batch(int n, int h, int w, const uint8_t* rgb, const float* pts, float* out,
+                                      cudaStream_t st);
 cudaError_t launch_global_mlp(Ctx* c, int n, const float* glob, cudaStream_t st);
 cudaError_t launch_act_to_nchw(Ctx* c, const ActBuf& b, int n, float* out, cudaStream_t st);
 cudaError_t launch_nchw_to_act(Ctx* c, const ActBuf& b, int n, const float* in, cudaStream_t st);

@@ -7,6 +7,8 @@
 //   rgb_sse_kernel       exact int64 sum of squared differences per image (get_result_PSNR before its float64 tail)
 //   hint_fill_mean_kernel  one thread per hint of a batch of hint blocks: the mean ground-truth ab under the hint's
 //                        rectangle (a simulated user revealing points of the photo's own colours)
+//   global_stats_batch_kernel  one CTA per network-size image: the global-hints statistics (313-bin histogram of the
+//                        4x4-pooled ab, mean HSV saturation) of a batch, deterministic and independent of the batch
 // The per-pixel arithmetic is the one of resize_linear_u8_kernel, rgb2lab_kernel and render_planes_kernel (the device
 // functions in idc_internal.h), so every photo equals the single-image path bit for bit.
 #include <algorithm>
@@ -130,6 +132,71 @@ __global__ void __launch_bounds__(kFillThreads) hint_fill_mean_kernel(int levels
   h->b = b;
 }
 
+// grid n, one CTA per image: global_stats.prototxt (rgb2lab -> 4x4 average pool of ab -> nearest of the 313 bins ->
+// global average; mean HSV saturation) for image blockIdx.x of rgb [n,h,w,3].  Thread t takes cells t, t + T, ...; a
+// cell's ab is the float64 row-major sum of its 16 pixels / 16, rounded once to float32, and its bin the first minimum
+// of the float32 ((a - pa)^2 + (b - pb)^2) with every operation rounded separately (numpy's order, no FMA).  Bin counts
+// are integer shared-memory atomics; the saturation partials are reduced in a fixed tree.  Nothing depends on n or on
+// where the image sits in the batch, so a row is identical bit for bit in any batch and on every run.
+constexpr int kStatsThreads = 512;
+
+__global__ void __launch_bounds__(kStatsThreads) global_stats_batch_kernel(int h, int w, const uint8_t* __restrict__ rgb,
+                                                                           const float* __restrict__ pts,
+                                                                           float* __restrict__ out) {
+  __shared__ int count[313];
+  __shared__ float2 bins[313];
+  __shared__ double s_warp[kStatsThreads / 32];
+  for (int k = threadIdx.x; k < 313; k += kStatsThreads) {
+    count[k] = 0;
+    bins[k] = make_float2(pts[2 * k], pts[2 * k + 1]);
+  }
+  __syncthreads();
+  const uint8_t* img = rgb + (size_t)blockIdx.x * h * w * 3;
+  const int w4 = w / 4, cells = (h / 4) * w4;
+  double sat = 0.0;
+  for (int c = threadIdx.x; c < cells; c += kStatsThreads) {
+    const int cy = c / w4, cx = c - cy * w4;
+    double sa = -0.0, sb = -0.0;
+    for (int dy = 0; dy < 4; ++dy) {
+      const uint8_t* row = img + ((size_t)(cy * 4 + dy) * w + cx * 4) * 3;
+      for (int dx = 0; dx < 4; ++dx) {
+        const uint8_t* px = row + dx * 3;
+        double l, a, b;
+        rgb_u8_to_lab(px, l, a, b);
+        sa = __dadd_rn(sa, a);
+        sb = __dadd_rn(sb, b);
+        // skimage rgb2hsv: S = (max - min) / max of the /255 values, 0 where max = 0
+        const double r8 = px[0] / 255.0, g8 = px[1] / 255.0, b8 = px[2] / 255.0;
+        const double mx = fmax(r8, fmax(g8, b8)), mn = fmin(r8, fmin(g8, b8));
+        sat = __dadd_rn(sat, mx > 0.0 ? __ddiv_rn(__dsub_rn(mx, mn), mx) : 0.0);
+      }
+    }
+    const float a = __double2float_rn(__ddiv_rn(sa, 16.0)), b = __double2float_rn(__ddiv_rn(sb, 16.0));
+    int best = 0;
+    float bd = 0.f;
+    for (int k = 0; k < 313; ++k) {
+      const float da = __fsub_rn(a, bins[k].x), db = __fsub_rn(b, bins[k].y);
+      const float d = __fadd_rn(__fmul_rn(da, da), __fmul_rn(db, db));
+      if (k == 0 || d < bd) { bd = d; best = k; }
+    }
+    atomicAdd(&count[best], 1);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) sat = __dadd_rn(sat, __shfl_xor_sync(0xffffffffu, sat, o));
+  if ((threadIdx.x & 31) == 0) s_warp[threadIdx.x >> 5] = sat;
+  __syncthreads();
+  float* o = out + (size_t)blockIdx.x * 316;
+  for (int k = threadIdx.x; k < 313; k += kStatsThreads)
+    o[k] = __double2float_rn(__ddiv_rn((double)count[k], (double)cells));
+  if (threadIdx.x == 0) {
+    double t = s_warp[0];
+    for (int i = 1; i < kStatsThreads / 32; ++i) t = __dadd_rn(t, s_warp[i]);
+    o[313] = 1.f;
+    o[314] = __double2float_rn(__ddiv_rn(t, (double)h * w));
+    o[315] = 1.f;
+  }
+}
+
 static PhotoTable make_table(int n, const idc_photo* table) {
   PhotoTable t{};
   for (int i = 0; i < n; ++i) t.p[i] = table[i];
@@ -164,6 +231,12 @@ cudaError_t launch_hint_fill_mean(int n_blocks, int levels, int X, const double*
   if (cap == 0) return cudaSuccess;                      // blocks without room for a hint: nothing to fill
   const dim3 grid((unsigned)((cap + kFillThreads - 1) / kFillThreads), (unsigned)n_blocks);
   hint_fill_mean_kernel<<<grid, kFillThreads, 0, st>>>(levels, X, lab, blocks, stride, cap);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_global_stats_batch(int n, int h, int w, const uint8_t* rgb, const float* pts, float* out,
+                                      cudaStream_t st) {
+  global_stats_batch_kernel<<<(unsigned)n, kStatsThreads, 0, st>>>(h, w, rgb, pts, out);
   return cudaGetLastError();
 }
 

@@ -19,6 +19,13 @@ truth (`reveal_points`), all levels of a photo in the same device pass:
 
     H2D -> idc_photo_prep -> idc_rgb2lab_f64 (ground truth) -> idc_hint_fill_mean -> idc_hint_raster per image
     -> L and img_rgb repeated once per level -> idc_forward -> idc_rgb_sse -> D2H of the network-size results
+
+`PhotoColorizer.global_stats` gives each photo's global-hints statistics (313-bin ab histogram and mean saturation of
+the network-size photo, global_stats.prototxt), and `PhotoColorizer.global_sweep` measures PSNR under the global-hints
+conditions of GLOBAL_CONDITIONS, every condition of a photo in the same device pass:
+
+    H2D -> idc_photo_prep -> idc_global_stats_batch -> glob rows per condition (exact 0/1 masks) -> L and img_rgb
+    repeated once per condition -> zero ab / mask planes (idc_hint_raster) -> idc_forward -> idc_rgb_sse -> D2H
 """
 import collections
 import concurrent.futures
@@ -44,8 +51,23 @@ RevealResult.__doc__ = """One photo of a reveal sweep, over the L levels in the 
     rgb     uint8 [L,X,X,3]      output_rgb of each level
     points  int32 [max(levels),3] the revealed points (y0, x0, P) (reveal_points); level m used the first m"""
 
+GlobalSweepResult = collections.namedtuple("GlobalSweepResult", "psnr ab rgb stats")
+GlobalSweepResult.__doc__ = """One photo of a global-hints sweep, over the C conditions in the order given.
+    psnr    float64 [C]          get_result_PSNR() of each condition's output_rgb against the network-size photo
+    ab      float32 [C,2,X,X]    output_ab_raw of each condition
+    rgb     uint8 [C,X,X,3]      output_rgb of each condition
+    stats   float32 [316]        the photo's own statistics [313 histogram, 1, s_avg, 1] (idc_global_stats_batch)"""
+
 XFULLRES_MAX = 10000          # the wrapper's Xfullres_max (ColorizeImageBase): larger photos are resized on the host
 REVEAL_LEVELS = (0, 1, 2, 5, 10, 20, 50, 100, 200, 500)
+# The paper's global-hints evaluation: no hints, the photo's own saturation, its own histogram, both.
+GLOBAL_CONDITIONS = ("none", "sat", "hist", "hist+sat")
+# Which entries of a [316] statistics row each condition keeps (the others are 0): the histogram with its indicator
+# (313), the saturation (314) with its indicator (315).
+_GLOB_KEEP = {"none": np.zeros(316, bool),
+              "sat": np.r_[np.zeros(314, bool), True, True],
+              "hist": np.r_[np.ones(314, bool), False, False],
+              "hist+sat": np.ones(316, bool)}
 
 
 def reveal_points(X, m, seed, index):
@@ -91,6 +113,44 @@ def check_levels(levels, batch):
     if len(levels) > batch:
         raise ValueError("%d levels do not fit one device pass of batch = %d" % (len(levels), batch))
     return levels
+
+
+def glob_vector(stats, condition):
+    """A [316] statistics row [313 histogram, 1, s_avg, 1] -> the float32 glob vector of one condition of
+    GLOBAL_CONDITIONS; every entry is copied or set to 0, so each vector is exact:
+        none      all zeros (the reference's "run without this", data/colorize_image.py:454-456)
+        sat       [0] * 313, 0, s_avg, 1
+        hist      hist, 1, 0, 0   (what ColorizeImageB200GlobDist.net_forward(ab, mask, glob_dist=hist) feeds the engine)
+        hist+sat  the row as it is
+    colorize(photos, glob=[glob_vector(ref_stats, "hist")] * n) colours every photo like the reference photo whose
+    statistics ref_stats are (DemoGlobalHistogramTransfer.ipynb)."""
+    stats = np.asarray(stats, np.float32).reshape(-1)
+    if stats.shape != (316,):
+        raise ValueError("a statistics row has 316 values, got %d" % stats.size)
+    if condition not in _GLOB_KEEP:
+        raise ValueError("unknown global-hints condition %r, expected one of %s" % (condition, GLOBAL_CONDITIONS))
+    return np.where(_GLOB_KEEP[condition], stats, np.float32(0))
+
+
+def check_conditions(conditions, batch):
+    """conditions of a global-hints sweep -> tuple of names.  Raise ValueError unless they are distinct names of
+    GLOBAL_CONDITIONS, at least one and at most `batch` of them (one device pass carries every condition of a photo)."""
+    if isinstance(conditions, str):
+        raise ValueError("conditions: need a sequence of names, got the string %r" % conditions)
+    try:
+        conditions = tuple(conditions)
+    except TypeError:
+        raise ValueError("conditions: need a sequence of names, got %r" % (conditions,))
+    if not conditions:
+        raise ValueError("conditions: need at least one condition")
+    for c in conditions:
+        if not isinstance(c, str) or c not in GLOBAL_CONDITIONS:
+            raise ValueError("conditions: %r is not one of %s" % (c, GLOBAL_CONDITIONS))
+    if len(set(conditions)) != len(conditions):
+        raise ValueError("conditions: %s repeats a condition" % (conditions,))
+    if len(conditions) > batch:
+        raise ValueError("%d conditions do not fit one device pass of batch = %d" % (len(conditions), batch))
+    return conditions
 
 
 def read_photo(path):
@@ -157,16 +217,27 @@ class PhotoColorizer(object):
     readahead   photos decoded ahead of the device (default 2 * batch); workers: decoding threads
     calibrate   None, or what sets the storage exponents of the wgmma engine's activations from measured ranges instead
                 of the weights: a list of colour photos to measure on now, a {buffer: max_abs} dict, or the path of a
-                JSON file of one (engine.save_act_ranges); the ranges used are kept in `act_ranges`"""
+                JSON file of one (engine.save_act_ranges); the ranges used are kept in `act_ranges`
+    caffe       the weights are a Caffe-scaled checkpoint (conv1_1 trained on raw L-50, ab and mask x 110, regression
+                head tanh x 100), loaded as ColorizeImageB200Caffe.prep_net loads them (colorize_image.
+                caffe_scaled_state_dict, option tanh_scale = 100); a hint's mask of 1 is then the reference's mask x 110.
+                Not with maskcent."""
 
     def __init__(self, state_dict, Xd=256, batch=32, device=0, maskcent=False, global_hints=False, engine="wgmma",
-                 max_batch_bytes=96 << 20, readahead=None, workers=4, calibrate=None):
+                 max_batch_bytes=96 << 20, readahead=None, workers=4, calibrate=None, caffe=False):
         if Xd < 8 or Xd % 8:
             raise ValueError("Xd must be a multiple of 8, got %d" % Xd)
         if not 1 <= batch <= _lib.MAX_PHOTOS:
             raise ValueError("batch must be in [1, %d], got %d" % (_lib.MAX_PHOTOS, batch))
+        if caffe and maskcent:
+            raise ValueError("caffe=True takes no maskcent: the Caffe models do not centre the mask")
         self.Xd, self.batch, self.device = int(Xd), int(batch), int(device)
         self.maskcent, self.global_hints, self.engine = bool(maskcent), bool(global_hints), engine
+        self.caffe = bool(caffe)
+        self.options = {"tanh_scale": 100} if self.caffe else None
+        if self.caffe:
+            from .colorize_image import caffe_scaled_state_dict
+            state_dict = caffe_scaled_state_dict(state_dict)
         self.max_batch_bytes = int(max_batch_bytes)
         self.readahead = int(readahead) if readahead else 2 * self.batch
         self.workers = int(workers)
@@ -177,11 +248,11 @@ class PhotoColorizer(object):
         X, dev, glob = self.Xd, self.device, self.global_hints
         return engine.resolve_calibration(calibrate, lambda photos: engine.measure_act_ranges(
             state_dict, engine.calibration_batch(photos, X, device=dev, global_hints=glob), X, X, device=dev,
-            maskcent=0.5 if self.maskcent else 0.0, global_hints=glob))
+            maskcent=0.5 if self.maskcent else 0.0, global_hints=glob, options=self.options))
 
     def _make_backend(self, state_dict):
         return _DeviceBatches(state_dict, self.Xd, self.batch, self.device, 0.5 if self.maskcent else 0.0,
-                              self.global_hints, self.engine, self.max_batch_bytes, self.act_ranges)
+                              self.global_hints, self.engine, self.max_batch_bytes, self.act_ranges, self.options)
 
     def colorize(self, photos, hints=None, glob=None, psnr=False):
         """photos: a sequence of paths (read as load_image reads them) or HxWx3 uint8 RGB arrays.
@@ -230,6 +301,42 @@ class PhotoColorizer(object):
         return self._pipeline(cut_batches(items(), per, self.max_batch_bytes),
                               lambda b: self._backend.submit_reveal([a for _, a, _ in b], [p for _, _, p in b], levels),
                               self._backend.collect_reveal)
+
+    def global_stats(self, photos):
+        """The global-hints statistics of every photo: the float32 [316] row [313-bin ab histogram, 1, s_avg, 1] of the
+        network-size photo, the cv2-exact INTER_LINEAR resize to Xd x Xd that get_global_histogram does on the host
+        (idc_photo_prep, then idc_global_stats_batch; no forward).  photos: as colorize.  -> iterator of float32 [316],
+        in input order.  glob_vector(row, "hist") of a reference photo's row is the histogram-transfer vector."""
+        self._check_photos(photos)
+
+        def items():
+            for i, a in self._read(photos):
+                yield a.nbytes, 0, a
+
+        return self._pipeline(cut_batches(items(), self.batch, self.max_batch_bytes), self._backend.submit_stats,
+                              self._backend.collect_stats)
+
+    def global_sweep(self, photos, conditions=GLOBAL_CONDITIONS):
+        """PSNR under global hints taken from each photo itself: for every photo and every condition of
+        GLOBAL_CONDITIONS given, the network-size result with no local hints and glob_vector(stats, condition) as the
+        global-hints input, stats being the photo's own statistics (global_stats).  A device pass carries
+        batch // len(conditions) photos, each as len(conditions) consecutive forward images; nothing is rendered at full
+        resolution.  Needs global_hints=True.
+        photos: as colorize.  conditions: distinct names of GLOBAL_CONDITIONS, at most `batch` of them.
+        -> iterator of GlobalSweepResult, in input order.  Bad conditions or photos raise ValueError here, before any
+        device work (paths as in colorize)."""
+        if not self.global_hints:
+            raise ValueError("global_sweep needs PhotoColorizer(global_hints=True)")
+        conditions = check_conditions(conditions, self.batch)
+        self._check_photos(photos)
+
+        def items():
+            for i, a in self._read(photos):
+                yield a.nbytes, 0, a
+
+        per = self.batch // len(conditions)
+        return self._pipeline(cut_batches(items(), per, self.max_batch_bytes),
+                              lambda b: self._backend.submit_glob(b, conditions), self._backend.collect_glob)
 
     @staticmethod
     def _check_photos(photos):
@@ -323,11 +430,13 @@ class _DeviceBatches(object):
     the slot's next batch that fits, or close(), returns them to max_bytes (the page-locked host memory goes back to
     the system, the device memory to torch's caching allocator)."""
 
-    def __init__(self, state_dict, X, batch, device, maskcent, global_hints, engine_name, max_bytes, act_ranges=None):
+    def __init__(self, state_dict, X, batch, device, maskcent, global_hints, engine_name, max_bytes, act_ranges=None,
+                 options=None):
         import torch
         self.torch, self.lib = torch, _lib.load()
         self.X, self.batch, self.device, self.maskcent = X, batch, device, maskcent
-        self.ctx = engine.LhnContext(device=device, max_n=batch, H=X, W=X, engine=engine_name, global_hints=global_hints)
+        self.ctx = engine.LhnContext(device=device, max_n=batch, H=X, W=X, engine=engine_name, global_hints=global_hints,
+                                     options=options)
         self.ctx.load_state_dict(state_dict, act_ranges=act_ranges)
         dev = self.dev = torch.device("cuda:%d" % device)
         f32 = torch.float32
@@ -336,6 +445,10 @@ class _DeviceBatches(object):
         self.ab_in = torch.empty((batch, 2, X, X), dtype=f32, device=dev)
         self.mask = torch.empty((batch, 1, X, X), dtype=f32, device=dev)
         self.lab = torch.empty((batch, 3, X, X), dtype=torch.float64, device=dev)
+        from . import prepost
+        self.pts313 = torch.from_numpy(prepost.pts_in_hull()).to(dev)        # the 313 ab bin centres
+        self._keep = {}                                                       # conditions -> _glob_keep's masks
+        self.zero = torch.zeros((), dtype=f32, device=dev)
         self.max_bytes = max_bytes
         self.slots = [self._slot() for _ in range(2)]
         self.s_in, self.s_comp, self.s_out = (torch.cuda.Stream(dev) for _ in range(3))
@@ -361,6 +474,7 @@ class _DeviceBatches(object):
                 "ab": torch.empty((n, 2, X, X), dtype=torch.float32, device=dev), "h_ab": pin((n, 2, X, X), torch.float32),
                 "rgb": torch.empty((n, X, X, 3), dtype=torch.uint8, device=dev), "h_rgb": pin((n, X, X, 3), torch.uint8),
                 "sse": torch.empty((n,), dtype=torch.int64, device=dev), "h_sse": pin((n,), torch.int64),
+                "stats": torch.empty((n, 316), dtype=torch.float32, device=dev), "h_stats": pin((n, 316), torch.float32),
                 "ev_in": torch.cuda.Event(), "ev_comp": torch.cuda.Event(), "ev_out": torch.cuda.Event()}
 
     def _free_big(self, s):
@@ -480,13 +594,21 @@ class _DeviceBatches(object):
             out.append(PhotoResult(full[off * 3:(off + h * w) * 3].reshape(h, w, 3).copy(), rgb[i].copy(), ab[i].copy(), p))
         return out
 
-    def _reveal_buffers(self):
-        """Buffers of reveal sweeps, made on the first one: the prepared photos before they are repeated per level
-        (compute stream only, one copy) and, per slot, room for `batch` hint blocks of IDC_MAX_HINTS hints each."""
+    def _photo_buffers(self):
+        """The prepared photos of a sweep before they are repeated per level or condition (compute stream only, one
+        copy), made on the first sweep."""
         if getattr(self, "L_photo", None) is None:
             torch, X, n, dev = self.torch, self.X, self.batch, self.dev
             self.L_photo = torch.empty((n, 1, X, X), dtype=torch.float32, device=dev)
             self.rgb_photo = torch.empty((n, X, X, 3), dtype=torch.uint8, device=dev)
+            self._after_alloc()
+
+    def _reveal_buffers(self):
+        """Buffers of reveal sweeps, made on the first one: _photo_buffers and, per slot, room for `batch` hint blocks
+        of IDC_MAX_HINTS hints each."""
+        self._photo_buffers()
+        if "blocks" not in self.slots[0]:
+            torch, n, dev = self.torch, self.batch, self.dev
             nb = n * (_lib.HINT_HDR_BYTES + _lib.MAX_HINTS * _lib.HINT_DTYPE.itemsize)
             for s in self.slots:
                 s["blocks"] = torch.empty((nb,), dtype=torch.uint8, device=dev)
@@ -562,6 +684,107 @@ class _DeviceBatches(object):
             # the formula of collect(): get_result_PSNR with an exact sum of err2
             psnr = np.array([float(20 * np.log10(255. / np.sqrt(np.float64(e) / N))) for e in sse[k]], np.float64)
             out.append(RevealResult(psnr, ab[k].copy(), rgb[k].copy(), pts))
+        return out
+
+    def _upload_photos(self, s, nbytes, extra=()):
+        """H2D of the packed photos (and the (device, host) pairs of `extra`) on the copy stream; the compute stream
+        waits for it."""
+        with self.torch.cuda.stream(self.s_in):
+            s["src"][:nbytes].copy_(s["h_src"].tensor[:nbytes], non_blocking=True)
+            for d, h in extra:
+                d.copy_(h, non_blocking=True)
+            s["ev_in"].record(self.s_in)
+        self.s_comp.wait_event(s["ev_in"])
+
+    def submit_stats(self, photos):
+        """One device pass of global_stats: prep -> idc_global_stats_batch -> D2H of the [n,316] rows."""
+        torch, lib, X = self.torch, self.lib, self.X
+        n = len(photos)
+        s = self._next_slot()
+        table, nbytes = self._pack(s, photos)
+        self._upload_photos(s, nbytes)
+        st = self.s_comp
+        sh = st.cuda_stream
+        with torch.cuda.stream(st):
+            _lib.check(None, lib.idc_photo_prep(self.device, n, table.ctypes.data, s["src"].data_ptr(), X,
+                                                self.L_mc.data_ptr(), s["img_rgb"].data_ptr(), sh))
+            _lib.check(None, lib.idc_global_stats_batch(self.device, n, X, X, s["img_rgb"].data_ptr(),
+                                                        self.pts313.data_ptr(), s["stats"].data_ptr(), sh))
+            s["ev_comp"].record(st)
+        with torch.cuda.stream(self.s_out):
+            self.s_out.wait_event(s["ev_comp"])
+            s["h_stats"][:n].copy_(s["stats"][:n], non_blocking=True)
+            s["ev_out"].record(self.s_out)
+        return s, s["batch"], n
+
+    def collect_stats(self, token):
+        s, batch, n = token
+        if s["batch"] != batch:
+            raise RuntimeError("this batch's buffers were reused by a later batch: iterate one result iterator at a "
+                               "time per PhotoColorizer")
+        s["ev_out"].synchronize()
+        return [r.copy() for r in s["h_stats"].numpy()[:n]]
+
+    def _glob_keep(self, conditions):
+        """[C,316] bool device tensor: the entries of a statistics row each condition keeps (_GLOB_KEEP)."""
+        if conditions not in self._keep:
+            self._keep[conditions] = self.torch.from_numpy(np.stack([_GLOB_KEEP[c] for c in conditions])).to(self.dev)
+            self._after_alloc()
+        return self._keep[conditions]
+
+    def submit_glob(self, photos, conditions):
+        """One device pass of a global-hints sweep: photo i of the batch is forward images i*C .. i*C+C-1 (C =
+        len(conditions)), image i*C+j with glob_vector(stats_i, conditions[j]), no local hints."""
+        torch, lib, X = self.torch, self.lib, self.X
+        m, C = len(photos), len(conditions)
+        N = m * C
+        self._photo_buffers()
+        keep = self._glob_keep(conditions)
+        s = self._next_slot()
+        table, nbytes = self._pack(s, photos)
+        s["h_hints"].numpy()[:_lib.HINT_HDR_BYTES].view(np.int32)[:] = 0        # an empty hint block: zero planes
+        self._upload_photos(s, nbytes, [(s["hints"][:_lib.HINT_HDR_BYTES], s["h_hints"][:_lib.HINT_HDR_BYTES])])
+        st = self.s_comp
+        sh = st.cuda_stream
+        with torch.cuda.stream(st):
+            _lib.check(None, lib.idc_photo_prep(self.device, m, table.ctypes.data, s["src"].data_ptr(), X,
+                                                self.L_photo.data_ptr(), self.rgb_photo.data_ptr(), sh))
+            _lib.check(None, lib.idc_global_stats_batch(self.device, m, X, X, self.rgb_photo.data_ptr(),
+                                                        self.pts313.data_ptr(), s["stats"].data_ptr(), sh))
+            # glob rows: each entry of the photo's row copied or 0 (exact, as glob_vector)
+            torch.where(keep[None], s["stats"][:m, None], self.zero, out=s["glob"][:N].view(m, C, 316))
+            self.L_mc[:N].view(m, C, 1, X, X).copy_(self.L_photo[:m, None].expand(m, C, 1, X, X))
+            s["img_rgb"][:N].view(m, C, X, X, 3).copy_(self.rgb_photo[:m, None].expand(m, C, X, X, 3))
+            _lib.check(None, lib.idc_hint_raster(self.device, N, X, X, 0, s["hints"].data_ptr(), self.ab_in.data_ptr(),
+                                                 self.mask.data_ptr(), sh))
+            self.ctx.forward_device(self.L_mc[:N], self.ab_in[:N], self.mask[:N], self.maskcent, glob=s["glob"][:N],
+                                    want_rgb=True, out_ab=s["ab"][:N], out_rgb=s["rgb"][:N])
+            _lib.check(None, lib.idc_rgb_sse(self.device, N, X, X, s["img_rgb"].data_ptr(), s["rgb"].data_ptr(),
+                                             s["sse"].data_ptr(), sh))
+            s["ev_comp"].record(st)
+        with torch.cuda.stream(self.s_out):
+            self.s_out.wait_event(s["ev_comp"])
+            s["h_ab"][:N].copy_(s["ab"][:N], non_blocking=True)
+            s["h_rgb"][:N].copy_(s["rgb"][:N], non_blocking=True)
+            s["h_sse"][:N].copy_(s["sse"][:N], non_blocking=True)
+            s["h_stats"][:m].copy_(s["stats"][:m], non_blocking=True)
+            s["ev_out"].record(self.s_out)
+        return s, s["batch"], m, C
+
+    def collect_glob(self, token):
+        s, batch, m, C = token
+        if s["batch"] != batch:
+            raise RuntimeError("this batch's buffers were reused by a later batch: iterate one result iterator at a "
+                               "time per PhotoColorizer")
+        s["ev_out"].synchronize()
+        ab, rgb, sse, stats = s["h_ab"].numpy(), s["h_rgb"].numpy(), s["h_sse"].numpy(), s["h_stats"].numpy()
+        N = self.X * self.X * 3
+        out = []
+        for i in range(m):
+            k = slice(i * C, (i + 1) * C)
+            # the formula of collect(): get_result_PSNR with an exact sum of err2
+            psnr = np.array([float(20 * np.log10(255. / np.sqrt(np.float64(e) / N))) for e in sse[k]], np.float64)
+            out.append(GlobalSweepResult(psnr, ab[k].copy(), rgb[k].copy(), stats[i].copy()))
         return out
 
     def discard(self, token):

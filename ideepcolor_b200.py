@@ -15,8 +15,14 @@ Automatic colorization of a folder of photos, in batches on the device (photos.P
     python ideepcolor_b200.py --color_model caffemodel.pth --image_dir scans/ --out scans_color/ [--batch 32] [--psnr]
 
 writes <out>/<stem>.png per photo (the full-resolution result, get_img_fullres) and, with --psnr, <out>/psnr.csv
-(get_result_PSNR of each photo).  PSNR against the number of hint points revealed from each photo's own colours
-(photos.reveal_points), written to <out>/reveal_psnr.csv with no images:
+(get_result_PSNR of each photo).  With --hints_dir HDIR a photo <stem>.<ext> is coloured with the hints of HDIR/<stem>.json
+(the --hints format; no file = no hints), and --suggest K also writes <out>/<stem>_suggestions.json, in the format of
+the single-image suggestions.json, for every photo that has hints:
+
+    python ideepcolor_b200.py --color_model caffemodel.pth --image_dir scans/ --hints_dir scan_hints/ --out o/ --suggest 9
+
+PSNR against the number of hint points revealed from each photo's own colours (photos.reveal_points), written to
+<out>/reveal_psnr.csv with no images:
 
     python ideepcolor_b200.py --color_model caffemodel.pth --image_dir val/ --out sweep/ --reveal_sweep 0,1,2,5,10,20,50
         [--reveal_seed 0] [--batch 60]
@@ -55,6 +61,9 @@ def parse_args(argv=None):
     ap.add_argument("--image_dir", default="", help="colorize every photo of this folder automatically (needs --out)")
     ap.add_argument("--batch", type=int, default=32, help="photos per device pass (--image_dir)")
     ap.add_argument("--psnr", action="store_true", help="also write psnr.csv (--image_dir)")
+    ap.add_argument("--hints_dir", default="", metavar="HDIR",
+                    help="with --image_dir: colour photo <stem>.<ext> with the hints of HDIR/<stem>.json (the --hints "
+                         "format; a missing file means no hints); with --suggest K also write <out>/<stem>_suggestions.json")
     ap.add_argument("--calibrate", default="", metavar="DIR_OR_JSON",
                     help="set the activation storage exponents from measured ranges instead of the weights: a folder of "
                          "colour photos to measure on (a seeded sample of at most 16), or a JSON file saved earlier")
@@ -75,10 +84,18 @@ def parse_args(argv=None):
                          "(no images are written)")
     args = ap.parse_args(argv)
     given = {"global_hints": args.global_hints, "caffe": args.caffe, "glob_ref": bool(args.glob_ref),
-             "glob_sweep": args.glob_sweep is not None}
-    for flag in ("global_hints", "caffe", "glob_ref", "glob_sweep"):
+             "glob_sweep": args.glob_sweep is not None, "hints_dir": bool(args.hints_dir)}
+    for flag in ("global_hints", "caffe", "glob_ref", "glob_sweep", "hints_dir"):
         if given[flag] and not args.image_dir:
             ap.error("--%s needs --image_dir" % flag)
+    if args.hints_dir:
+        for flag, on in (("reveal_sweep", bool(args.reveal_sweep)), ("glob_sweep", given["glob_sweep"]),
+                         ("glob_ref", given["glob_ref"])):
+            if on:
+                ap.error("--hints_dir excludes --%s" % flag)
+        if args.suggest > 0 and (args.caffe or args.global_hints):
+            ap.error("--hints_dir with --suggest works with the 529-bin distribution head only, not with --%s"
+                     % ("caffe" if args.caffe else "global_hints"))
     if args.caffe and args.pytorch_maskcent:
         ap.error("--caffe and --pytorch_maskcent exclude each other: the Caffe models do not centre the mask")
     args.glob_conditions = None
@@ -150,6 +167,34 @@ def hint_ab(h):
     return [float(lab[0, 0, 1]), float(lab[0, 0, 2])]
 
 
+def hint_rects(hints, X):
+    """A --hints list -> the hint rectangles (colorize_image.HINT_LIST_DTYPE) the notebook's put_point calls paint."""
+    from interactive_deep_colorization_b200 import colorize_image as CI
+    return CI.hints_from_points([([int(h["loc"][0]), int(h["loc"][1])], int(h.get("size", 3)), hint_ab(h)) for h in hints], X)
+
+
+def write_suggestions(path, hints, centers, conf):
+    """suggestions.json: one entry per hint, {"loc": its loc, "ab": the K centres rounded to 3 places, "conf": their
+    mass rounded to 5} -- the one format of the single-image and the folder mode."""
+    out = [{"loc": h["loc"], "ab": np.round(c, 3).tolist(), "conf": np.round(f, 5).tolist()}
+           for h, c, f in zip(hints, centers, conf)]
+    with open(path, "w") as f:
+        json.dump(out, f, indent=1)
+
+
+def read_hints_dir(hdir, names):
+    """--hints_dir: the hint list of each photo name, from HDIR/<stem>.json; [] where there is no such file."""
+    out = []
+    for name in names:
+        p = os.path.join(hdir, os.path.splitext(name)[0] + ".json")
+        if os.path.isfile(p):
+            with open(p) as f:
+                out.append(json.load(f))
+        else:
+            out.append([])
+    return out
+
+
 IMAGE_EXTS = (".jpg", ".jpeg", ".png", ".bmp", ".tif", ".tiff", ".webp")
 
 
@@ -172,10 +217,14 @@ def colorize_dir(args):
     paths = [os.path.join(args.image_dir, f) for f in names]
     if not os.path.isdir(args.out):
         os.makedirs(args.out)
+    hints = read_hints_dir(args.hints_dir, names) if args.hints_dir else None
     sd = torch.load(args.color_model, map_location="cpu")
+    extra = {"suggest": True} if hints is not None and args.suggest > 0 else {}
     pc = PhotoColorizer(sd, Xd=args.load_size, batch=args.batch, device=args.gpu, maskcent=args.pytorch_maskcent,
-                        calibrate=args.calibrate_source, global_hints=args.global_hints, caffe=args.caffe)
+                        calibrate=args.calibrate_source, global_hints=args.global_hints, caffe=args.caffe, **extra)
     save_ranges(args, pc.act_ranges)
+    if hints is not None:
+        return hinted_dir(args, pc, names, paths, hints)
     if args.reveal_levels is not None:
         return reveal_dir(args, pc, names, paths)
     if args.glob_conditions is not None:
@@ -196,6 +245,35 @@ def colorize_dir(args):
         with open(os.path.join(args.out, "psnr.csv"), "w") as f:
             f.write("image,psnr\n" + "".join(row + "\n" for row in rows))
     print("colorized %d photos into <%s>" % (len(names), args.out))
+    return 0
+
+
+def hinted_dir(args, pc, names, paths, hints):
+    """--hints_dir: colorize(hints=...) over the folder -> OUT/<stem>.png (+ psnr.csv); with --suggest K,
+    PhotoColorizer.suggest at every hint's loc -> OUT/<stem>_suggestions.json for each photo that has hints."""
+    import cv2
+    X = args.load_size
+    rects = [hint_rects(h, X) for h in hints]
+    if args.suggest > 0:
+        locs = [np.array([[int(h["loc"][0]), int(h["loc"][1])] for h in hl], np.int64).reshape(-1, 2) for hl in hints]
+        results = pc.suggest(paths, rects, locs, K=args.suggest, psnr=args.psnr)
+    else:
+        results = pc.colorize(paths, hints=rects, psnr=args.psnr)
+    rows = []
+    for name, hl, r in zip(names, hints, results):
+        stem = os.path.splitext(name)[0]
+        if args.suggest > 0:
+            if hl:
+                write_suggestions(os.path.join(args.out, stem + "_suggestions.json"), hl, r.centers, r.conf)
+            r = r.result
+        cv2.imwrite(os.path.join(args.out, stem + ".png"), np.ascontiguousarray(r.fullres[:, :, ::-1]))
+        if args.psnr:
+            rows.append("%s,%.17g" % (name, r.psnr))
+    pc.close()
+    if args.psnr:
+        with open(os.path.join(args.out, "psnr.csv"), "w") as f:
+            f.write("image,psnr\n" + "".join(row + "\n" for row in rows))
+    print("colorized %d photos with the hints of <%s> into <%s>" % (len(names), args.hints_dir, args.out))
     return 0
 
 
@@ -260,7 +338,7 @@ def main(argv=None):
 
     hints = json.load(open(args.hints)) if args.hints else []
     # the notebook's put_point calls as a rectangle list: the engine rasterises it on the device
-    rects = CI.hints_from_points([([int(h["loc"][0]), int(h["loc"][1])], int(h.get("size", 3)), hint_ab(h)) for h in hints], X)
+    rects = hint_rects(hints, X)
     result = color_model.net_forward_hints(rects)
     if isinstance(result, int):
         print("net_forward failed")
@@ -271,10 +349,8 @@ def main(argv=None):
     if args.suggest > 0 and hints:
         dist_model.set_image(color_model.img_rgb)
         dist_model.net_forward_hints(rects)             # answered from the colour model's forward above
-        suggestions = []
-        for h in hints:
-            centers, conf = dist_model.get_ab_reccs(int(h["loc"][0]), int(h["loc"][1]), K=args.suggest, return_conf=True)
-            suggestions.append({"loc": h["loc"], "ab": np.round(centers, 3).tolist(), "conf": np.round(conf, 5).tolist()})
+        suggestions = [dist_model.get_ab_reccs(int(h["loc"][0]), int(h["loc"][1]), K=args.suggest, return_conf=True)
+                       for h in hints]
 
     out = args.out or (os.path.splitext(os.path.abspath(args.image_file))[0] + "_b200")
     if not os.path.isdir(out):
@@ -290,7 +366,8 @@ def main(argv=None):
                       ("input.png", color_model.get_input_img()), ("input_ab.png", color_model.get_sup_img())):
         cv2.imwrite(os.path.join(out, name), np.ascontiguousarray(rgb[:, :, ::-1]))
     if suggestions is not None:
-        json.dump(suggestions, open(os.path.join(out, "suggestions.json"), "w"), indent=1)
+        write_suggestions(os.path.join(out, "suggestions.json"), hints, [c for c, _ in suggestions],
+                          [f for _, f in suggestions])
     return 0
 
 

@@ -212,6 +212,26 @@ int idc_ab_reccs(idc_ctx* ctx, int img, int y4, int x4, int K, int max_iter, int
 /* Same clustering for a caller-supplied pmf (host, 529 floats, need not be normalised); no ctx needed. */
 int idc_ab_reccs_pmf(int device, const float* pmf_host, int K, int max_iter, int n_init, const float* pts_host,
                      float* centers_host, float* conf_host, int* iters_out);
+/* idc_ab_reccs for many pixels of the images of the context's LAST forward (any forward entry point; resident mode is
+ * not needed), in one stream-ordered pass: queries_host [q][3] int32 (img, y4, x4) on the (h/4 x w/4) grid.  Each
+ * query's pmf is computed from the class logits by the per-pixel routine of the full-map softmax (bit-identical to
+ * dist[img, :, y4, x4]), all q x n_init restarts run in one launch, and the best restart of each query is picked on the
+ * device by idc_ab_reccs's rule.  Query i's answer equals idc_ab_reccs on the same forward bit for bit, whatever its
+ * position in the list, and repeated queries get the same answer.  Outputs (DEVICE memory, float32 / int32):
+ * centers_dev [q][K][2], conf_dev [q][K] (may be NULL), iters_dev [q] (may be NULL), pmf_dev [q][529] (may be
+ * NULL: each query's pmf, the 529 floats of dist[img, :, y4, x4]).  pts_host: [529][2] HOST, or NULL
+ * for the PyTorch wrapper's grid.  Asynchronous on `stream` with no host synchronisation: the queries and the points
+ * travel as kernel parameters, so the host arrays may be reused as soon as the call returns.  Scratch (14.7 KB per
+ * query) belongs to the context and grows, stream-ordered, only when q exceeds every earlier q; calls on different
+ * streams must be ordered by the caller, as must the next forward (it overwrites the logits).  1 <= q <=
+ * IDC_MAX_RECCS_QUERIES (the k-means grid has one row per query).  IDC_ERR_STATE without IDC_FLAG_DIST or before any
+ * forward; IDC_ERR_ARG for q, K, max_iter, n_init out of range (as idc_ab_reccs), a NULL queries or centers, and a
+ * query whose img is outside [0, n) of the last forward or whose pixel is off the grid (idc_last_error names it), all
+ * before any device call. */
+#define IDC_MAX_RECCS_QUERIES 65535
+int idc_ab_reccs_batch(idc_ctx* ctx, int q, const int32_t* queries_host, int K, int max_iter, int n_init,
+                       const float* pts_host, float* centers_dev, float* conf_dev, int32_t* iters_dev, float* pmf_dev,
+                       void* stream);
 
 /* Caffe-spec 313-bin head (SURVEY row a14; models/reference_model/deploy_nopred.prototxt:651-850, weight
  * injection data/colorize_image.py:405-413).  With IDC_FLAG_CAFFE313 every forward also runs the
@@ -360,6 +380,11 @@ int idc_global_stats_batch(int device, int n, int h, int w, const uint8_t* rgb, 
                            void* stream);
 
 /* ---- introspection / test hooks (used by tests/, never by the product path) ---- */
+/* The host argument checks of idc_ab_reccs_batch, the same code, for a context with (has_head != 0) or without the
+ * 529-bin head whose last forward carried n_img images of h x w (n_img = 0: no forward yet) -> the code
+ * idc_ab_reccs_batch returns; msg (may be NULL) receives idc_last_error's text.  Touches no device. */
+int idc_ab_reccs_batch_check(int has_head, int n_img, int h, int w, int q, const int32_t* queries, int K, int max_iter,
+                             int n_init, char* msg, size_t msg_bytes);
 /* wgmma engine: the exponent S with which activation `name` is stored (FP16 hi/lo planes of value * 2^S), chosen per
  * buffer from the weights by idc_finalize_weights (DESIGN.md §3); 0 on the SIMT engine.  IDC_ERR_KEY for an unknown
  * name, IDC_ERR_STATE before the weights are packed. */

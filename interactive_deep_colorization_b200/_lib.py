@@ -29,6 +29,7 @@ MAX_HINTS = 1024                      # IDC_MAX_HINTS
 MAX_PHOTOS = 128                      # IDC_MAX_PHOTOS
 MAX_PHOTO_SIDE = 1 << 24               # IDC_MAX_PHOTO_SIDE
 MAX_PHOTO_X = 16384                   # IDC_MAX_PHOTO_X
+MAX_RECCS_QUERIES = 65535             # IDC_MAX_RECCS_QUERIES
 HINT_HDR_BYTES = 16                   # header {count, 0, 0, 0} of an idc_hint_raster block
 # idc_photo: a photo of a packed batch, its first pixel and its size
 PHOTO_DTYPE = np.dtype([("off", "<i8"), ("h", "<i4"), ("w", "<i4")])
@@ -63,6 +64,9 @@ SYMBOLS = [
     ("idc_set_click", _c.c_int, [_P, _c.c_int, _c.c_int, _c.c_int, _c.c_int]),
     ("idc_ab_reccs", _c.c_int, [_P, _c.c_int, _c.c_int, _c.c_int, _c.c_int, _c.c_int, _c.c_int, _P, _P, _P, _P]),
     ("idc_ab_reccs_pmf", _c.c_int, [_c.c_int, _P, _c.c_int, _c.c_int, _c.c_int, _P, _P, _P, _P]),
+    ("idc_ab_reccs_batch", _c.c_int, [_P, _c.c_int, _P, _c.c_int, _c.c_int, _c.c_int, _P, _P, _P, _P, _P, _P]),
+    ("idc_ab_reccs_batch_check", _c.c_int, [_c.c_int, _c.c_int, _c.c_int, _c.c_int, _c.c_int, _P, _c.c_int, _c.c_int,
+                                            _c.c_int, _P, _c.c_size_t]),
     ("idc_caffe313_pred_ab", _c.c_int, [_P, _c.c_int, _c.c_float, _P, _P]),
     ("idc_caffe313_dist_pixel", _c.c_int, [_P, _c.c_int, _c.c_int, _c.c_int, _c.c_float, _P]),
     ("idc_caffe313_dist_map", _c.c_int, [_P, _c.c_int, _c.c_float, _P, _P]),

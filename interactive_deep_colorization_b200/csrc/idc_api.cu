@@ -1360,21 +1360,16 @@ int idc_fetch_dist(idc_ctx* c, int img, int y4, int x4, float* out) {
 
 // shared by idc_ab_reccs / idc_ab_reccs_pmf.  scratch (doubles): [kReccsMaxInit][3*32+2] results, then the 529x2
 // gamut points as floats.
-constexpr int kReccsMaxInit = 16, kReccsRes = 3 * 32 + 2;
 constexpr size_t kReccsScratchBytes = (size_t)kReccsMaxInit * kReccsRes * sizeof(double) + 529 * 2 * sizeof(float);
 
 static bool reccs_args_ok(int K, int max_iter, int n_init) {
   return K >= 1 && K <= 32 && max_iter >= 1 && n_init >= 1 && n_init <= kReccsMaxInit;
 }
 
-// best restart = lowest inertia; restarts within 1e-9 (relative) of it count as ties -> lowest index
+// the restart reccs_best picks, as float32 outputs
 static void reccs_pick(const double* res, int K, int n_init, float* centers_host, float* conf_host, int* iters_out) {
   const int stride = 3 * K + 2;
-  double best = res[stride - 1];
-  for (int v = 1; v < n_init; ++v) best = std::min(best, res[v * stride + stride - 1]);
-  int pick = 0;
-  while (res[pick * stride + stride - 1] > best * (1.0 + 1e-9) + 1e-300) ++pick;
-  const double* r = res + (size_t)pick * stride;
+  const double* r = res + (size_t)reccs_best(res, K, n_init) * stride;
   for (int i = 0; i < 2 * K; ++i) centers_host[i] = (float)r[i];
   if (conf_host) for (int k = 0; k < K; ++k) conf_host[k] = (float)r[2 * K + k];
   if (iters_out) *iters_out = (int)r[3 * K];
@@ -1445,6 +1440,59 @@ int idc_ab_reccs_pmf(int device, const float* pmf_host, int K, int max_iter, int
     e = reccs_run(pmf_dev, 1, reinterpret_cast<double*>(buf.get()), K, max_iter, n_init, pts_host, centers_host, conf_host,
                   iters_out);
   return e == cudaSuccess ? IDC_OK : IDC_ERR_CUDA;
+}
+
+// The host checks of idc_ab_reccs_batch for a context with / without the 529-bin head whose last forward carried
+// n_img images of h x w; the message names the first bad query.
+static int reccs_batch_check(bool head, int n_img, int h, int w, int q, const int32_t* queries, int K, int max_iter,
+                             int n_init, char* msg, size_t cap) {
+  if (!head) return snprintf(msg, cap, "idc_ab_reccs_batch needs the 529-bin head (IDC_FLAG_DIST)"), IDC_ERR_STATE;
+  if (n_img < 1) return snprintf(msg, cap, "idc_ab_reccs_batch: no forward has run on this context"), IDC_ERR_STATE;
+  if (q < 1 || q > IDC_MAX_RECCS_QUERIES || !queries)
+    return snprintf(msg, cap, "idc_ab_reccs_batch: need 1 <= q <= %d queries, got %d", IDC_MAX_RECCS_QUERIES, q), IDC_ERR_ARG;
+  if (!reccs_args_ok(K, max_iter, n_init))
+    return snprintf(msg, cap, "idc_ab_reccs_batch: need 1 <= K <= 32, max_iter >= 1, 1 <= n_init <= %d", kReccsMaxInit),
+           IDC_ERR_ARG;
+  const int H4 = h / 4, W4 = w / 4;
+  for (int i = 0; i < q; ++i) {
+    const int32_t* t = queries + 3 * (size_t)i;
+    if (t[0] < 0 || t[0] >= n_img)
+      return snprintf(msg, cap, "idc_ab_reccs_batch: query %d: image %d outside the last forward's [0, %d)", i, t[0], n_img),
+             IDC_ERR_ARG;
+    if (t[1] < 0 || t[1] >= H4 || t[2] < 0 || t[2] >= W4)
+      return snprintf(msg, cap, "idc_ab_reccs_batch: query %d: pixel (%d,%d) outside the %dx%d grid", i, t[1], t[2], H4, W4),
+             IDC_ERR_ARG;
+  }
+  return IDC_OK;
+}
+
+int idc_ab_reccs_batch(idc_ctx* c, int q, const int32_t* queries_host, int K, int max_iter, int n_init,
+                       const float* pts_host, float* centers_dev, float* conf_dev, int32_t* iters_dev, float* pmf_dev,
+                       void* stream) {
+  if (!c) return IDC_ERR_ARG;
+  char msg[256];
+  const int rc = reccs_batch_check(c->dist, c->last_n, c->H, c->W, q, queries_host, K, max_iter, n_init, msg, sizeof(msg));
+  if (rc != IDC_OK) return fail(c, rc, "%s", msg);
+  if (!centers_dev) return fail(c, IDC_ERR_ARG, "idc_ab_reccs_batch: NULL centers");
+  const cudaStream_t st = (cudaStream_t)stream;
+  CUDA_TRY(c, cudaSetDevice(c->dev));
+  if (q > c->reccs_batch_q) {   // grow, stream-ordered: neither the release nor the allocation waits for the device
+    if (c->d_reccs_batch.get()) CUDA_TRY(c, cudaFreeAsync(c->d_reccs_batch.release(), st));
+    c->reccs_batch_q = 0;
+    CUDA_TRY(c, cudaMallocAsync(reinterpret_cast<void**>(c->d_reccs_batch.put()), reccs_batch_scratch_bytes(q), st));
+    c->reccs_batch_q = q;
+  }
+  CUDA_TRY(c, launch_reccs_batch(c, q, queries_host, pts_host, K, max_iter, n_init, c->d_reccs_batch.get(), centers_dev,
+                                 conf_dev, iters_dev, pmf_dev, st));
+  return IDC_OK;
+}
+
+int idc_ab_reccs_batch_check(int has_head, int n_img, int h, int w, int q, const int32_t* queries, int K, int max_iter,
+                             int n_init, char* msg, size_t msg_bytes) {
+  char buf[256];
+  const int rc = reccs_batch_check(has_head != 0, n_img, h, w, q, queries, K, max_iter, n_init, buf, sizeof(buf));
+  if (rc != IDC_OK && msg && msg_bytes) snprintf(msg, msg_bytes, "%s", buf);
+  return rc;
 }
 
 int idc_caffe313_pred_ab(idc_ctx* c, int n, float T, float* out_ab, void* stream) {

@@ -31,6 +31,7 @@ class Owner {
   H get() const { return h_; }
   H* put() { reset(); return &h_; }
   void reset() { if (h_) Release(h_); h_ = nullptr; }
+  H release() { H h = h_; h_ = nullptr; return h; }   // the caller frees it (e.g. stream-ordered, cudaFreeAsync)
  private:
   H h_ = nullptr;
 };
@@ -258,6 +259,8 @@ struct Ctx {
   bool gadd_active = false;     // a global-hints vector was supplied to this forward
   int last_n = 0;
   DevMem<double> d_reccs;       // idc_ab_reccs scratch (results of every restart, then the 529x2 gamut points)
+  DevMem<char> d_reccs_batch;   // idc_ab_reccs_batch scratch: gamut points, [Q][529] pmfs, every restart of every query
+  int reccs_batch_q = 0;        // the query count it holds room for
   DevMem<float> d_negent;       // idc_dist_negentropy result, (H/4)*(W/4) floats
   DevMem<float> d_dist313;      // idc_caffe313_dist_pixel result, 320 floats
   bool dist_resident = false;   // keep the dist of the last forward_host on the device (idc_fetch_dist)
@@ -301,9 +304,23 @@ cudaError_t launch_decode313(Ctx* c, int n, float T, float* out_ab, cudaStream_t
 cudaError_t launch_dist313_pixel(Ctx* c, int img, int y, int x, float S, float* out313_dev, cudaStream_t st);
 cudaError_t launch_dist313_map(Ctx* c, int n, float S, float* out_dev, cudaStream_t st);
 cudaError_t launch_negentropy(int n, int bins, int hw, const float* dist, float* out, cudaStream_t st);
+// n_query > 1: pmf holds n_query pmfs of 529 bins back to back (bin_stride 1) and out_dev n_query * n_init rows
 cudaError_t launch_ab_reccs(const float* pmf, size_t bin_stride, const float* pts_dev, int K, int max_iter,
-                            int n_init, double* out_dev, cudaStream_t st, const int* dyn = nullptr);
+                            int n_init, double* out_dev, cudaStream_t st, const int* dyn = nullptr, int n_query = 1);
 cudaError_t launch_click_pmf(Ctx* c, const int* click_dev, int n_img, int* out_hdr, float* out_pmf, cudaStream_t st);
+// idc_ab_reccs_batch on the device: queries [q][3] (img, y4, x4, HOST memory, checked by the caller), pts [529][2]
+// (HOST memory); scratch = kReccsBatchPtsBytes, then reccs_batch_pmf_bytes(q), then q * kReccsMaxInit * kReccsRes
+// doubles.  The pmfs go to pmf_out when given (else to the scratch).  Stream-ordered: the queries and points reach the
+// device as kernel parameters.
+constexpr int kReccsMaxInit = 16, kReccsRes = 3 * 32 + 2;   // restarts per query, doubles per restart (at K = 32)
+constexpr size_t kReccsBatchPtsBytes = 4352;                 // 529 x 2 floats, rounded up to 256 bytes
+inline size_t reccs_batch_pmf_bytes(int q) { return ((size_t)q * 529 * sizeof(float) + 255) / 256 * 256; }
+inline size_t reccs_batch_scratch_bytes(int q) {
+  return kReccsBatchPtsBytes + reccs_batch_pmf_bytes(q) + (size_t)q * kReccsMaxInit * kReccsRes * sizeof(double);
+}
+cudaError_t launch_reccs_batch(Ctx* c, int q, const int32_t* queries, const float* pts, int K, int max_iter, int n_init,
+                               char* scratch, float* centers, float* conf, int32_t* iters, float* pmf_out,
+                               cudaStream_t st);
 cudaError_t launch_global_stats(int h, int w, const uint8_t* rgb, const float* pts, float* out316, cudaStream_t st);
 cudaError_t launch_rgb2lab(int n, int h, int w, const uint8_t* rgb, double* lab, cudaStream_t st);
 cudaError_t launch_render_planes(const double* ab, int ab_order, int ab_f32, const double* mask, int mask_f32, int l_mode,
@@ -480,6 +497,29 @@ __device__ __forceinline__ double zoom_sample(const double* __restrict__ p, int 
   s = __dadd_rn(s, __dmul_rn(__dmul_rn(v01, ty.w0), tx.w1));
   s = __dadd_rn(s, __dmul_rn(__dmul_rn(v10, ty.w1), tx.w0));
   return __dadd_rn(s, __dmul_rn(__dmul_rn(v11, ty.w1), tx.w1));
+}
+
+// Colour suggestions: which of n_init k-means restarts wins.  res = n_init rows of 3K+2 doubles ([K][2] centres, [K]
+// mass, iterations, inertia).  Lowest inertia; restarts within 1e-9 (relative) of it count as ties -> lowest index.
+// The one definition of the rule, for the host pick of idc_ab_reccs and reccs_pick_kernel: on the device the threshold
+// is rounded step by step as on the host (no FMA), so both pick the same restart.  The walk stops at the last restart:
+// a negative inertia (negative weights, i.e. a caller's pmf with negative entries) puts the threshold below the
+// minimum, and an unbounded walk would read past the rows.
+__host__ __device__ __forceinline__ int reccs_best(const double* res, int K, int n_init) {
+  const int stride = 3 * K + 2;
+  double best = res[stride - 1];
+  for (int v = 1; v < n_init; ++v) {
+    const double e = res[v * stride + stride - 1];
+    if (e < best) best = e;
+  }
+#ifdef __CUDA_ARCH__
+  const double thr = __dadd_rn(__dmul_rn(best, 1.0 + 1e-9), 1e-300);
+#else
+  const double thr = best * (1.0 + 1e-9) + 1e-300;
+#endif
+  int pick = 0;
+  while (pick + 1 < n_init && res[pick * stride + stride - 1] > thr) ++pick;
+  return pick;
 }
 
 __device__ __forceinline__ void pdl_prologue_done() {   // small kernels: let the successor start, then wait for the predecessor

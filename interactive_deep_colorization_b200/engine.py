@@ -425,6 +425,32 @@ class LhnContext(object):
                                                  ctypes.byref(iters)))
         return centers, conf, iters.value
 
+    def ab_reccs_batch(self, queries, K=5, max_iter=100, n_init=8, pts=None, out=None, out_pmf=None):
+        """Colour suggestions at many pixels of the last forward's images in one device pass (idc_ab_reccs_batch):
+        queries int [Q,3] rows (img, y4, x4) -> (centres [Q,K,2] float32, mass [Q,K] float32, Lloyd iterations [Q]
+        int32) torch CUDA tensors, asynchronous on torch's current stream.  Query i equals ab_reccs(*queries[i], ...) on
+        the same forward bit for bit.  Needs dist=True; the forward may be any forward call.  out: optional
+        (centres, mass, iterations) tensors of those shapes and dtypes to write into (mass / iterations may be None).
+        out_pmf: optional float32 CUDA tensor [Q,529] that receives each query's pmf (dist[img, :, y4, x4])."""
+        import torch
+        q = np.ascontiguousarray(queries, np.int32).reshape(-1, 3)
+        p = None if pts is None else np.ascontiguousarray(pts, np.float32)
+        if p is not None and p.shape != (529, 2):
+            raise ValueError("pts: need [529, 2] ab coordinates, got %s" % (p.shape,))
+        dev = torch.device("cuda:%d" % self.device)
+        if out is None:
+            n, k = q.shape[0], max(int(K), 0)
+            out = (torch.empty((n, k, 2), dtype=torch.float32, device=dev), torch.empty((n, k), dtype=torch.float32, device=dev),
+                   torch.empty((n,), dtype=torch.int32, device=dev))
+        centers, conf, iters = out
+        st = torch.cuda.current_stream(dev).cuda_stream
+        _lib.check(self.h, self.lib.idc_ab_reccs_batch(self.h, int(q.shape[0]), _np_ptr(q), int(K), int(max_iter),
+                                                       int(n_init), None if p is None else _np_ptr(p), centers.data_ptr(),
+                                                       None if conf is None else conf.data_ptr(),
+                                                       None if iters is None else iters.data_ptr(),
+                                                       None if out_pmf is None else out_pmf.data_ptr(), st))
+        return centers, conf, iters
+
     # ---- Caffe-spec 313-bin head (IDC_FLAG_CAFFE313) ----------------------------------------
     def caffe313_pred_ab(self, n, T=2.6):
         """Annealed-mean ab [n,2,H,W] (device tensor) from the 313-bin logits of the last forward."""

@@ -26,6 +26,11 @@ conditions of GLOBAL_CONDITIONS, every condition of a photo in the same device p
 
     H2D -> idc_photo_prep -> idc_global_stats_batch -> glob rows per condition (exact 0/1 masks) -> L and img_rgb
     repeated once per condition -> zero ab / mask planes (idc_hint_raster) -> idc_forward -> idc_rgb_sse -> D2H
+
+`PhotoColorizer.suggest` (a colorizer made with suggest=True, whose context carries the 529-bin distribution head)
+colours every photo with its hints as `colorize(hints=...)` does and also answers the GUI palette's question, the K
+colour suggestions get_ab_reccs(h, w, K) gives, at each photo's query points, on the distribution of that photo's own
+forward: the colorize pass with idc_ab_reccs_batch right after idc_forward (every query of the batch in one pass).
 """
 import collections
 import concurrent.futures
@@ -50,6 +55,12 @@ RevealResult.__doc__ = """One photo of a reveal sweep, over the L levels in the 
     ab      float32 [L,2,X,X]    output_ab_raw of each level
     rgb     uint8 [L,X,X,3]      output_rgb of each level
     points  int32 [max(levels),3] the revealed points (y0, x0, P) (reveal_points); level m used the first m"""
+
+SuggestResult = collections.namedtuple("SuggestResult", "result centers conf")
+SuggestResult.__doc__ = """One photo of PhotoColorizer.suggest, with P query points.
+    result   PhotoResult   what colorize(hints=...) gives for the photo
+    centers  float64 [P,K,2]  get_ab_reccs(h, w, K) at each point (ab centres, heaviest cluster first)
+    conf     float64 [P,K]    the clusters' mass (get_ab_reccs(..., return_conf=True))"""
 
 GlobalSweepResult = collections.namedtuple("GlobalSweepResult", "psnr ab rgb stats")
 GlobalSweepResult.__doc__ = """One photo of a global-hints sweep, over the C conditions in the order given.
@@ -221,19 +232,25 @@ class PhotoColorizer(object):
     caffe       the weights are a Caffe-scaled checkpoint (conv1_1 trained on raw L-50, ab and mask x 110, regression
                 head tanh x 100), loaded as ColorizeImageB200Caffe.prep_net loads them (colorize_image.
                 caffe_scaled_state_dict, option tanh_scale = 100); a hint's mask of 1 is then the reference's mask x 110.
-                Not with maskcent."""
+                Not with maskcent.
+    suggest     the context also carries the 529-bin distribution head, for `suggest` (the head runs beside the colour
+                result and leaves it as it is).  Not with caffe or global_hints: their distribution models (313 bins,
+                global hints) have no batched suggestions."""
 
     def __init__(self, state_dict, Xd=256, batch=32, device=0, maskcent=False, global_hints=False, engine="wgmma",
-                 max_batch_bytes=96 << 20, readahead=None, workers=4, calibrate=None, caffe=False):
+                 max_batch_bytes=96 << 20, readahead=None, workers=4, calibrate=None, caffe=False, suggest=False):
         if Xd < 8 or Xd % 8:
             raise ValueError("Xd must be a multiple of 8, got %d" % Xd)
         if not 1 <= batch <= _lib.MAX_PHOTOS:
             raise ValueError("batch must be in [1, %d], got %d" % (_lib.MAX_PHOTOS, batch))
         if caffe and maskcent:
             raise ValueError("caffe=True takes no maskcent: the Caffe models do not centre the mask")
+        if suggest and (caffe or global_hints):
+            raise ValueError("suggest=True works with the 529-bin distribution head only, not with %s"
+                             % ("caffe=True" if caffe else "global_hints=True"))
         self.Xd, self.batch, self.device = int(Xd), int(batch), int(device)
         self.maskcent, self.global_hints, self.engine = bool(maskcent), bool(global_hints), engine
-        self.caffe = bool(caffe)
+        self.caffe, self.dist = bool(caffe), bool(suggest)
         self.options = {"tanh_scale": 100} if self.caffe else None
         if self.caffe:
             from .colorize_image import caffe_scaled_state_dict
@@ -252,7 +269,8 @@ class PhotoColorizer(object):
 
     def _make_backend(self, state_dict):
         return _DeviceBatches(state_dict, self.Xd, self.batch, self.device, 0.5 if self.maskcent else 0.0,
-                              self.global_hints, self.engine, self.max_batch_bytes, self.act_ranges, self.options)
+                              self.global_hints, self.engine, self.max_batch_bytes, self.act_ranges, self.options,
+                              self.dist)
 
     def colorize(self, photos, hints=None, glob=None, psnr=False):
         """photos: a sequence of paths (read as load_image reads them) or HxWx3 uint8 RGB arrays.
@@ -276,6 +294,41 @@ class PhotoColorizer(object):
             if any(g.shape != (316,) for g in glob):
                 raise ValueError("every glob vector must have 316 values")
         return self._run(photos, hints, glob, bool(psnr))
+
+    def suggest(self, photos, hints, points, K=9, psnr=False):
+        """Colour suggestions at query points, with the colour result: for every photo, colorize(hints=..., psnr=...)'s
+        PhotoResult and, at each of its points (h, w) (network coordinates, 0 <= h, w < Xd), the K suggestions
+        get_ab_reccs(h, w, K, return_conf=True) of the single-image distribution model gives after net_forward with
+        the photo's hints (8 restarts, 100 Lloyd iterations, the PyTorch wrapper's gamut grid), read from the
+        distribution of the forward that used those hints.  Needs suggest=True.
+        photos, hints: as colorize (hints may be None, or None per photo).  points: one int [P,2] array of (h, w) per
+        photo (P may be 0).  K in [1, 32].
+        -> iterator of SuggestResult, in input order.  Argument errors raise ValueError here, before any device work
+        (paths as in colorize)."""
+        if not self.dist:
+            raise ValueError("suggest needs PhotoColorizer(suggest=True)")
+        n = len(photos)
+        if isinstance(K, (bool, np.bool_)) or not isinstance(K, (int, np.integer)) or not 1 <= K <= 32:
+            raise ValueError("K must be an integer in [1, 32], got %r" % (K,))
+        if len(points) != n:
+            raise ValueError("%d point lists for %d photos" % (len(points), n))
+        points = [self._point_list(p, i) for i, p in enumerate(points)]
+        if hints is not None and len(hints) != n:
+            raise ValueError("%d hint lists for %d photos" % (len(hints), n))
+        self._check_photos(photos)
+        if hints is not None:
+            hints = [self._hint_list(h, i) for i, h in enumerate(hints)]
+        return self._run(photos, hints, None, bool(psnr), points, int(K))
+
+    def _point_list(self, p, i):
+        p = np.asarray(p)
+        if p.size == 0:
+            return np.zeros((0, 2), np.int64)
+        if p.ndim != 2 or p.shape[1] != 2 or not np.issubdtype(p.dtype, np.integer):
+            raise ValueError("photo %d: points must be an integer [P,2] array of (h, w), got %s %s" % (i, p.dtype, p.shape))
+        if p.min() < 0 or p.max() >= self.Xd:
+            raise ValueError("photo %d: a point lies outside the %d x %d network grid" % (i, self.Xd, self.Xd))
+        return p.astype(np.int64)
 
     def reveal_sweep(self, photos, levels=REVEAL_LEVELS, seed=0):
         """PSNR against the number of revealed hint points: for every photo and every level m, the network-size result
@@ -364,7 +417,7 @@ class PhotoColorizer(object):
             return i, check_photo(read_photo(p), "photo %d (%s)" % (i, p))
         return read_ahead(range(len(photos)), load, self.readahead, self.workers)
 
-    def _run(self, photos, hints, glob, psnr):
+    def _run(self, photos, hints, glob, psnr, points=None, K=0):
         def items():
             for i, a in self._read(photos):
                 nh = 0 if hints is None or hints[i] is None else hints[i].shape[0]
@@ -372,8 +425,11 @@ class PhotoColorizer(object):
 
         def submit(b):
             idx = [i for i, _ in b]
-            return self._backend.submit([a for _, a in b], None if hints is None else [hints[i] for i in idx],
-                                        None if glob is None else [glob[i] for i in idx], psnr)
+            args = ([a for _, a in b], None if hints is None else [hints[i] for i in idx],
+                    None if glob is None else [glob[i] for i in idx], psnr)
+            if points is None:
+                return self._backend.submit(*args)
+            return self._backend.submit(*args, points=[points[i] for i in idx], K=K)
 
         return self._pipeline(cut_batches(items(), self.batch, self.max_batch_bytes), submit, self._backend.collect)
 
@@ -431,12 +487,12 @@ class _DeviceBatches(object):
     the system, the device memory to torch's caching allocator)."""
 
     def __init__(self, state_dict, X, batch, device, maskcent, global_hints, engine_name, max_bytes, act_ranges=None,
-                 options=None):
+                 options=None, dist=False):
         import torch
         self.torch, self.lib = torch, _lib.load()
         self.X, self.batch, self.device, self.maskcent = X, batch, device, maskcent
         self.ctx = engine.LhnContext(device=device, max_n=batch, H=X, W=X, engine=engine_name, global_hints=global_hints,
-                                     options=options)
+                                     options=options, dist=dist)
         self.ctx.load_state_dict(state_dict, act_ranges=act_ranges)
         dev = self.dev = torch.device("cuda:%d" % device)
         f32 = torch.float32
@@ -518,11 +574,29 @@ class _DeviceBatches(object):
             h_src[o:o + a.nbytes] = a.reshape(-1)
         return table, nbytes
 
-    def submit(self, photos, hints, glob, psnr):
+    def _reccs_buffers(self, s, size):
+        """Slot s's suggestion outputs, room for `size` centres (queries x K): device and page-locked host.  The slot is
+        idle (submit waited for it)."""
+        if s.get("rc_cap", 0) < size:
+            torch, dev = self.torch, self.dev
+            s["cen"] = torch.empty((size, 2), dtype=torch.float32, device=dev)
+            s["conf"] = torch.empty((size,), dtype=torch.float32, device=dev)
+            s["h_cen"] = torch.empty((size, 2), dtype=torch.float32, pin_memory=True)
+            s["h_conf"] = torch.empty((size,), dtype=torch.float32, pin_memory=True)
+            s["rc_cap"] = size
+            self._after_alloc()
+
+    def submit(self, photos, hints, glob, psnr, points=None, K=0):
         torch, lib, X = self.torch, self.lib, self.X
         n = len(photos)
         s = self._next_slot()
         table, nbytes = self._pack(s, photos)
+        queries = None
+        if points is not None:   # one query (photo of the batch, y4, x4) per point, photo by photo
+            queries = np.concatenate([np.zeros((0, 3), np.int32)] + [
+                np.column_stack([np.full(len(p), i), p // 4]).astype(np.int32) for i, p in enumerate(points)])
+            if len(queries):
+                self._reccs_buffers(s, len(queries) * K)
         count = 0
         if hints is not None:
             lists = []
@@ -560,6 +634,12 @@ class _DeviceBatches(object):
             self.ctx.forward_device(self.L_mc[:n], self.ab_in[:n], self.mask[:n], self.maskcent,
                                     glob=None if glob is None else s["glob"][:n], want_rgb=True,
                                     out_ab=s["ab"][:n], out_rgb=s["rgb"][:n])
+            if queries is not None:        # on this forward's class logits, before the next forward replaces them
+                Q, M = len(queries), _lib.MAX_RECCS_QUERIES
+                for q0 in range(0, Q, M):
+                    q1 = min(q0 + M, Q)
+                    self.ctx.ab_reccs_batch(queries[q0:q1], K, out=(s["cen"][q0 * K:q1 * K].view(q1 - q0, K, 2),
+                                                                    s["conf"][q0 * K:q1 * K].view(q1 - q0, K), None))
             _lib.check(None, lib.idc_rgb2lab_f64(self.device, n, X, X, s["rgb"].data_ptr(), self.lab.data_ptr(), sh))
             _lib.check(None, lib.idc_photo_render(self.device, n, tp, s["src"].data_ptr(), X, self.lab.data_ptr(),
                                                   s["src"].data_ptr(), sh))
@@ -575,11 +655,14 @@ class _DeviceBatches(object):
             s["h_rgb"][:n].copy_(s["rgb"][:n], non_blocking=True)
             if psnr:
                 s["h_sse"][:n].copy_(s["sse"][:n], non_blocking=True)
+            if queries is not None and len(queries):
+                s["h_cen"][:len(queries) * K].copy_(s["cen"][:len(queries) * K], non_blocking=True)
+                s["h_conf"][:len(queries) * K].copy_(s["conf"][:len(queries) * K], non_blocking=True)
             s["ev_out"].record(self.s_out)
-        return s, s["batch"], table, psnr
+        return s, s["batch"], table, psnr, None if points is None else [len(p) for p in points], K
 
     def collect(self, token):
-        s, batch, table, psnr = token
+        s, batch, table, psnr, counts, K = token
         if s["batch"] != batch:
             raise RuntimeError("this batch's buffers were reused by a later batch: iterate one colorize() result at a "
                                "time per PhotoColorizer")
@@ -592,7 +675,15 @@ class _DeviceBatches(object):
             if psnr:    # get_result_PSNR: 20 * log10(255 / sqrt(mean(err2))); the sum of err2 is exact, so is the mean
                 p = float(20 * np.log10(255. / np.sqrt(np.float64(sse[i]) / N)))
             out.append(PhotoResult(full[off * 3:(off + h * w) * 3].reshape(h, w, 3).copy(), rgb[i].copy(), ab[i].copy(), p))
-        return out
+        if counts is None:
+            return out
+        Q = sum(counts)
+        cen = s["h_cen"].numpy()[:Q * K].reshape(Q, K, 2) if Q else np.zeros((0, K, 2), np.float32)
+        conf = s["h_conf"].numpy()[:Q * K].reshape(Q, K) if Q else np.zeros((0, K), np.float32)
+        ends = np.cumsum(counts)
+        # float64 like get_ab_reccs (centers.astype(np.float64), conf.astype(np.float64))
+        return [SuggestResult(r, cen[e - c:e].astype(np.float64), conf[e - c:e].astype(np.float64))
+                for r, c, e in zip(out, counts, ends)]
 
     def _photo_buffers(self):
         """The prepared photos of a sweep before they are repeated per level or condition (compute stream only, one

@@ -200,7 +200,6 @@ IMAGE_EXTS = (".jpg", ".jpeg", ".png", ".bmp", ".tif", ".tiff", ".webp")
 
 def colorize_dir(args):
     """--image_dir: every photo of the folder (sorted by name) through PhotoColorizer -> OUT/<stem>.png (+ psnr.csv)."""
-    import cv2
     import torch
     from interactive_deep_colorization_b200.photos import PhotoColorizer
     if not args.out:
@@ -234,8 +233,17 @@ def colorize_dir(args):
         from interactive_deep_colorization_b200 import photos
         ref = next(iter(pc.global_stats([args.glob_ref])))
         glob = [photos.glob_vector(ref, "hist")] * len(paths)
+    write_photos(args, pc, names, pc.colorize(paths, glob=glob, psnr=args.psnr))
+    print("colorized %d photos into <%s>" % (len(names), args.out))
+    return 0
+
+
+def write_photos(args, pc, names, results):
+    """OUT/<stem>.png of each photo's PhotoResult (its full-resolution result) and, with --psnr, OUT/psnr.csv; then
+    closes pc."""
+    import cv2
     rows = []
-    for name, r in zip(names, pc.colorize(paths, glob=glob, psnr=args.psnr)):
+    for name, r in zip(names, results):
         stem = os.path.splitext(name)[0]
         cv2.imwrite(os.path.join(args.out, stem + ".png"), np.ascontiguousarray(r.fullres[:, :, ::-1]))
         if args.psnr:
@@ -244,75 +252,64 @@ def colorize_dir(args):
     if args.psnr:
         with open(os.path.join(args.out, "psnr.csv"), "w") as f:
             f.write("image,psnr\n" + "".join(row + "\n" for row in rows))
-    print("colorized %d photos into <%s>" % (len(names), args.out))
-    return 0
 
 
 def hinted_dir(args, pc, names, paths, hints):
     """--hints_dir: colorize(hints=...) over the folder -> OUT/<stem>.png (+ psnr.csv); with --suggest K,
     PhotoColorizer.suggest at every hint's loc -> OUT/<stem>_suggestions.json for each photo that has hints."""
-    import cv2
     X = args.load_size
     rects = [hint_rects(h, X) for h in hints]
     if args.suggest > 0:
         locs = [np.array([[int(h["loc"][0]), int(h["loc"][1])] for h in hl], np.int64).reshape(-1, 2) for hl in hints]
-        results = pc.suggest(paths, rects, locs, K=args.suggest, psnr=args.psnr)
+        suggested = pc.suggest(paths, rects, locs, K=args.suggest, psnr=args.psnr)
+
+        def results():
+            for name, hl, r in zip(names, hints, suggested):
+                if hl:
+                    write_suggestions(os.path.join(args.out, os.path.splitext(name)[0] + "_suggestions.json"), hl,
+                                      r.centers, r.conf)
+                yield r.result
+        write_photos(args, pc, names, results())
     else:
-        results = pc.colorize(paths, hints=rects, psnr=args.psnr)
-    rows = []
-    for name, hl, r in zip(names, hints, results):
-        stem = os.path.splitext(name)[0]
-        if args.suggest > 0:
-            if hl:
-                write_suggestions(os.path.join(args.out, stem + "_suggestions.json"), hl, r.centers, r.conf)
-            r = r.result
-        cv2.imwrite(os.path.join(args.out, stem + ".png"), np.ascontiguousarray(r.fullres[:, :, ::-1]))
-        if args.psnr:
-            rows.append("%s,%.17g" % (name, r.psnr))
-    pc.close()
-    if args.psnr:
-        with open(os.path.join(args.out, "psnr.csv"), "w") as f:
-            f.write("image,psnr\n" + "".join(row + "\n" for row in rows))
+        write_photos(args, pc, names, pc.colorize(paths, hints=rects, psnr=args.psnr))
     print("colorized %d photos with the hints of <%s> into <%s>" % (len(names), args.hints_dir, args.out))
     return 0
 
 
-def reveal_dir(args, pc, names, paths):
-    """--reveal_sweep: PhotoColorizer.reveal_sweep over the folder -> OUT/reveal_psnr.csv (a row per photo, a column per
-    level, then the mean row), and the mean curve on stdout."""
-    levels = args.reveal_levels
+def write_sweep(args, pc, names, csv, labels, results, title, line):
+    """A sweep's PSNR, one result per photo -> OUT/<csv> (a row per photo, a column per label, then the mean row), and
+    `title` and the mean per label (`line` % (label, mean)) on stdout; closes pc."""
     rows, curves = [], []
-    for name, r in zip(names, pc.reveal_sweep(paths, levels=levels, seed=args.reveal_seed)):
+    for name, r in zip(names, results):
         rows.append([name] + ["%.17g" % v for v in r.psnr])
         curves.append(r.psnr)
     pc.close()
-    mean = np.mean(curves, axis=0) if curves else np.full(len(levels), np.nan)
+    mean = np.mean(curves, axis=0) if curves else np.full(len(labels), np.nan)
     rows.append(["mean"] + ["%.17g" % v for v in mean])
-    with open(os.path.join(args.out, "reveal_psnr.csv"), "w") as f:
-        f.write(",".join(["image"] + [str(m) for m in levels]) + "\n" + "".join(",".join(row) + "\n" for row in rows))
-    print("reveal sweep of %d photos (seed %d), mean PSNR per number of revealed points:" % (len(names), args.reveal_seed))
-    for m, v in zip(levels, mean):
-        print("  %4d  %.3f dB" % (m, v))
+    with open(os.path.join(args.out, csv), "w") as f:
+        f.write(",".join(["image"] + [str(c) for c in labels]) + "\n" + "".join(",".join(row) + "\n" for row in rows))
+    print(title)
+    for c, v in zip(labels, mean):
+        print(line % (c, v))
     return 0
+
+
+def reveal_dir(args, pc, names, paths):
+    """--reveal_sweep: PhotoColorizer.reveal_sweep over the folder -> OUT/reveal_psnr.csv, and the mean curve on
+    stdout."""
+    levels = args.reveal_levels
+    return write_sweep(args, pc, names, "reveal_psnr.csv", levels,
+                       pc.reveal_sweep(paths, levels=levels, seed=args.reveal_seed),
+                       "reveal sweep of %d photos (seed %d), mean PSNR per number of revealed points:"
+                       % (len(names), args.reveal_seed), "  %4d  %.3f dB")
 
 
 def glob_sweep_dir(args, pc, names, paths):
-    """--glob_sweep: PhotoColorizer.global_sweep over the folder -> OUT/glob_psnr.csv (a row per photo, a column per
-    condition, then the mean row), and the mean per condition on stdout."""
+    """--glob_sweep: PhotoColorizer.global_sweep over the folder -> OUT/glob_psnr.csv, and the mean per condition on
+    stdout."""
     conds = args.glob_conditions
-    rows, curves = [], []
-    for name, r in zip(names, pc.global_sweep(paths, conditions=conds)):
-        rows.append([name] + ["%.17g" % v for v in r.psnr])
-        curves.append(r.psnr)
-    pc.close()
-    mean = np.mean(curves, axis=0) if curves else np.full(len(conds), np.nan)
-    rows.append(["mean"] + ["%.17g" % v for v in mean])
-    with open(os.path.join(args.out, "glob_psnr.csv"), "w") as f:
-        f.write(",".join(["image"] + list(conds)) + "\n" + "".join(",".join(row) + "\n" for row in rows))
-    print("global-hints sweep of %d photos, mean PSNR per condition:" % len(names))
-    for c, v in zip(conds, mean):
-        print("  %-8s  %.3f dB" % (c, v))
-    return 0
+    return write_sweep(args, pc, names, "glob_psnr.csv", conds, pc.global_sweep(paths, conditions=conds),
+                       "global-hints sweep of %d photos, mean PSNR per condition:" % len(names), "  %-8s  %.3f dB")
 
 
 def main(argv=None):

@@ -24,8 +24,11 @@ truth (`reveal_points`), all levels of a photo in the same device pass:
 the network-size photo, global_stats.prototxt), and `PhotoColorizer.global_sweep` measures PSNR under the global-hints
 conditions of GLOBAL_CONDITIONS, every condition of a photo in the same device pass:
 
-    H2D -> idc_photo_prep -> idc_global_stats_batch -> glob rows per condition (exact 0/1 masks) -> L and img_rgb
-    repeated once per condition -> zero ab / mask planes (idc_hint_raster) -> idc_forward -> idc_rgb_sse -> D2H
+    H2D -> idc_photo_prep -> idc_global_stats_batch -> glob rows per condition (exact 0/1 masks) -> zero ab / mask
+    planes (idc_hint_raster) -> L and img_rgb repeated once per condition -> idc_forward -> idc_rgb_sse -> D2H
+
+The two sweeps are one pass from the repeat of L and img_rgb on; they differ only in how they make the forward's ab /
+mask planes and glob rows.
 
 `PhotoColorizer.suggest` (a colorizer made with suggest=True, whose context carries the 529-bin distribution head)
 colours every photo with its hints as `colorize(hints=...)` does and also answers the GUI palette's question, the K
@@ -81,6 +84,13 @@ _GLOB_KEEP = {"none": np.zeros(316, bool),
               "hist+sat": np.ones(316, bool)}
 
 
+def _psnr(sse, X):
+    """get_result_PSNR of an X x X result, 20 * log10(255 / sqrt(mean(err2))), from its exact sum of err2 (so the mean
+    is exact too).  numpy's scalar log10, one result at a time, as get_result_PSNR computes it: the array log10 need
+    not round the same way."""
+    return float(20 * np.log10(255. / np.sqrt(np.float64(sse) / (X * X * 3))))
+
+
 def reveal_points(X, m, seed, index):
     """The first m points a simulated user reveals on the X x X network grid of photo number `index` -> int32 [m, 3],
     one row (y0, x0, P) per point: a P x P square with top-left corner (y0, x0), painted with the photo's mean
@@ -113,17 +123,22 @@ def check_levels(levels, batch):
         levels = list(levels)
     except TypeError:
         raise ValueError("levels: need a sequence of integers, got %r" % (levels,))
-    if not levels:
-        raise ValueError("levels: need at least one level")
     for v in levels:
         if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, np.integer)) or not 0 <= v <= _lib.MAX_HINTS:
             raise ValueError("levels: %r is not an integer in [0, %d]" % (v, _lib.MAX_HINTS))
-    levels = tuple(int(v) for v in levels)
-    if len(set(levels)) != len(levels):
-        raise ValueError("levels: %s repeats a level" % (levels,))
-    if len(levels) > batch:
-        raise ValueError("%d levels do not fit one device pass of batch = %d" % (len(levels), batch))
-    return levels
+    return _check_one_pass(tuple(int(v) for v in levels), "level", batch)
+
+
+def _check_one_pass(values, noun, batch):
+    """The variants of a sweep (a tuple) -> themselves.  Raise ValueError unless there is at least one, none repeats and
+    at most `batch` of them fit one device pass.  noun: "level" or "condition", for the messages."""
+    if not values:
+        raise ValueError("%ss: need at least one %s" % (noun, noun))
+    if len(set(values)) != len(values):
+        raise ValueError("%ss: %s repeats a %s" % (noun, values, noun))
+    if len(values) > batch:
+        raise ValueError("%d %ss do not fit one device pass of batch = %d" % (len(values), noun, batch))
+    return values
 
 
 def glob_vector(stats, condition):
@@ -152,16 +167,10 @@ def check_conditions(conditions, batch):
         conditions = tuple(conditions)
     except TypeError:
         raise ValueError("conditions: need a sequence of names, got %r" % (conditions,))
-    if not conditions:
-        raise ValueError("conditions: need at least one condition")
     for c in conditions:
         if not isinstance(c, str) or c not in GLOBAL_CONDITIONS:
             raise ValueError("conditions: %r is not one of %s" % (c, GLOBAL_CONDITIONS))
-    if len(set(conditions)) != len(conditions):
-        raise ValueError("conditions: %s repeats a condition" % (conditions,))
-    if len(conditions) > batch:
-        raise ValueError("%d conditions do not fit one device pass of batch = %d" % (len(conditions), batch))
-    return conditions
+    return _check_one_pass(conditions, "condition", batch)
 
 
 def read_photo(path):
@@ -281,10 +290,7 @@ class PhotoColorizer(object):
         its batch is submitted."""
         n = len(photos)
         self._check_photos(photos)
-        if hints is not None:
-            if len(hints) != n:
-                raise ValueError("%d hint lists for %d photos" % (len(hints), n))
-            hints = [self._hint_list(h, i) for i, h in enumerate(hints)]
+        hints = self._hint_lists(hints, n)
         if glob is not None:
             if not self.global_hints:
                 raise ValueError("glob vectors need PhotoColorizer(global_hints=True)")
@@ -313,11 +319,8 @@ class PhotoColorizer(object):
         if len(points) != n:
             raise ValueError("%d point lists for %d photos" % (len(points), n))
         points = [self._point_list(p, i) for i, p in enumerate(points)]
-        if hints is not None and len(hints) != n:
-            raise ValueError("%d hint lists for %d photos" % (len(hints), n))
         self._check_photos(photos)
-        if hints is not None:
-            hints = [self._hint_list(h, i) for i, h in enumerate(hints)]
+        hints = self._hint_lists(hints, n)
         return self._run(photos, hints, None, bool(psnr), points, int(K))
 
     def _point_list(self, p, i):
@@ -345,14 +348,9 @@ class PhotoColorizer(object):
         self._check_photos(photos)
         seed = int(seed)
         M = max(levels)
-
-        def items():
-            for i, a in self._read(photos):
-                yield a.nbytes, 0, (i, a, reveal_points(self.Xd, M, seed, i))
-
-        per = self.batch // len(levels)
-        return self._pipeline(cut_batches(items(), per, self.max_batch_bytes),
-                              lambda b: self._backend.submit_reveal([a for _, a, _ in b], [p for _, _, p in b], levels),
+        return self._pipeline(self._batches(photos, self.batch // len(levels)),
+                              lambda idx, imgs: self._backend.submit_reveal(
+                                  imgs, [reveal_points(self.Xd, M, seed, i) for i in idx], levels),
                               self._backend.collect_reveal)
 
     def global_stats(self, photos):
@@ -361,12 +359,7 @@ class PhotoColorizer(object):
         (idc_photo_prep, then idc_global_stats_batch; no forward).  photos: as colorize.  -> iterator of float32 [316],
         in input order.  glob_vector(row, "hist") of a reference photo's row is the histogram-transfer vector."""
         self._check_photos(photos)
-
-        def items():
-            for i, a in self._read(photos):
-                yield a.nbytes, 0, a
-
-        return self._pipeline(cut_batches(items(), self.batch, self.max_batch_bytes), self._backend.submit_stats,
+        return self._pipeline(self._batches(photos, self.batch), lambda idx, imgs: self._backend.submit_stats(imgs),
                               self._backend.collect_stats)
 
     def global_sweep(self, photos, conditions=GLOBAL_CONDITIONS):
@@ -382,14 +375,8 @@ class PhotoColorizer(object):
             raise ValueError("global_sweep needs PhotoColorizer(global_hints=True)")
         conditions = check_conditions(conditions, self.batch)
         self._check_photos(photos)
-
-        def items():
-            for i, a in self._read(photos):
-                yield a.nbytes, 0, a
-
-        per = self.batch // len(conditions)
-        return self._pipeline(cut_batches(items(), per, self.max_batch_bytes),
-                              lambda b: self._backend.submit_glob(b, conditions), self._backend.collect_glob)
+        return self._pipeline(self._batches(photos, self.batch // len(conditions)),
+                              lambda idx, imgs: self._backend.submit_glob(imgs, conditions), self._backend.collect_glob)
 
     @staticmethod
     def _check_photos(photos):
@@ -400,38 +387,46 @@ class PhotoColorizer(object):
                 raise ValueError("photo %d: need a path or an HxWx3 uint8 array, got %s" % (i, type(p).__name__))
 
     @staticmethod
-    def _hint_list(h, i):
-        if h is None:
+    def _hint_lists(hints, n):
+        """None, or one hint list (or None) per photo -> the same with each list as engine.as_hints gives it."""
+        if hints is None:
             return None
-        h = engine.as_hints(h)
-        if h.shape[0] > _lib.MAX_HINTS:
-            raise ValueError("photo %d: %d hints, at most %d" % (i, h.shape[0], _lib.MAX_HINTS))
-        return h
+        if len(hints) != n:
+            raise ValueError("%d hint lists for %d photos" % (len(hints), n))
+        out = []
+        for i, h in enumerate(hints):
+            if h is not None:
+                h = engine.as_hints(h)
+                if h.shape[0] > _lib.MAX_HINTS:
+                    raise ValueError("photo %d: %d hints, at most %d" % (i, h.shape[0], _lib.MAX_HINTS))
+            out.append(h)
+        return out
 
-    def _read(self, photos):
-        """(index, photo array) in input order, decoded `readahead` ahead of the consumer."""
+    def _batches(self, photos, per_pass, hints=None):
+        """The photos, decoded `readahead` ahead of the consumer, cut into device passes of at most per_pass photos,
+        max_batch_bytes source bytes and IDC_MAX_HINTS hints -> (indices, photo arrays) per pass, in input order."""
         def load(i):
             p = photos[i]
             if isinstance(p, np.ndarray):
                 return i, np.ascontiguousarray(p)
             return i, check_photo(read_photo(p), "photo %d (%s)" % (i, p))
-        return read_ahead(range(len(photos)), load, self.readahead, self.workers)
+
+        def items():
+            for i, a in read_ahead(range(len(photos)), load, self.readahead, self.workers):
+                yield a.nbytes, 0 if hints is None or hints[i] is None else hints[i].shape[0], (i, a)
+
+        for b in cut_batches(items(), per_pass, self.max_batch_bytes):
+            yield [i for i, _ in b], [a for _, a in b]
 
     def _run(self, photos, hints, glob, psnr, points=None, K=0):
-        def items():
-            for i, a in self._read(photos):
-                nh = 0 if hints is None or hints[i] is None else hints[i].shape[0]
-                yield a.nbytes, nh, (i, a)
-
-        def submit(b):
-            idx = [i for i, _ in b]
-            args = ([a for _, a in b], None if hints is None else [hints[i] for i in idx],
+        def submit(idx, imgs):
+            args = (imgs, None if hints is None else [hints[i] for i in idx],
                     None if glob is None else [glob[i] for i in idx], psnr)
             if points is None:
                 return self._backend.submit(*args)
             return self._backend.submit(*args, points=[points[i] for i in idx], K=K)
 
-        return self._pipeline(cut_batches(items(), self.batch, self.max_batch_bytes), submit, self._backend.collect)
+        return self._pipeline(self._batches(photos, self.batch, hints), submit, self._backend.collect)
 
     def _pipeline(self, batches, submit, collect):
         # Batch k-1 is collected after batch k is submitted, so the device always has the next batch queued.  Whatever
@@ -439,8 +434,8 @@ class PhotoColorizer(object):
         # in flight, so no batch is left behind in a buffer slot.
         pending = None
         try:
-            for b in batches:
-                token = submit(b)
+            for idx, imgs in batches:
+                token = submit(idx, imgs)
                 prev, pending = pending, token
                 if prev is not None:
                     for r in collect(prev):
@@ -474,6 +469,11 @@ class _HostBuffer(object):
             self.array = self.tensor = None
             self.lib.idc_host_free(self.ptr)
             self.ptr = None
+
+
+# What a _DeviceBatches submit returns and its collect takes: the slot, the serial number of the batch in it, the
+# batch's n photos with V forward images each, and what the collect needs besides.
+_Batch = collections.namedtuple("_Batch", "slot serial n V info")
 
 
 class _DeviceBatches(object):
@@ -552,15 +552,13 @@ class _DeviceBatches(object):
         s["cap"] = cap
         self._after_alloc()
 
-    def _next_slot(self):
+    def _next_slot(self, photos):
+        """The next slot, once its previous batch (if any) is off the device: render, D2H, all; the batch's photo table,
+        and the photos packed back to back into the slot's page-locked source buffer -> (slot, table, nbytes)."""
         s = self.slots[self.k % 2]
         self.k += 1
-        s["ev_out"].synchronize()          # the slot's previous batch (if any) is off the device: render, D2H, all
+        s["ev_out"].synchronize()
         s["batch"] = self.k
-        return s
-
-    def _pack(self, s, photos):
-        """The batch's photo table; the photos packed back to back into slot s's page-locked source buffer."""
         table = np.zeros(len(photos), _lib.PHOTO_DTYPE)
         off = 0
         for i, a in enumerate(photos):
@@ -572,7 +570,48 @@ class _DeviceBatches(object):
         for i, a in enumerate(photos):
             o = int(table[i]["off"]) * 3
             h_src[o:o + a.nbytes] = a.reshape(-1)
-        return table, nbytes
+        return s, table, nbytes
+
+    def _upload_photos(self, s, nbytes, pairs=()):
+        """H2D of the packed photos and the (device, host) pairs on the copy stream; the compute stream waits for it."""
+        with self.torch.cuda.stream(self.s_in):
+            s["src"][:nbytes].copy_(s["h_src"].tensor[:nbytes], non_blocking=True)
+            for d, h in pairs:
+                d.copy_(h, non_blocking=True)
+            s["ev_in"].record(self.s_in)
+        self.s_comp.wait_event(s["ev_in"])
+
+    def _download(self, s, pairs):
+        """After the work enqueued on the compute stream so far: D2H of the (device, host) pairs on the copy stream,
+        then ev_out, which the slot's next batch and the collect wait for."""
+        s["ev_comp"].record(self.s_comp)
+        with self.torch.cuda.stream(self.s_out):
+            self.s_out.wait_event(s["ev_comp"])
+            for d, h in pairs:
+                h.copy_(d, non_blocking=True)
+            s["ev_out"].record(self.s_out)
+
+    def _finish(self, token):
+        """Wait for a submitted batch's D2H -> its slot.  Raise if the slot has taken a later batch since."""
+        s = token.slot
+        if s["batch"] != token.serial:
+            raise RuntimeError("this batch's buffers were reused by a later batch: iterate one result iterator at a "
+                               "time per PhotoColorizer")
+        s["ev_out"].synchronize()
+        return s
+
+    def _prep(self, s, n, table, L, rgb):
+        """idc_photo_prep of the slot's n photos into L [n,1,X,X] and, unless rgb is None, rgb [n,X,X,3]."""
+        _lib.check(None, self.lib.idc_photo_prep(self.device, n, table.ctypes.data, s["src"].data_ptr(), self.X,
+                                                 L.data_ptr(), None if rgb is None else rgb.data_ptr(),
+                                                 self.s_comp.cuda_stream))
+
+    def _prep_stats(self, s, n, table, L, rgb):
+        """_prep, then each photo's [316] statistics row from rgb into the slot's stats (idc_global_stats_batch)."""
+        self._prep(s, n, table, L, rgb)
+        _lib.check(None, self.lib.idc_global_stats_batch(self.device, n, self.X, self.X, rgb.data_ptr(),
+                                                         self.pts313.data_ptr(), s["stats"].data_ptr(),
+                                                         self.s_comp.cuda_stream))
 
     def _reccs_buffers(self, s, size):
         """Slot s's suggestion outputs, room for `size` centres (queries x K): device and page-locked host.  The slot is
@@ -589,8 +628,7 @@ class _DeviceBatches(object):
     def submit(self, photos, hints, glob, psnr, points=None, K=0):
         torch, lib, X = self.torch, self.lib, self.X
         n = len(photos)
-        s = self._next_slot()
-        table, nbytes = self._pack(s, photos)
+        s, table, nbytes = self._next_slot(photos)
         queries = None
         if points is not None:   # one query (photo of the batch, y4, x4) per point, photo by photo
             queries = np.concatenate([np.zeros((0, 3), np.int32)] + [
@@ -614,21 +652,13 @@ class _DeviceBatches(object):
         if glob is not None:
             s["h_glob"].numpy()[:n] = np.stack(glob)
         hint_len = _lib.HINT_HDR_BYTES + count * _lib.HINT_DTYPE.itemsize
-
-        with torch.cuda.stream(self.s_in):
-            s["src"][:nbytes].copy_(s["h_src"].tensor[:nbytes], non_blocking=True)
-            s["hints"][:hint_len].copy_(s["h_hints"][:hint_len], non_blocking=True)
-            if glob is not None:
-                s["glob"][:n].copy_(s["h_glob"][:n], non_blocking=True)
-            s["ev_in"].record(self.s_in)
+        self._upload_photos(s, nbytes, [(s["hints"][:hint_len], s["h_hints"][:hint_len])]
+                            + ([] if glob is None else [(s["glob"][:n], s["h_glob"][:n])]))
 
         st = self.s_comp
-        st.wait_event(s["ev_in"])
         sh = st.cuda_stream
-        tp = table.ctypes.data
         with torch.cuda.stream(st):
-            _lib.check(None, lib.idc_photo_prep(self.device, n, tp, s["src"].data_ptr(), X, self.L_mc.data_ptr(),
-                                                s["img_rgb"].data_ptr() if psnr else None, sh))
+            self._prep(s, n, table, self.L_mc, s["img_rgb"] if psnr else None)
             _lib.check(None, lib.idc_hint_raster(self.device, n, X, X, count, s["hints"].data_ptr(), self.ab_in.data_ptr(),
                                                  self.mask.data_ptr(), sh))
             self.ctx.forward_device(self.L_mc[:n], self.ab_in[:n], self.mask[:n], self.maskcent,
@@ -641,40 +671,29 @@ class _DeviceBatches(object):
                     self.ctx.ab_reccs_batch(queries[q0:q1], K, out=(s["cen"][q0 * K:q1 * K].view(q1 - q0, K, 2),
                                                                     s["conf"][q0 * K:q1 * K].view(q1 - q0, K), None))
             _lib.check(None, lib.idc_rgb2lab_f64(self.device, n, X, X, s["rgb"].data_ptr(), self.lab.data_ptr(), sh))
-            _lib.check(None, lib.idc_photo_render(self.device, n, tp, s["src"].data_ptr(), X, self.lab.data_ptr(),
-                                                  s["src"].data_ptr(), sh))
+            _lib.check(None, lib.idc_photo_render(self.device, n, table.ctypes.data, s["src"].data_ptr(), X,
+                                                  self.lab.data_ptr(), s["src"].data_ptr(), sh))
             if psnr:
                 _lib.check(None, lib.idc_rgb_sse(self.device, n, X, X, s["img_rgb"].data_ptr(), s["rgb"].data_ptr(),
                                                  s["sse"].data_ptr(), sh))
-            s["ev_comp"].record(st)
 
-        with torch.cuda.stream(self.s_out):
-            self.s_out.wait_event(s["ev_comp"])
-            s["h_full"].tensor[:nbytes].copy_(s["src"][:nbytes], non_blocking=True)
-            s["h_ab"][:n].copy_(s["ab"][:n], non_blocking=True)
-            s["h_rgb"][:n].copy_(s["rgb"][:n], non_blocking=True)
-            if psnr:
-                s["h_sse"][:n].copy_(s["sse"][:n], non_blocking=True)
-            if queries is not None and len(queries):
-                s["h_cen"][:len(queries) * K].copy_(s["cen"][:len(queries) * K], non_blocking=True)
-                s["h_conf"][:len(queries) * K].copy_(s["conf"][:len(queries) * K], non_blocking=True)
-            s["ev_out"].record(self.s_out)
-        return s, s["batch"], table, psnr, None if points is None else [len(p) for p in points], K
+        pairs = [(s["src"][:nbytes], s["h_full"].tensor[:nbytes]), (s["ab"][:n], s["h_ab"][:n]),
+                 (s["rgb"][:n], s["h_rgb"][:n])]
+        if psnr:
+            pairs.append((s["sse"][:n], s["h_sse"][:n]))
+        if queries is not None and len(queries):
+            QK = len(queries) * K
+            pairs += [(s["cen"][:QK], s["h_cen"][:QK]), (s["conf"][:QK], s["h_conf"][:QK])]
+        self._download(s, pairs)
+        return _Batch(s, s["batch"], n, 1, (table, psnr, None if points is None else [len(p) for p in points], K))
 
     def collect(self, token):
-        s, batch, table, psnr, counts, K = token
-        if s["batch"] != batch:
-            raise RuntimeError("this batch's buffers were reused by a later batch: iterate one colorize() result at a "
-                               "time per PhotoColorizer")
-        s["ev_out"].synchronize()
+        s = self._finish(token)
+        table, psnr, counts, K = token.info
         full, ab, rgb, sse = s["h_full"].array, s["h_ab"].numpy(), s["h_rgb"].numpy(), s["h_sse"].numpy()
-        N = self.X * self.X * 3
-        out = []
-        for i, (off, h, w) in enumerate(table.tolist()):
-            p = None
-            if psnr:    # get_result_PSNR: 20 * log10(255 / sqrt(mean(err2))); the sum of err2 is exact, so is the mean
-                p = float(20 * np.log10(255. / np.sqrt(np.float64(sse[i]) / N)))
-            out.append(PhotoResult(full[off * 3:(off + h * w) * 3].reshape(h, w, 3).copy(), rgb[i].copy(), ab[i].copy(), p))
+        out = [PhotoResult(full[off * 3:(off + h * w) * 3].reshape(h, w, 3).copy(), rgb[i].copy(), ab[i].copy(),
+                           _psnr(sse[i], self.X) if psnr else None)
+               for i, (off, h, w) in enumerate(table.tolist())]
         if counts is None:
             return out
         Q = sum(counts)
@@ -706,116 +725,6 @@ class _DeviceBatches(object):
                 s["h_blocks"] = torch.empty((nb,), dtype=torch.uint8, pin_memory=True)
             self._after_alloc()
 
-    def submit_reveal(self, photos, points, levels):
-        """One device pass of a reveal sweep: photo i of the batch is forward images i*L .. i*L+L-1 (L = len(levels)),
-        image i*L+j with the first levels[j] rows of points[i] as hints."""
-        torch, lib, X = self.torch, self.lib, self.X
-        m, L = len(photos), len(levels)
-        N = m * L
-        self._reveal_buffers()
-        s = self._next_slot()
-        table, nbytes = self._pack(s, photos)
-        # hint blocks, one per forward image, in idc_hint_raster's layout; the colours are filled on the device
-        stride = _lib.HINT_HDR_BYTES + (max(levels) * _lib.HINT_DTYPE.itemsize + 15) // 16 * 16
-        hb = s["h_blocks"].numpy()[:N * stride].reshape(N, stride)
-        for i, pts in enumerate(points):
-            rect = np.zeros(max(levels), _lib.HINT_DTYPE)
-            rect["y0"], rect["x0"] = pts[:, 0], pts[:, 1]
-            rect["y1"], rect["x1"] = pts[:, 0] + pts[:, 2] - 1, pts[:, 1] + pts[:, 2] - 1
-            raw = rect.view(np.uint8)
-            for j, c in enumerate(levels):
-                row = hb[i * L + j]
-                row[:_lib.HINT_HDR_BYTES].view(np.int32)[:] = (c, 0, 0, 0)
-                row[_lib.HINT_HDR_BYTES:_lib.HINT_HDR_BYTES + c * _lib.HINT_DTYPE.itemsize] = raw[:c * _lib.HINT_DTYPE.itemsize]
-
-        with torch.cuda.stream(self.s_in):
-            s["src"][:nbytes].copy_(s["h_src"].tensor[:nbytes], non_blocking=True)
-            s["blocks"][:N * stride].copy_(s["h_blocks"][:N * stride], non_blocking=True)
-            s["ev_in"].record(self.s_in)
-
-        st = self.s_comp
-        st.wait_event(s["ev_in"])
-        sh = st.cuda_stream
-        blocks = s["blocks"].data_ptr()
-        with torch.cuda.stream(st):
-            _lib.check(None, lib.idc_photo_prep(self.device, m, table.ctypes.data, s["src"].data_ptr(), X,
-                                                self.L_photo.data_ptr(), self.rgb_photo.data_ptr(), sh))
-            _lib.check(None, lib.idc_rgb2lab_f64(self.device, m, X, X, self.rgb_photo.data_ptr(), self.lab.data_ptr(), sh))
-            _lib.check(None, lib.idc_hint_fill_mean(self.device, N, L, X, self.lab.data_ptr(), blocks, stride, sh))
-            for b in range(N):
-                _lib.check(None, lib.idc_hint_raster(self.device, 1, X, X, levels[b % L], blocks + b * stride,
-                                                     self.ab_in[b].data_ptr(), self.mask[b].data_ptr(), sh))
-            self.L_mc[:N].view(m, L, 1, X, X).copy_(self.L_photo[:m, None].expand(m, L, 1, X, X))
-            s["img_rgb"][:N].view(m, L, X, X, 3).copy_(self.rgb_photo[:m, None].expand(m, L, X, X, 3))
-            self.ctx.forward_device(self.L_mc[:N], self.ab_in[:N], self.mask[:N], self.maskcent, want_rgb=True,
-                                    out_ab=s["ab"][:N], out_rgb=s["rgb"][:N])
-            _lib.check(None, lib.idc_rgb_sse(self.device, N, X, X, s["img_rgb"].data_ptr(), s["rgb"].data_ptr(),
-                                             s["sse"].data_ptr(), sh))
-            s["ev_comp"].record(st)
-
-        with torch.cuda.stream(self.s_out):
-            self.s_out.wait_event(s["ev_comp"])
-            s["h_ab"][:N].copy_(s["ab"][:N], non_blocking=True)
-            s["h_rgb"][:N].copy_(s["rgb"][:N], non_blocking=True)
-            s["h_sse"][:N].copy_(s["sse"][:N], non_blocking=True)
-            s["ev_out"].record(self.s_out)
-        return s, s["batch"], points, L
-
-    def collect_reveal(self, token):
-        s, batch, points, L = token
-        if s["batch"] != batch:
-            raise RuntimeError("this batch's buffers were reused by a later batch: iterate one result iterator at a "
-                               "time per PhotoColorizer")
-        s["ev_out"].synchronize()
-        ab, rgb, sse = s["h_ab"].numpy(), s["h_rgb"].numpy(), s["h_sse"].numpy()
-        N = self.X * self.X * 3
-        out = []
-        for i, pts in enumerate(points):
-            k = slice(i * L, (i + 1) * L)
-            # the formula of collect(): get_result_PSNR with an exact sum of err2
-            psnr = np.array([float(20 * np.log10(255. / np.sqrt(np.float64(e) / N))) for e in sse[k]], np.float64)
-            out.append(RevealResult(psnr, ab[k].copy(), rgb[k].copy(), pts))
-        return out
-
-    def _upload_photos(self, s, nbytes, extra=()):
-        """H2D of the packed photos (and the (device, host) pairs of `extra`) on the copy stream; the compute stream
-        waits for it."""
-        with self.torch.cuda.stream(self.s_in):
-            s["src"][:nbytes].copy_(s["h_src"].tensor[:nbytes], non_blocking=True)
-            for d, h in extra:
-                d.copy_(h, non_blocking=True)
-            s["ev_in"].record(self.s_in)
-        self.s_comp.wait_event(s["ev_in"])
-
-    def submit_stats(self, photos):
-        """One device pass of global_stats: prep -> idc_global_stats_batch -> D2H of the [n,316] rows."""
-        torch, lib, X = self.torch, self.lib, self.X
-        n = len(photos)
-        s = self._next_slot()
-        table, nbytes = self._pack(s, photos)
-        self._upload_photos(s, nbytes)
-        st = self.s_comp
-        sh = st.cuda_stream
-        with torch.cuda.stream(st):
-            _lib.check(None, lib.idc_photo_prep(self.device, n, table.ctypes.data, s["src"].data_ptr(), X,
-                                                self.L_mc.data_ptr(), s["img_rgb"].data_ptr(), sh))
-            _lib.check(None, lib.idc_global_stats_batch(self.device, n, X, X, s["img_rgb"].data_ptr(),
-                                                        self.pts313.data_ptr(), s["stats"].data_ptr(), sh))
-            s["ev_comp"].record(st)
-        with torch.cuda.stream(self.s_out):
-            self.s_out.wait_event(s["ev_comp"])
-            s["h_stats"][:n].copy_(s["stats"][:n], non_blocking=True)
-            s["ev_out"].record(self.s_out)
-        return s, s["batch"], n
-
-    def collect_stats(self, token):
-        s, batch, n = token
-        if s["batch"] != batch:
-            raise RuntimeError("this batch's buffers were reused by a later batch: iterate one result iterator at a "
-                               "time per PhotoColorizer")
-        s["ev_out"].synchronize()
-        return [r.copy() for r in s["h_stats"].numpy()[:n]]
-
     def _glob_keep(self, conditions):
         """[C,316] bool device tensor: the entries of a statistics row each condition keeps (_GLOB_KEEP)."""
         if conditions not in self._keep:
@@ -823,66 +732,115 @@ class _DeviceBatches(object):
             self._after_alloc()
         return self._keep[conditions]
 
-    def submit_glob(self, photos, conditions):
-        """One device pass of a global-hints sweep: photo i of the batch is forward images i*C .. i*C+C-1 (C =
-        len(conditions)), image i*C+j with glob_vector(stats_i, conditions[j]), no local hints."""
+    def _submit_sweep(self, photos, V, fill):
+        """One device pass of a sweep: photo i of the batch is forward images i*V .. i*V+V-1 (V variants: the levels or
+        the conditions), each with the photo's prepared L and img_rgb.  fill(s, m, table, nbytes) uploads the batch,
+        preps its m photos into L_photo / rgb_photo and makes the forward's ab / mask planes on the compute stream; it
+        returns the forward's glob rows (or None) and the (device, host) pairs it adds to the D2H of ab, rgb and SSE."""
         torch, lib, X = self.torch, self.lib, self.X
-        m, C = len(photos), len(conditions)
-        N = m * C
-        self._photo_buffers()
-        keep = self._glob_keep(conditions)
-        s = self._next_slot()
-        table, nbytes = self._pack(s, photos)
-        s["h_hints"].numpy()[:_lib.HINT_HDR_BYTES].view(np.int32)[:] = 0        # an empty hint block: zero planes
-        self._upload_photos(s, nbytes, [(s["hints"][:_lib.HINT_HDR_BYTES], s["h_hints"][:_lib.HINT_HDR_BYTES])])
-        st = self.s_comp
-        sh = st.cuda_stream
-        with torch.cuda.stream(st):
-            _lib.check(None, lib.idc_photo_prep(self.device, m, table.ctypes.data, s["src"].data_ptr(), X,
-                                                self.L_photo.data_ptr(), self.rgb_photo.data_ptr(), sh))
-            _lib.check(None, lib.idc_global_stats_batch(self.device, m, X, X, self.rgb_photo.data_ptr(),
-                                                        self.pts313.data_ptr(), s["stats"].data_ptr(), sh))
-            # glob rows: each entry of the photo's row copied or 0 (exact, as glob_vector)
-            torch.where(keep[None], s["stats"][:m, None], self.zero, out=s["glob"][:N].view(m, C, 316))
-            self.L_mc[:N].view(m, C, 1, X, X).copy_(self.L_photo[:m, None].expand(m, C, 1, X, X))
-            s["img_rgb"][:N].view(m, C, X, X, 3).copy_(self.rgb_photo[:m, None].expand(m, C, X, X, 3))
-            _lib.check(None, lib.idc_hint_raster(self.device, N, X, X, 0, s["hints"].data_ptr(), self.ab_in.data_ptr(),
-                                                 self.mask.data_ptr(), sh))
-            self.ctx.forward_device(self.L_mc[:N], self.ab_in[:N], self.mask[:N], self.maskcent, glob=s["glob"][:N],
+        m = len(photos)
+        N = m * V
+        s, table, nbytes = self._next_slot(photos)
+        glob, extra = fill(s, m, table, nbytes)
+        with torch.cuda.stream(self.s_comp):
+            self.L_mc[:N].view(m, V, 1, X, X).copy_(self.L_photo[:m, None].expand(m, V, 1, X, X))
+            s["img_rgb"][:N].view(m, V, X, X, 3).copy_(self.rgb_photo[:m, None].expand(m, V, X, X, 3))
+            self.ctx.forward_device(self.L_mc[:N], self.ab_in[:N], self.mask[:N], self.maskcent, glob=glob,
                                     want_rgb=True, out_ab=s["ab"][:N], out_rgb=s["rgb"][:N])
             _lib.check(None, lib.idc_rgb_sse(self.device, N, X, X, s["img_rgb"].data_ptr(), s["rgb"].data_ptr(),
-                                             s["sse"].data_ptr(), sh))
-            s["ev_comp"].record(st)
-        with torch.cuda.stream(self.s_out):
-            self.s_out.wait_event(s["ev_comp"])
-            s["h_ab"][:N].copy_(s["ab"][:N], non_blocking=True)
-            s["h_rgb"][:N].copy_(s["rgb"][:N], non_blocking=True)
-            s["h_sse"][:N].copy_(s["sse"][:N], non_blocking=True)
-            s["h_stats"][:m].copy_(s["stats"][:m], non_blocking=True)
-            s["ev_out"].record(self.s_out)
-        return s, s["batch"], m, C
+                                             s["sse"].data_ptr(), self.s_comp.cuda_stream))
+        self._download(s, [(s["ab"][:N], s["h_ab"][:N]), (s["rgb"][:N], s["h_rgb"][:N]),
+                           (s["sse"][:N], s["h_sse"][:N])] + extra)
+        return _Batch(s, s["batch"], m, V, None)
 
-    def collect_glob(self, token):
-        s, batch, m, C = token
-        if s["batch"] != batch:
-            raise RuntimeError("this batch's buffers were reused by a later batch: iterate one result iterator at a "
-                               "time per PhotoColorizer")
-        s["ev_out"].synchronize()
-        ab, rgb, sse, stats = s["h_ab"].numpy(), s["h_rgb"].numpy(), s["h_sse"].numpy(), s["h_stats"].numpy()
-        N = self.X * self.X * 3
+    def _collect_sweep(self, token):
+        """A sweep's results -> per photo (psnr float64 [V], ab float32 [V,2,X,X], rgb uint8 [V,X,X,3])."""
+        s, V = self._finish(token), token.V
+        ab, rgb, sse = s["h_ab"].numpy(), s["h_rgb"].numpy(), s["h_sse"].numpy()
         out = []
-        for i in range(m):
-            k = slice(i * C, (i + 1) * C)
-            # the formula of collect(): get_result_PSNR with an exact sum of err2
-            psnr = np.array([float(20 * np.log10(255. / np.sqrt(np.float64(e) / N))) for e in sse[k]], np.float64)
-            out.append(GlobalSweepResult(psnr, ab[k].copy(), rgb[k].copy(), stats[i].copy()))
+        for i in range(token.n):
+            k = slice(i * V, (i + 1) * V)
+            out.append((np.array([_psnr(e, self.X) for e in sse[k]], np.float64), ab[k].copy(), rgb[k].copy()))
         return out
 
+    def submit_reveal(self, photos, points, levels):
+        """One device pass of a reveal sweep: image i*L+j of the sweep (L = len(levels)) has the first levels[j] rows of
+        points[i] as hints, coloured with the mean ground-truth ab under each (idc_hint_fill_mean)."""
+        lib, X, L = self.lib, self.X, len(levels)
+        self._reveal_buffers()
+        # hint blocks, one per forward image, in idc_hint_raster's layout; the colours are filled on the device
+        stride = _lib.HINT_HDR_BYTES + (max(levels) * _lib.HINT_DTYPE.itemsize + 15) // 16 * 16
+
+        def fill(s, m, table, nbytes):
+            N = m * L
+            hb = s["h_blocks"].numpy()[:N * stride].reshape(N, stride)
+            for i, pts in enumerate(points):
+                rect = np.zeros(max(levels), _lib.HINT_DTYPE)
+                rect["y0"], rect["x0"] = pts[:, 0], pts[:, 1]
+                rect["y1"], rect["x1"] = pts[:, 0] + pts[:, 2] - 1, pts[:, 1] + pts[:, 2] - 1
+                raw = rect.view(np.uint8)
+                for j, c in enumerate(levels):
+                    row = hb[i * L + j]
+                    row[:_lib.HINT_HDR_BYTES].view(np.int32)[:] = (c, 0, 0, 0)
+                    row[_lib.HINT_HDR_BYTES:_lib.HINT_HDR_BYTES + c * _lib.HINT_DTYPE.itemsize] = \
+                        raw[:c * _lib.HINT_DTYPE.itemsize]
+            self._upload_photos(s, nbytes, [(s["blocks"][:N * stride], s["h_blocks"][:N * stride])])
+            sh, blocks = self.s_comp.cuda_stream, s["blocks"].data_ptr()
+            self._prep(s, m, table, self.L_photo, self.rgb_photo)
+            _lib.check(None, lib.idc_rgb2lab_f64(self.device, m, X, X, self.rgb_photo.data_ptr(), self.lab.data_ptr(), sh))
+            _lib.check(None, lib.idc_hint_fill_mean(self.device, N, L, X, self.lab.data_ptr(), blocks, stride, sh))
+            for b in range(N):
+                _lib.check(None, lib.idc_hint_raster(self.device, 1, X, X, levels[b % L], blocks + b * stride,
+                                                     self.ab_in[b].data_ptr(), self.mask[b].data_ptr(), sh))
+            return None, []
+
+        return self._submit_sweep(photos, L, fill)._replace(info=points)
+
+    def collect_reveal(self, token):
+        return [RevealResult(p, ab, rgb, pts) for (p, ab, rgb), pts in zip(self._collect_sweep(token), token.info)]
+
+    def submit_stats(self, photos):
+        """One device pass of global_stats: prep -> idc_global_stats_batch -> D2H of the [n,316] rows."""
+        n = len(photos)
+        s, table, nbytes = self._next_slot(photos)
+        self._upload_photos(s, nbytes)
+        self._prep_stats(s, n, table, self.L_mc, s["img_rgb"])
+        self._download(s, [(s["stats"][:n], s["h_stats"][:n])])
+        return _Batch(s, s["batch"], n, 1, None)
+
+    def collect_stats(self, token):
+        return [r.copy() for r in self._finish(token)["h_stats"].numpy()[:token.n]]
+
+    def submit_glob(self, photos, conditions):
+        """One device pass of a global-hints sweep: image i*C+j of the sweep (C = len(conditions)) has no local hints
+        and glob_vector(stats_i, conditions[j]), stats_i being photo i's own statistics."""
+        torch, X, C = self.torch, self.X, len(conditions)
+        self._photo_buffers()
+        keep = self._glob_keep(conditions)
+
+        def fill(s, m, table, nbytes):
+            N = m * C
+            s["h_hints"].numpy()[:_lib.HINT_HDR_BYTES].view(np.int32)[:] = 0        # an empty hint block: zero planes
+            self._upload_photos(s, nbytes, [(s["hints"][:_lib.HINT_HDR_BYTES], s["h_hints"][:_lib.HINT_HDR_BYTES])])
+            with torch.cuda.stream(self.s_comp):
+                self._prep_stats(s, m, table, self.L_photo, self.rgb_photo)
+                # glob rows: each entry of the photo's row copied or 0 (exact, as glob_vector)
+                torch.where(keep[None], s["stats"][:m, None], self.zero, out=s["glob"][:N].view(m, C, 316))
+                _lib.check(None, self.lib.idc_hint_raster(self.device, N, X, X, 0, s["hints"].data_ptr(),
+                                                          self.ab_in.data_ptr(), self.mask.data_ptr(),
+                                                          self.s_comp.cuda_stream))
+            return s["glob"][:N], [(s["stats"][:m], s["h_stats"][:m])]
+
+        return self._submit_sweep(photos, C, fill)
+
+    def collect_glob(self, token):
+        out, stats = self._collect_sweep(token), token.slot["h_stats"].numpy()
+        return [GlobalSweepResult(p, ab, rgb, stats[i].copy()) for i, (p, ab, rgb) in enumerate(out)]
+
     def discard(self, token):
-        """Wait for a batch nobody will collect (its results are dropped)."""
-        s, batch = token[:2]
-        if s["batch"] == batch:
-            s["ev_out"].synchronize()
+        """Wait for a batch nobody will collect (its results are dropped), unless its slot was reused since."""
+        if token.slot["batch"] == token.serial:
+            self._finish(token)
 
     def close(self):
         self.torch.cuda.synchronize(self.dev)

@@ -623,16 +623,30 @@ int take_device_flags(Ctx* c, const char* msg) {
               "saturated; lower the exponent with act_exp.<buffer>)", names.c_str());
 }
 
-// idc_forward_host's copy/compute overlap: the batch is cut into image chunks; conv1_1 of chunk k waits for the
-// H2D of chunk k only (issued on HostPipeStreams::s_in), and the last op (c10_2 + fused model_out) runs per chunk so
-// that the D2H of ab chunk k (on HostPipeStreams::s_out) overlaps the compute of chunk k+1.  Everything in between
-// runs on the whole batch.
+// idc_forward_host's copy/compute overlap (eager path, batches >= 8): the batch is cut into image chunks; conv1_1 of
+// chunk k waits for the L, ab and mask copies of chunk k only (issued on HostPipeStreams::s_in), and the last op (c10_2
+// + fused model_out) runs per chunk so that the D2H of ab chunk k (on HostPipeStreams::s_out) overlaps the compute of
+// chunk k+1.  Everything in between runs on the whole batch.
 struct HostPipe {
   static constexpr int kMaxChunks = 8;   // == the size of HostPipeStreams::ev_in / ev_out
   int nchunks = 0;
   int start[kMaxChunks + 1] = {};        // image ranges [start[k], start[k+1])
-  float* ab_dst = nullptr;    // pinned host destination of out_ab (caller's buffer or the staging block)
+  float* ab_dst = nullptr;    // pinned host destination of out_ab: the caller's buffer or its twin in h_out
 };
+
+// One copy of an idc_forward_host call: the caller's buffer `user`, the device region `dev` and its page-locked twin
+// `twin` (HostStaging).  A staged copy goes through the twin; the CPU moves the bytes between it and `user`.  The hint
+// block is its own twin (user == twin): it is never staged.
+struct HostCopy {
+  char* user = nullptr;
+  char* dev = nullptr;
+  char* twin = nullptr;
+  size_t bytes = 0;             // 0: the call has no such tensor (dev and twin are still its place)
+  bool d2h = false, staged = false;
+  char* host() const { return staged ? twin : user; }
+};
+// the copy list, in issue order: the inputs, then the outputs
+enum { kCpHints, kCpL, kCpAb, kCpMask, kCpGlob, kCpOutAb, kCpRgb, kCpAbq, kCpDist, kNumCopies };
 
 // idc_set_click: layout of the click answer block (device d_clickout, pinned host h_clickout)
 constexpr int kClickInit = 8, kClickMaxIter = 100;                       // the defaults of LhnContext.ab_reccs
@@ -967,110 +981,125 @@ int idc_forward_host(idc_ctx* c, int n, int h, int w, const float* L, const floa
   return idc_forward_host_q(c, n, h, w, L, ab, mask, maskcent, glob, out_ab, out_dist, out_rgb, nullptr);
 }
 
+// The copies of one idc_forward_host call (see HostStaging for the regions).  The inputs sit packed for n at the head
+// of d_in; the outputs land in d_small on the click graph (`graph`), in d_out, d_rgb and AbqStaging otherwise.
+static void host_copies(Ctx* c, int n, bool graph, const float* L, const float* ab, const float* mask, const float* glob,
+                        float* out_ab, float* out_dist, uint8_t* out_rgb, double* out_abq, HostCopy* cp) {
+  const HostStaging& sg = *c->stage;
+  const size_t HW = (size_t)c->H * c->W, HW4 = (size_t)(c->H / 4) * (c->W / 4);
+  auto set = [&](int k, const void* user, void* dev, void* twin, size_t bytes, bool d2h) {
+    cp[k] = {(char*)user, (char*)dev, (char*)twin, user ? bytes : 0, d2h};
+  };
+  const size_t b_L = (size_t)n * HW * sizeof(float), b_ab = 2 * b_L, b_rgb = (size_t)n * 3 * HW, b_q = 2 * b_ab;
+  char* d_in = (char*)sg.d_in.get(); char* h_in = (char*)sg.h_in.get();
+  char* hints = (!ab && !mask) ? c->hints->h_hints.get() : nullptr;
+  set(kCpHints, hints, hints ? c->hints->d_hints.get() : nullptr, hints, kHintBlockBytes, false);
+  set(kCpL, L, d_in, h_in, b_L, false);
+  set(kCpAb, ab, d_in + b_L, h_in + b_L, b_ab, false);
+  set(kCpMask, mask, d_in + 3 * b_L, h_in + 3 * b_L, b_L, false);
+  set(kCpGlob, glob, d_in + 4 * b_L, h_in + 4 * b_L, (size_t)n * 316 * sizeof(float), false);
+  if (graph) {
+    char* d = sg.d_small.get(); char* h = sg.h_small.get();
+    set(kCpOutAb, out_ab, d, h, b_ab, true);
+    set(kCpRgb, out_rgb, d + b_ab, h + b_ab, b_rgb, true);
+    set(kCpAbq, out_abq, d + b_ab + b_rgb, h + b_ab + b_rgb, b_q, true);
+  } else {
+    set(kCpOutAb, out_ab, sg.d_out.get(), sg.h_out.get(), b_ab, true);
+    set(kCpRgb, out_rgb, sg.d_rgb.get(), sg.h_rgb.get(), b_rgb, true);
+    set(kCpAbq, out_abq, c->abq ? c->abq->d_abq.get() : nullptr, c->abq ? c->abq->h_abq.get() : nullptr, b_q, true);
+  }
+  const size_t dist_off = (size_t)c->max_n * 2 * HW;
+  set(kCpDist, out_dist, sg.d_out.get() + dist_off, sg.h_out.get() + dist_off, (size_t)n * 529 * HW4 * sizeof(float), true);
+}
+
+// images [i0, i1) of a per-image copy
+static HostCopy image_range(HostCopy e, int n, int i0, int i1) {
+  const size_t per = e.bytes / n;
+  e.user += i0 * per; e.dev += i0 * per; e.twin += i0 * per;
+  e.bytes = (i1 - i0) * per;
+  return e;
+}
+
+static void stage_inputs(const HostCopy* cp, int count) {
+  for (int k = 0; k < count; ++k) if (cp[k].bytes && cp[k].staged && !cp[k].d2h) memcpy(cp[k].twin, cp[k].user, cp[k].bytes);
+}
+
+static void unstage_outputs(const HostCopy* cp, int count) {
+  for (int k = 0; k < count; ++k) if (cp[k].bytes && cp[k].staged && cp[k].d2h) memcpy(cp[k].user, cp[k].twin, cp[k].bytes);
+}
+
+static cudaError_t copy_async(const HostCopy& e, size_t bytes, cudaStream_t st) {
+  return e.d2h ? cudaMemcpyAsync(e.host(), e.dev, bytes, cudaMemcpyDeviceToHost, st)
+               : cudaMemcpyAsync(e.dev, e.host(), bytes, cudaMemcpyHostToDevice, st);
+}
+
+// cp[0, count) as ONE copy when they follow each other both on the host and on the device, one copy each otherwise.
+// All or nothing: caller buffers that merely touch may be separate allocations, which one copy cannot span; the click
+// buffers and each twin are one block.
+static cudaError_t issue_copies(const HostCopy* cp, int count, cudaStream_t st) {
+  const HostCopy* a = nullptr;
+  size_t bytes = 0;
+  bool one = true;
+  for (int k = 0; k < count; ++k) {
+    if (!cp[k].bytes) continue;
+    if (a) one = one && cp[k].host() == a->host() + bytes && cp[k].dev == a->dev + bytes;
+    else a = &cp[k];
+    bytes += cp[k].bytes;
+  }
+  if (!a || one) return a ? copy_async(*a, bytes, st) : cudaSuccess;
+  for (int k = 0; k < count; ++k) {
+    cudaError_t e = cp[k].bytes ? copy_async(cp[k], cp[k].bytes, st) : cudaSuccess;
+    if (e != cudaSuccess) return e;
+  }
+  return cudaSuccess;
+}
+
+static int run_host_forward(Ctx* c, int n, float maskcent, const HostCopy* cp, bool want_dist, cudaStream_t st,
+                            const HostPipe* hp) {
+  auto f = [&](int k) { return reinterpret_cast<float*>(cp[k].dev); };
+  auto on = [&](int k) { return cp[k].bytes != 0; };
+  return run_forward(c, n, f(kCpL), f(kCpAb), f(kCpMask), maskcent, on(kCpGlob) ? f(kCpGlob) : nullptr, f(kCpOutAb),
+                     want_dist ? f(kCpDist) : nullptr, on(kCpRgb) ? reinterpret_cast<uint8_t*>(cp[kCpRgb].dev) : nullptr,
+                     st, hp, on(kCpAbq) ? reinterpret_cast<double*>(cp[kCpAbq].dev) : nullptr,
+                     on(kCpHints) ? cp[kCpHints].dev : nullptr);
+}
+
 // Small batches (the interactive click): ONE graph launch does everything -- the H2D of the inputs, the kernels
 // (chained by programmatic dependent launch), the D2H of the results.
-//   * pinned caller buffers (idc_host_alloc; see LhnContext.click_buffers): the copy nodes read / write the caller's
-//     memory directly -- no CPU copy at all.  Buffers laid out back to back ([L | ab | mask | glob], [ab | rgb | abq])
-//     travel as ONE copy each way.  The graph is keyed on the pointers and re-captured when they change.
-//   * pageable caller buffers: staged through the context's pinned blocks by the CPU (one copy node each way).
-//   * hint mode (ab == mask == NULL): the ab / mask H2D is replaced by one fixed-size copy of the whole pinned hint block
-//     and the raster kernel; the list length lives in the block, so editing the hints never re-captures the graph.
-static int forward_host_small(idc_ctx* c, int n, const float* L, const float* ab, const float* mask, float maskcent,
-                              const float* glob, float* out_ab, float* out_dist, uint8_t* out_rgb, double* out_abq,
-                              bool hint_mode) {
-  const size_t HW = (size_t)c->H * c->W, HW4 = (size_t)(c->H / 4) * (c->W / 4);
+//   * page-locked caller buffers (idc_host_alloc; see LhnContext.click_buffers): the copy nodes read / write the
+//     caller's memory directly -- no CPU copy at all.  Buffers laid out back to back ([L | ab | mask | glob],
+//     [ab | rgb | abq]) travel as ONE copy each way.  The graph is keyed on the pointers and re-captured when they change.
+//   * otherwise every copy is staged: the CPU copies through the twins, which are one copy node each way.
+//   * hint mode: the list length lives in the fixed-size hint block, so editing the hints never re-captures the graph.
+static int forward_host_graph(Ctx* c, int n, float maskcent, HostCopy* cp, bool want_dist) {
   cudaStream_t st = c->own_stream.get();
-  const HostStaging& sg = *c->stage;
-  const bool copy_dist = out_dist != nullptr;
-  const bool want_dist = copy_dist || (c->dist_resident && c->dist);
-  const bool want_rgb = out_rgb != nullptr, want_glob = glob != nullptr, want_q = out_abq != nullptr;
-  // compact device layouts for this n
-  float* dL = sg.d_in.get(); float* dab = dL + (size_t)n * HW; float* dmask = dab + (size_t)n * 2 * HW;
-  float* dglob = dmask + (size_t)n * HW;
-  const size_t b_ab = (size_t)n * 2 * HW * sizeof(float), b_rgb = (size_t)n * 3 * HW, b_q = (size_t)n * 2 * HW * sizeof(double);
-  char* dsm = sg.d_small.get(); char* hsm = sg.h_small.get();
-  float* dout = reinterpret_cast<float*>(dsm);
-  uint8_t* drgb = reinterpret_cast<uint8_t*>(dsm + b_ab);
-  double* dq = reinterpret_cast<double*>(dsm + b_ab + b_rgb);
-  float* ddist = sg.d_out.get() + (size_t)c->max_n * 2 * HW;
-  const size_t out_bytes = b_ab + (want_rgb ? b_rgb : 0) + (want_q ? b_q : 0);
+  const bool copy_dist = cp[kCpDist].bytes, want_rgb = cp[kCpRgb].bytes, want_glob = cp[kCpGlob].bytes;
+  const bool want_q = cp[kCpAbq].bytes, hint_mode = cp[kCpHints].bytes, have_L = cp[kCpL].bytes;
   const uintptr_t flags = (uintptr_t)n | ((uintptr_t)want_dist << 8) | ((uintptr_t)want_rgb << 9) | ((uintptr_t)want_glob << 10) |
                           ((uintptr_t)want_q << 11) | ((uintptr_t)copy_dist << 12) | ((uintptr_t)c->click_mode << 13) |
                           ((uintptr_t)hint_mode << 14);
-  c->click_served = false;
-  const bool have_L = L != nullptr;          // false: the image set by idc_set_image stays where it is
-  const size_t in_floats = (size_t)n * (have_L ? 4 : 3) * HW + (want_glob ? (size_t)n * 316 : 0);
-  const void* direct_key[8] = {(void*)(flags | (1u << 16)), L, ab, mask, glob, out_ab, out_rgb, out_abq};
+  const void* direct_key[8] = {(void*)(flags | (1u << 16)), cp[kCpL].user, cp[kCpAb].user, cp[kCpMask].user,
+                               cp[kCpGlob].user, cp[kCpOutAb].user, cp[kCpRgb].user, cp[kCpAbq].user};
   // fast path: same pinned buffers as the captured graph -> replay without touching the driver's pointer tables
-  bool direct = c->graph_exec.get() && !copy_dist && memcmp(direct_key, c->graph_ptrs, sizeof(direct_key)) == 0 &&
-                c->graph_maskcent == maskcent;
-  bool replay = direct;
-  if (!direct) {
-    direct = !copy_dist && (!have_L || is_pinned(L)) && (hint_mode || (is_pinned(ab) && is_pinned(mask))) &&
-             (!glob || is_pinned(glob)) && is_pinned(out_ab) && (!out_rgb || is_pinned(out_rgb)) &&
-             (!out_abq || is_pinned(out_abq));
-  }
+  const bool replay = c->graph_exec.get() && !copy_dist && memcmp(direct_key, c->graph_ptrs, sizeof(direct_key)) == 0 &&
+                      c->graph_maskcent == maskcent;
+  bool direct = replay || !copy_dist;
+  for (int k = 0; k < kNumCopies && direct && !replay; ++k)
+    direct = !cp[k].bytes || cp[k].user == cp[k].twin || is_pinned(cp[k].user);
+  for (int k = 0; k < kNumCopies; ++k) cp[k].staged = !direct && cp[k].user != cp[k].twin;
   const void* staged_key[8] = {(void*)(flags | ((uintptr_t)have_L << 17)), nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
   const void** key = direct ? direct_key : staged_key;
-  if (!direct) {   // stage the inputs
-    if (have_L) memcpy(sg.h_in.get(), L, (size_t)n * HW * sizeof(float));
-    if (!hint_mode) {
-      memcpy(sg.h_in.get() + (size_t)n * HW, ab, (size_t)n * 2 * HW * sizeof(float));
-      memcpy(sg.h_in.get() + (size_t)n * 3 * HW, mask, (size_t)n * HW * sizeof(float));
-    }
-    if (want_glob) memcpy(sg.h_in.get() + (size_t)n * 4 * HW, glob, (size_t)n * 316 * sizeof(float));
-  }
+  stage_inputs(cp, kCpOutAb);
   if (!replay && (!c->graph_exec.get() || memcmp(key, c->graph_ptrs, sizeof(staged_key)) != 0 || c->graph_maskcent != maskcent)) {
     c->graph_exec.reset();
     cudaGraph_t g = nullptr;
     CUDA_TRY(c, cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
     const bool prof = c->profiling;
     c->profiling = false;            // event timing is meaningless inside a capture
-    cudaError_t ce = cudaSuccess;
-    auto cp = [&](void* dst, const void* src, size_t bytes, cudaMemcpyKind kind) {
-      if (ce == cudaSuccess && bytes) ce = cudaMemcpyAsync(dst, src, bytes, kind, st);
-    };
-    if (hint_mode) {   // the whole hint block (fixed size), then the L planes and the glob vector if they travel
-      cp(c->hints->d_hints.get(), c->hints->h_hints.get(), kHintBlockBytes, cudaMemcpyHostToDevice);
-      if (have_L) cp(dL, direct ? L : sg.h_in.get(), (size_t)n * HW * sizeof(float), cudaMemcpyHostToDevice);
-      if (want_glob) cp(dglob, direct ? glob : sg.h_in.get() + (size_t)n * 4 * HW, (size_t)n * 316 * sizeof(float), cudaMemcpyHostToDevice);
-    } else if (direct) {
-      const bool contig = (!have_L || ab == L + (size_t)n * HW) && mask == ab + (size_t)n * 2 * HW &&
-                          (!want_glob || glob == mask + (size_t)n * HW);
-      if (contig) {
-        cp(have_L ? dL : dab, have_L ? L : ab, in_floats * sizeof(float), cudaMemcpyHostToDevice);
-      } else {
-        if (have_L) cp(dL, L, (size_t)n * HW * sizeof(float), cudaMemcpyHostToDevice);
-        cp(dab, ab, (size_t)n * 2 * HW * sizeof(float), cudaMemcpyHostToDevice);
-        cp(dmask, mask, (size_t)n * HW * sizeof(float), cudaMemcpyHostToDevice);
-        if (want_glob) cp(dglob, glob, (size_t)n * 316 * sizeof(float), cudaMemcpyHostToDevice);
-      }
-    } else {
-      const size_t off = have_L ? 0 : (size_t)n * HW;
-      cp(sg.d_in.get() + off, sg.h_in.get() + off, in_floats * sizeof(float), cudaMemcpyHostToDevice);
-    }
-    int rc = IDC_OK;
-    if (ce == cudaSuccess)
-      rc = run_forward(c, n, dL, dab, dmask, maskcent, want_glob ? dglob : nullptr, dout, want_dist ? ddist : nullptr,
-                       want_rgb ? drgb : nullptr, st, nullptr, want_q ? dq : nullptr, hint_mode ? c->hints->d_hints.get() : nullptr);
-    if (rc == IDC_OK) {
-      if (direct) {
-        const char* o0 = reinterpret_cast<const char*>(out_ab);
-        const bool contig = (!want_rgb || reinterpret_cast<const char*>(out_rgb) == o0 + b_ab) &&
-                            (!want_q || reinterpret_cast<const char*>(out_abq) == o0 + b_ab + b_rgb);
-        if (contig) {
-          cp(out_ab, dsm, out_bytes, cudaMemcpyDeviceToHost);
-        } else {
-          cp(out_ab, dout, b_ab, cudaMemcpyDeviceToHost);
-          if (want_rgb) cp(out_rgb, drgb, b_rgb, cudaMemcpyDeviceToHost);
-          if (want_q) cp(out_abq, dq, b_q, cudaMemcpyDeviceToHost);
-        }
-      } else {
-        cp(hsm, dsm, out_bytes, cudaMemcpyDeviceToHost);
-        if (copy_dist)
-          cp(sg.h_out.get() + (size_t)c->max_n * 2 * HW, ddist, (size_t)n * 529 * HW4 * sizeof(float), cudaMemcpyDeviceToHost);
-      }
-    }
+    cudaError_t ce = issue_copies(cp, kCpOutAb, st);
+    int rc = ce == cudaSuccess ? run_host_forward(c, n, maskcent, cp, want_dist, st, nullptr) : IDC_OK;
+    if (rc == IDC_OK && ce == cudaSuccess) ce = issue_copies(cp + kCpOutAb, kCpDist - kCpOutAb, st);   // [ab | rgb | abq]
+    if (rc == IDC_OK && ce == cudaSuccess) ce = issue_copies(cp + kCpDist, 1, st);
     c->profiling = prof;
     cudaError_t ce2 = cudaStreamEndCapture(st, &g);
     if (rc != IDC_OK) { if (g) cudaGraphDestroy(g); return rc; }
@@ -1091,15 +1120,56 @@ static int forward_host_small(idc_ctx* c, int n, const float* L, const float* ab
   c->last_n = n;
   CUDA_TRY(c, cudaStreamSynchronize(st));
   if (c->dbg_graph_timing) cudaEventElapsedTime(&c->dbg_graph_ms, c->dbg_ev[0].get(), c->dbg_ev[1].get());
-  if (!direct) {
-    memcpy(out_ab, hsm, b_ab);
-    if (want_rgb) memcpy(out_rgb, hsm + b_ab, b_rgb);
-    if (want_q) memcpy(out_abq, hsm + b_ab + b_rgb, b_q);
-    if (copy_dist) memcpy(out_dist, sg.h_out.get() + (size_t)c->max_n * 2 * HW, (size_t)n * 529 * HW4 * sizeof(float));
+  return IDC_OK;
+}
+
+// Every other call: eager copies on the context's stream, with the chunked overlap of HostPipe for batches >= 8.
+// Caller memory is staged tensor by tensor, and each input is copied on its own, so the CPU stages the next input
+// while the last one is in flight.
+static int forward_host_eager(Ctx* c, int n, float maskcent, HostCopy* cp, bool want_dist) {
+  for (int k = 0; k < kNumCopies; ++k) cp[k].staged = cp[k].bytes && cp[k].user != cp[k].twin && !is_pinned(cp[k].user);
+  cudaStream_t st = c->own_stream.get();
+  // large batches: chunked copy/compute overlap (see HostPipe); option host_pipe=0 turns it off for A/B runs
+  const bool pipe_on = c->opt.host_pipe != 0;
+  const bool fused_head = !c->simt && !(c->flags & IDC_FLAG_KEEP_CONV10);
+  HostPipe hp;
+  bool last_splits = false;
+  for (auto& op : c->ops) if (op.fuse_out_head) last_splits = umma_op_uses_split_k(op);
+  if (pipe_on && n >= 8 && fused_head && !last_splits && !c->profiling) {
+    hp.nchunks = n >= 32 ? 4 : 2;   // measured: 8 chunks at n = 64 is 1.3 % slower end to end than 4
+    for (int k = 0; k <= hp.nchunks; ++k) hp.start[k] = (int)((long long)n * k / hp.nchunks);
+    hp.ab_dst = reinterpret_cast<float*>(cp[kCpOutAb].host());
+    if (!c->pipe) {
+      auto g = std::make_unique<HostPipeStreams>();
+      CUDA_TRY(c, new_stream(g->s_in));
+      CUDA_TRY(c, new_stream(g->s_out));
+      for (int k = 0; k < HostPipe::kMaxChunks; ++k) {
+        CUDA_TRY(c, new_event(g->ev_in[k]));
+        CUDA_TRY(c, new_event(g->ev_out[k]));
+      }
+      c->pipe = std::move(g);
+    }
   }
-  c->dist_valid_n = want_dist ? n : 0;
-  c->click_served = want_dist && c->click_mode && c->click;     // the side branch delivered the click's answer
-  if (have_L) c->image_n = n;          // the planes just uploaded are the resident image now
+  auto put = [](const HostCopy& e, cudaStream_t s) { stage_inputs(&e, 1); return issue_copies(&e, 1, s); };
+  if (hp.nchunks) {
+    // the glob vector and the hint block go ahead of the first chunk, so ev_in[0] (which the MLP and the raster launch
+    // wait for) covers them
+    const cudaStream_t s_in = c->pipe->s_in.get();
+    CUDA_TRY(c, put(cp[kCpGlob], s_in));
+    CUDA_TRY(c, put(cp[kCpHints], s_in));
+    for (int k = 0; k < hp.nchunks; ++k) {
+      for (int j = kCpL; j <= kCpMask; ++j) CUDA_TRY(c, put(image_range(cp[j], n, hp.start[k], hp.start[k + 1]), s_in));
+      CUDA_TRY(c, cudaEventRecord(c->pipe->ev_in[k].get(), s_in));
+    }
+  } else {
+    for (int k = 0; k < kCpOutAb; ++k) CUDA_TRY(c, put(cp[k], st));
+  }
+  int rc = run_host_forward(c, n, maskcent, cp, want_dist, st, hp.nchunks ? &hp : nullptr);
+  if (rc != IDC_OK) return rc;
+  for (int k = hp.nchunks ? kCpRgb : kCpOutAb; k < kNumCopies; ++k)   // with HostPipe, run_forward brings ab back
+    CUDA_TRY(c, issue_copies(cp + k, 1, st));
+  CUDA_TRY(c, cudaStreamSynchronize(st));
+  if (hp.nchunks) CUDA_TRY(c, cudaStreamSynchronize(c->pipe->s_out.get()));
   return IDC_OK;
 }
 
@@ -1178,108 +1248,28 @@ int idc_forward_host_q(idc_ctx* c, int n, int h, int w, const float* L, const fl
   CUDA_TRY(c, cudaSetDevice(c->dev));
   rc = take_device_flags(c, "device pipeline watchdog fired earlier (code %d)");   // left over from an asynchronous idc_forward
   if (rc != IDC_OK) return rc;
-  const size_t HW = (size_t)c->H * c->W, HW4 = (size_t)(c->H / 4) * (c->W / 4);
   rc = ensure_host_staging(c);
   if (rc != IDC_OK) return rc;
   if (!L && c->image_n != n)
     return fail(c, IDC_ERR_STATE, "L_mc is NULL but no %d-image set is resident (idc_set_image)", n);
   const bool use_graph = !(c->flags & IDC_FLAG_NO_GRAPH) && n <= 4;
-  if (use_graph) {
-    rc = forward_host_small(c, n, L, ab, mask, maskcent, glob, out_ab, out_dist, out_rgb, out_abq, hint_mode);
-    return rc != IDC_OK ? rc : take_device_flags(c, "device pipeline watchdog fired (code %d)");
-  }
-  if (out_abq && !c->abq) {
+  if (!use_graph && out_abq && !c->abq) {
+    const size_t bytes = (size_t)c->max_n * 2 * c->H * c->W * sizeof(double);
     auto g = std::make_unique<AbqStaging>();
-    CUDA_TRY(c, cudaMalloc(g->d_abq.put(), (size_t)c->max_n * 2 * HW * sizeof(double)));
-    CUDA_TRY(c, cudaMallocHost(g->h_abq.put(), (size_t)c->max_n * 2 * HW * sizeof(double)));
+    CUDA_TRY(c, cudaMalloc(g->d_abq.put(), bytes));
+    CUDA_TRY(c, cudaMallocHost(g->h_abq.put(), bytes));
     c->abq = std::move(g);
   }
-  cudaStream_t st = c->own_stream.get();
-  const HostStaging& sg = *c->stage;
-  // device-side layout of the staging block: [L | ab | mask | glob], [out_ab | out_dist]
-  float* dL = sg.d_in.get(); float* dab = dL + (size_t)c->max_n * HW; float* dmask = dab + (size_t)c->max_n * 2 * HW;
-  float* dglob = dmask + (size_t)c->max_n * HW;
-  float* dout = sg.d_out.get(); float* ddist = dout + (size_t)c->max_n * 2 * HW;
-  auto h2d = [&](float* d, const float* src, size_t count, size_t stage_off) -> cudaError_t {
-    const float* s = src;
-    if (!is_pinned(src)) {   // pageable caller memory: stage through our pinned block
-      memcpy(sg.h_in.get() + stage_off, src, count * sizeof(float));
-      s = sg.h_in.get() + stage_off;
-    }
-    return cudaMemcpyAsync(d, s, count * sizeof(float), cudaMemcpyHostToDevice, st);
-  };
-  // large batches: chunked copy/compute overlap (see HostPipe); option host_pipe=0 turns it off for A/B runs
-  const bool pipe_on = c->opt.host_pipe != 0;
-  const bool fused_head = !c->simt && !(c->flags & IDC_FLAG_KEEP_CONV10);
-  HostPipe hp;
-  bool last_splits = false;
-  for (auto& op : c->ops) if (op.fuse_out_head) last_splits = umma_op_uses_split_k(op);
-  if (pipe_on && n >= 8 && fused_head && !last_splits && !c->profiling) {
-    hp.nchunks = n >= 32 ? 4 : 2;   // measured: 8 chunks at n = 64 is 1.3 % slower end to end than 4
-    for (int k = 0; k <= hp.nchunks; ++k) hp.start[k] = (int)((long long)n * k / hp.nchunks);
-    hp.ab_dst = is_pinned(out_ab) ? out_ab : sg.h_out.get();
-    if (!c->pipe) {
-      auto g = std::make_unique<HostPipeStreams>();
-      CUDA_TRY(c, new_stream(g->s_in));
-      CUDA_TRY(c, new_stream(g->s_out));
-      for (int k = 0; k < HostPipe::kMaxChunks; ++k) {
-        CUDA_TRY(c, new_event(g->ev_in[k]));
-        CUDA_TRY(c, new_event(g->ev_out[k]));
-      }
-      c->pipe = std::move(g);
-    }
-  }
-  if (hp.nchunks) {
-    cudaStream_t compute = st;
-    st = c->pipe->s_in.get();                       // the h2d lambda copies on `st`
-    if (glob) CUDA_TRY(c, h2d(dglob, glob, (size_t)n * 316, (size_t)c->max_n * 4 * HW));
-    // hint mode: the block goes ahead of the first L chunk, so ev_in[0] (which the raster launch waits for) covers it
-    if (hint_mode) CUDA_TRY(c, cudaMemcpyAsync(c->hints->d_hints.get(), c->hints->h_hints.get(), kHintBlockBytes, cudaMemcpyHostToDevice, st));
-    for (int k = 0; k < hp.nchunks; ++k) {
-      const size_t i0 = hp.start[k], nk = hp.start[k + 1] - hp.start[k];
-      if (L) CUDA_TRY(c, h2d(dL + i0 * HW, L + i0 * HW, nk * HW, i0 * HW));
-      if (!hint_mode) {
-        CUDA_TRY(c, h2d(dab + i0 * 2 * HW, ab + i0 * 2 * HW, nk * 2 * HW, (size_t)c->max_n * HW + i0 * 2 * HW));
-        CUDA_TRY(c, h2d(dmask + i0 * HW, mask + i0 * HW, nk * HW, (size_t)c->max_n * 3 * HW + i0 * HW));
-      }
-      CUDA_TRY(c, cudaEventRecord(c->pipe->ev_in[k].get(), st));
-    }
-    st = compute;
-  } else {
-    if (L) CUDA_TRY(c, h2d(dL, L, n * HW, 0));
-    if (hint_mode) {
-      CUDA_TRY(c, cudaMemcpyAsync(c->hints->d_hints.get(), c->hints->h_hints.get(), kHintBlockBytes, cudaMemcpyHostToDevice, st));
-    } else {
-      CUDA_TRY(c, h2d(dab, ab, n * 2 * HW, (size_t)c->max_n * HW));
-      CUDA_TRY(c, h2d(dmask, mask, n * HW, (size_t)c->max_n * 3 * HW));
-    }
-    if (glob) CUDA_TRY(c, h2d(dglob, glob, (size_t)n * 316, (size_t)c->max_n * 4 * HW));
-  }
-
-  const bool copy_dist = out_dist != nullptr;
-  const bool want_dist = copy_dist || (c->dist_resident && c->dist);
-  const bool want_rgb = out_rgb != nullptr, want_glob = glob != nullptr;
-  rc = run_forward(c, n, dL, dab, dmask, maskcent, want_glob ? dglob : nullptr, dout, want_dist ? ddist : nullptr,
-                   want_rgb ? sg.d_rgb.get() : nullptr, st, hp.nchunks ? &hp : nullptr, out_abq ? c->abq->d_abq.get() : nullptr,
-                   hint_mode ? c->hints->d_hints.get() : nullptr);
+  HostCopy cp[kNumCopies];
+  host_copies(c, n, use_graph, L, ab, mask, glob, out_ab, out_dist, out_rgb, out_abq, cp);
+  const bool want_dist = out_dist || (c->dist_resident && c->dist);
+  c->click_served = false;
+  rc = use_graph ? forward_host_graph(c, n, maskcent, cp, want_dist) : forward_host_eager(c, n, maskcent, cp, want_dist);
   if (rc != IDC_OK) return rc;
-  auto d2h = [&](void* dst, const void* d, size_t bytes, void* stage) -> cudaError_t {
-    if (is_pinned(dst)) return cudaMemcpyAsync(dst, d, bytes, cudaMemcpyDeviceToHost, st);
-    return cudaMemcpyAsync(stage, d, bytes, cudaMemcpyDeviceToHost, st);
-  };
-  float* h_out = sg.h_out.get();
-  if (!hp.nchunks) CUDA_TRY(c, d2h(out_ab, dout, n * 2 * HW * sizeof(float), h_out));
-  if (copy_dist) CUDA_TRY(c, d2h(out_dist, ddist, n * 529 * HW4 * sizeof(float), h_out + (size_t)c->max_n * 2 * HW));
-  if (want_rgb) CUDA_TRY(c, d2h(out_rgb, sg.d_rgb.get(), n * HW * 3, sg.h_rgb.get()));
-  if (out_abq) CUDA_TRY(c, d2h(out_abq, c->abq->d_abq.get(), n * 2 * HW * sizeof(double), c->abq->h_abq.get()));
-  CUDA_TRY(c, cudaStreamSynchronize(st));
-  if (hp.nchunks) CUDA_TRY(c, cudaStreamSynchronize(c->pipe->s_out.get()));
-  if (L) c->image_n = n;
-  if (!is_pinned(out_ab)) memcpy(out_ab, h_out, n * 2 * HW * sizeof(float));
-  if (copy_dist && !is_pinned(out_dist)) memcpy(out_dist, h_out + (size_t)c->max_n * 2 * HW, n * 529 * HW4 * sizeof(float));
+  unstage_outputs(cp, kNumCopies);
   c->dist_valid_n = want_dist ? n : 0;
-  if (want_rgb && !is_pinned(out_rgb)) memcpy(out_rgb, sg.h_rgb.get(), n * HW * 3);
-  if (out_abq && !is_pinned(out_abq)) memcpy(out_abq, c->abq->h_abq.get(), n * 2 * HW * sizeof(double));
+  c->click_served = use_graph && want_dist && c->click_mode && c->click;   // the side branch delivered the click's answer
+  if (L) c->image_n = n;               // the planes just uploaded are the resident image now
   return take_device_flags(c, "device pipeline watchdog fired (code %d)");
 }
 

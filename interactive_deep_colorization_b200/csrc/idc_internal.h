@@ -173,12 +173,18 @@ struct HostTensor {
 
 // Resources a context creates at first use, one group at a time.  A group is built into a local and moved into the
 // context only when every allocation in it succeeded, so the context holds it whole or not at all.
-struct HostStaging {   // idc_forward_host / idc_set_image: [L | ab | mask | glob] in, [out_ab | out_dist] out
+// idc_forward_host / idc_set_image.  Every device region has a page-locked host twin of the same size (d_in / h_in,
+// d_out / h_out, d_rgb / h_rgb, d_small / h_small, AbqStaging; the hint block is the same kind of pair): a copy through
+// pageable caller memory goes between a device address and the host address at the same offset in its twin.
+//   d_in    [L | ab | mask | glob] packed for the call's n; idc_set_image leaves L at its head
+//   d_out   ab of the eager path, then the dist at max_n * 2HW (idc_fetch_dist, idc_ab_reccs, idc_dist_negentropy)
+//   d_rgb   rgb of the eager path;  d_small  [ab | rgb | quantised ab] packed for n, the outputs of the click graph
+struct HostStaging {
   DevMem<float> d_in, d_out; HostMem<float> h_in, h_out;
   DevMem<uint8_t> d_rgb; HostMem<uint8_t> h_rgb;
-  DevMem<char> d_small; HostMem<char> h_small;   // compact [ab | rgb | quantised ab] block of the batch <= 4 graph path
+  DevMem<char> d_small; HostMem<char> h_small;
 };
-struct AbqStaging { DevMem<double> d_abq; HostMem<double> h_abq; };   // quantised ab (row a11) of the large-batch path
+struct AbqStaging { DevMem<double> d_abq; HostMem<double> h_abq; };   // quantised ab (row a11) of the eager path
 // idc_set_hints: [kHintHdrBytes header (int count) | IDC_MAX_HINTS x idc_hint], pinned host + device copy
 struct HintBlock { HostMem<char> h_hints; DevMem<char> d_hints; };
 // idc_set_click: the clicked pixel's pmf + K colour suggestions ride on a side branch of the click graph

@@ -362,29 +362,18 @@ class LhnContext(object):
         out_abq as outputs).  -> dict of numpy views; they stay valid until close().  hints=True: for hint-list clicks
         (set_hints); there is no ab / mask block ("ab" and "mask" are None)."""
         HW = self.H * self.W
-        if hints:
-            n_in = n * HW + (n * 316 if glob else 0)
-            sizes = (n_in * 4, n * 2 * HW * 4 + n * 3 * HW + n * 2 * HW * 8)
-            blocks = [self._host_block(nbytes) for nbytes in sizes]
-            fin = blocks[0].view(np.float32)
-            b_ab, b_rgb = n * 2 * HW * 4, n * 3 * HW
-            return {"L_mc": fin[:n * HW].reshape(n, 1, self.H, self.W), "ab": None, "mask": None,
-                    "glob": fin[n * HW:].reshape(n, 316) if glob else None,
-                    "out_ab": blocks[1][:b_ab].view(np.float32).reshape(n, 2, self.H, self.W),
-                    "out_rgb": blocks[1][b_ab:b_ab + b_rgb].reshape(n, self.H, self.W, 3),
-                    "out_abq": blocks[1][b_ab + b_rgb:].view(np.float64).reshape(n, 2, self.H, self.W)}
-        n_in = n * 4 * HW + (n * 316 if glob else 0)
+        planes = 1 if hints else 4                   # [L | glob] or [L | ab | mask | glob]
         b_ab, b_rgb, b_q = n * 2 * HW * 4, n * 3 * HW, n * 2 * HW * 8
-        blocks = [self._host_block(nbytes) for nbytes in (n_in * 4, b_ab + b_rgb + b_q)]
+        blocks = [self._host_block(nbytes) for nbytes in ((n * planes * HW + (n * 316 if glob else 0)) * 4,
+                                                          b_ab + b_rgb + b_q)]
         fin = blocks[0].view(np.float32)
-        out = {"L_mc": fin[:n * HW].reshape(n, 1, self.H, self.W),
-               "ab": fin[n * HW:3 * n * HW].reshape(n, 2, self.H, self.W),
-               "mask": fin[3 * n * HW:4 * n * HW].reshape(n, 1, self.H, self.W),
-               "glob": fin[4 * n * HW:].reshape(n, 316) if glob else None,
-               "out_ab": blocks[1][:b_ab].view(np.float32).reshape(n, 2, self.H, self.W),
-               "out_rgb": blocks[1][b_ab:b_ab + b_rgb].reshape(n, self.H, self.W, 3),
-               "out_abq": blocks[1][b_ab + b_rgb:].view(np.float64).reshape(n, 2, self.H, self.W)}
-        return out
+        return {"L_mc": fin[:n * HW].reshape(n, 1, self.H, self.W),
+                "ab": None if hints else fin[n * HW:3 * n * HW].reshape(n, 2, self.H, self.W),
+                "mask": None if hints else fin[3 * n * HW:4 * n * HW].reshape(n, 1, self.H, self.W),
+                "glob": fin[planes * n * HW:].reshape(n, 316) if glob else None,
+                "out_ab": blocks[1][:b_ab].view(np.float32).reshape(n, 2, self.H, self.W),
+                "out_rgb": blocks[1][b_ab:b_ab + b_rgb].reshape(n, self.H, self.W, 3),
+                "out_abq": blocks[1][b_ab + b_rgb:].view(np.float64).reshape(n, 2, self.H, self.W)}
 
     def _host_block(self, nbytes):
         p = self.lib.idc_host_alloc(nbytes)

@@ -21,6 +21,13 @@ the single-image suggestions.json, for every photo that has hints:
 
     python ideepcolor_b200.py --color_model caffemodel.pth --image_dir scans/ --hints_dir scan_hints/ --out o/ --suggest 9
 
+With a Caffe checkpoint that also holds the 313-bin distribution head (the caffe.* keys, as the Caffe GUI's colour and
+distribution models share one checkpoint), --caffe --caffe_dist gives the suggestions of that head, the colours from the
+regression head of the same forward:
+
+    python ideepcolor_b200.py --color_model caffe.pth --caffe --caffe_dist --image_dir scans/ --hints_dir h/ --out o/ \
+        --suggest 9
+
 PSNR against the number of hint points revealed from each photo's own colours (photos.reveal_points), written to
 <out>/reveal_psnr.csv with no images:
 
@@ -76,6 +83,9 @@ def parse_args(argv=None):
                     help="the checkpoint has the global-hints branch (glob.* keys; --image_dir)")
     ap.add_argument("--caffe", action="store_true",
                     help="Caffe-scaled weights (mask x 110 and tanh x 100, as ColorizeImageCaffe; --image_dir)")
+    ap.add_argument("--caffe_dist", action="store_true",
+                    help="with --caffe --hints_dir --suggest K: the suggestions of the checkpoint's 313-bin distribution "
+                         "head (caffe.* keys), as ColorizeImageCaffeDist")
     ap.add_argument("--glob_ref", default="", metavar="REF",
                     help="with --global_hints: colour every photo with the ab histogram of photo REF (histogram transfer)")
     ap.add_argument("--glob_sweep", nargs="?", const="", default=None, metavar="C1,C2,...",
@@ -84,18 +94,27 @@ def parse_args(argv=None):
                          "(no images are written)")
     args = ap.parse_args(argv)
     given = {"global_hints": args.global_hints, "caffe": args.caffe, "glob_ref": bool(args.glob_ref),
-             "glob_sweep": args.glob_sweep is not None, "hints_dir": bool(args.hints_dir)}
-    for flag in ("global_hints", "caffe", "glob_ref", "glob_sweep", "hints_dir"):
+             "glob_sweep": args.glob_sweep is not None, "hints_dir": bool(args.hints_dir), "caffe_dist": args.caffe_dist}
+    for flag in ("global_hints", "caffe", "glob_ref", "glob_sweep", "hints_dir", "caffe_dist"):
         if given[flag] and not args.image_dir:
             ap.error("--%s needs --image_dir" % flag)
+    if args.caffe_dist:
+        if not args.caffe:
+            ap.error("--caffe_dist needs --caffe: the 313-bin head belongs to a Caffe checkpoint")
+        if args.global_hints:
+            ap.error("--caffe_dist excludes --global_hints: the global model has no 313-bin head")
+        if not (args.hints_dir and args.suggest > 0):
+            ap.error("--caffe_dist serves --hints_dir HDIR --suggest K only")
     if args.hints_dir:
         for flag, on in (("reveal_sweep", bool(args.reveal_sweep)), ("glob_sweep", given["glob_sweep"]),
                          ("glob_ref", given["glob_ref"])):
             if on:
                 ap.error("--hints_dir excludes --%s" % flag)
-        if args.suggest > 0 and (args.caffe or args.global_hints):
-            ap.error("--hints_dir with --suggest works with the 529-bin distribution head only, not with --%s"
-                     % ("caffe" if args.caffe else "global_hints"))
+        if args.suggest > 0 and args.global_hints:
+            ap.error("--hints_dir with --suggest works with a distribution head, and the global model has none")
+        if args.suggest > 0 and args.caffe and not args.caffe_dist:
+            ap.error("--hints_dir with --suggest and --caffe needs --caffe_dist: a Caffe checkpoint's suggestions come "
+                     "from its 313-bin head")
     if args.caffe and args.pytorch_maskcent:
         ap.error("--caffe and --pytorch_maskcent exclude each other: the Caffe models do not centre the mask")
     args.glob_conditions = None
@@ -218,7 +237,9 @@ def colorize_dir(args):
         os.makedirs(args.out)
     hints = read_hints_dir(args.hints_dir, names) if args.hints_dir else None
     sd = torch.load(args.color_model, map_location="cpu")
-    extra = {"suggest": True} if hints is not None and args.suggest > 0 else {}
+    extra = {}
+    if hints is not None and args.suggest > 0:
+        extra = {"caffe_dist": True} if args.caffe_dist else {"suggest": True}
     pc = PhotoColorizer(sd, Xd=args.load_size, batch=args.batch, device=args.gpu, maskcent=args.pytorch_maskcent,
                         calibrate=args.calibrate_source, global_hints=args.global_hints, caffe=args.caffe, **extra)
     save_ranges(args, pc.act_ranges)

@@ -250,6 +250,19 @@ int idc_ab_reccs_batch(idc_ctx* ctx, int q, const int32_t* queries_host, int K, 
 int idc_caffe313_pred_ab(idc_ctx* ctx, int n, float T, float* out_ab, void* stream);
 int idc_caffe313_dist_pixel(idc_ctx* ctx, int img, int y, int x, float S, float* out313_host);
 int idc_caffe313_dist_map(idc_ctx* ctx, int n, float S, float* out_dist, void* stream);
+/* Colour suggestions of the Caffe distribution model (ColorizeImageCaffeDist.get_ab_reccs, data/colorize_image.py:
+ * 515-547) at many pixels of the images of the context's LAST forward, in one stream-ordered pass: idc_ab_reccs_batch
+ * with the 313-bin head.  queries_host [q][3] int32 (img, y, x) are FULL-resolution pixels (the head's dist_ab_S is the x4
+ * up-sample of the logits).  Each query's pmf is dist_ab_S[img, :, y, x] (the first 313 floats equal
+ * idc_caffe313_dist_pixel(img, y, x, S) bit for bit) padded with 216 zeros, the k-means points are the context's
+ * caffe.pts_in_hull padded with 216 rows of (0, 0), and each query's answer equals idc_ab_reccs_pmf on that padded pmf and
+ * those points bit for bit.  Outputs as idc_ab_reccs_batch (DEVICE memory; pmf_dev [q][529] may be NULL), the same
+ * context scratch, no host synchronisation, the same ordering rules.  IDC_ERR_STATE without IDC_FLAG_CAFFE313 or before
+ * any forward; IDC_ERR_ARG for q, K, max_iter, n_init out of range (as idc_ab_reccs_batch), a non-finite S, a NULL
+ * queries or centers, and a query whose img is outside [0, n) of the last forward or whose pixel is outside h x w
+ * (idc_last_error names it), all before any device call. */
+int idc_caffe313_reccs_batch(idc_ctx* ctx, int q, const int32_t* queries_host, float S, int K, int max_iter, int n_init,
+                             float* centers_dev, float* conf_dev, int32_t* iters_dev, float* pmf_dev, void* stream);
 
 /* Distribution entropy (`compute_entropy`, data/colorize_image.py:356-358 and :545-547:
  * `np.sum(dist_ab * np.log(dist_ab), axis=0)`, the NEGATIVE entropy): out[i, p] = sum_k dist[i, k, p] * logf(dist[i, k, p])
@@ -385,6 +398,9 @@ int idc_global_stats_batch(int device, int n, int h, int w, const uint8_t* rgb, 
  * idc_ab_reccs_batch returns; msg (may be NULL) receives idc_last_error's text.  Touches no device. */
 int idc_ab_reccs_batch_check(int has_head, int n_img, int h, int w, int q, const int32_t* queries, int K, int max_iter,
                              int n_init, char* msg, size_t msg_bytes);
+/* The same for idc_caffe313_reccs_batch: has_head = the context has IDC_FLAG_CAFFE313; queries on the h x w grid. */
+int idc_caffe313_reccs_batch_check(int has_head, int n_img, int h, int w, int q, const int32_t* queries, float S, int K,
+                                   int max_iter, int n_init, char* msg, size_t msg_bytes);
 /* wgmma engine: the exponent S with which activation `name` is stored (FP16 hi/lo planes of value * 2^S), chosen per
  * buffer from the weights by idc_finalize_weights (DESIGN.md §3); 0 on the SIMT engine.  IDC_ERR_KEY for an unknown
  * name, IDC_ERR_STATE before the weights are packed. */

@@ -70,6 +70,10 @@ SYMBOLS = [
     ("idc_caffe313_pred_ab", _c.c_int, [_P, _c.c_int, _c.c_float, _P, _P]),
     ("idc_caffe313_dist_pixel", _c.c_int, [_P, _c.c_int, _c.c_int, _c.c_int, _c.c_float, _P]),
     ("idc_caffe313_dist_map", _c.c_int, [_P, _c.c_int, _c.c_float, _P, _P]),
+    ("idc_caffe313_reccs_batch", _c.c_int, [_P, _c.c_int, _P, _c.c_float, _c.c_int, _c.c_int, _c.c_int, _P, _P, _P, _P,
+                                            _P]),
+    ("idc_caffe313_reccs_batch_check", _c.c_int, [_c.c_int, _c.c_int, _c.c_int, _c.c_int, _c.c_int, _P, _c.c_float,
+                                                  _c.c_int, _c.c_int, _c.c_int, _P, _c.c_size_t]),
     ("idc_negentropy", _c.c_int, [_c.c_int, _c.c_int, _c.c_int, _c.c_int, _P, _P, _P]),
     ("idc_dist_negentropy", _c.c_int, [_P, _c.c_int, _P]),
     ("idc_lab2rgb_u8", _c.c_int, [_c.c_int, _c.c_int, _c.c_int, _c.c_int, _P, _P, _P, _P]),

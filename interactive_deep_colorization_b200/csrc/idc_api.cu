@@ -1432,28 +1432,60 @@ int idc_ab_reccs_pmf(int device, const float* pmf_host, int K, int max_iter, int
   return e == cudaSuccess ? IDC_OK : IDC_ERR_CUDA;
 }
 
-// The host checks of idc_ab_reccs_batch for a context with / without the 529-bin head whose last forward carried
+// The heads a batched suggestion call reads: the entry point's name, the head it needs, and the grid its queries
+// address (the pixels of a forward's image divided by `div`).
+struct ReccsHead {
+  const char* fn;
+  const char* head;
+  int div;
+};
+static const ReccsHead kReccsHead529 = {"idc_ab_reccs_batch", "the 529-bin head (IDC_FLAG_DIST)", 4};
+static const ReccsHead kReccsHead313 = {"idc_caffe313_reccs_batch", "the Caffe 313-bin head (IDC_FLAG_CAFFE313)", 1};
+
+// The host checks of a batched suggestion call for a context with / without `hd`'s head whose last forward carried
 // n_img images of h x w; the message names the first bad query.
-static int reccs_batch_check(bool head, int n_img, int h, int w, int q, const int32_t* queries, int K, int max_iter,
-                             int n_init, char* msg, size_t cap) {
-  if (!head) return snprintf(msg, cap, "idc_ab_reccs_batch needs the 529-bin head (IDC_FLAG_DIST)"), IDC_ERR_STATE;
-  if (n_img < 1) return snprintf(msg, cap, "idc_ab_reccs_batch: no forward has run on this context"), IDC_ERR_STATE;
+static int reccs_batch_check(const ReccsHead& hd, bool head, int n_img, int h, int w, int q, const int32_t* queries, int K,
+                             int max_iter, int n_init, char* msg, size_t cap) {
+  if (!head) return snprintf(msg, cap, "%s needs %s", hd.fn, hd.head), IDC_ERR_STATE;
+  if (n_img < 1) return snprintf(msg, cap, "%s: no forward has run on this context", hd.fn), IDC_ERR_STATE;
   if (q < 1 || q > IDC_MAX_RECCS_QUERIES || !queries)
-    return snprintf(msg, cap, "idc_ab_reccs_batch: need 1 <= q <= %d queries, got %d", IDC_MAX_RECCS_QUERIES, q), IDC_ERR_ARG;
+    return snprintf(msg, cap, "%s: need 1 <= q <= %d queries, got %d", hd.fn, IDC_MAX_RECCS_QUERIES, q), IDC_ERR_ARG;
   if (!reccs_args_ok(K, max_iter, n_init))
-    return snprintf(msg, cap, "idc_ab_reccs_batch: need 1 <= K <= 32, max_iter >= 1, 1 <= n_init <= %d", kReccsMaxInit),
+    return snprintf(msg, cap, "%s: need 1 <= K <= 32, max_iter >= 1, 1 <= n_init <= %d", hd.fn, kReccsMaxInit),
            IDC_ERR_ARG;
-  const int H4 = h / 4, W4 = w / 4;
+  const int GH = h / hd.div, GW = w / hd.div;
   for (int i = 0; i < q; ++i) {
     const int32_t* t = queries + 3 * (size_t)i;
     if (t[0] < 0 || t[0] >= n_img)
-      return snprintf(msg, cap, "idc_ab_reccs_batch: query %d: image %d outside the last forward's [0, %d)", i, t[0], n_img),
+      return snprintf(msg, cap, "%s: query %d: image %d outside the last forward's [0, %d)", hd.fn, i, t[0], n_img),
              IDC_ERR_ARG;
-    if (t[1] < 0 || t[1] >= H4 || t[2] < 0 || t[2] >= W4)
-      return snprintf(msg, cap, "idc_ab_reccs_batch: query %d: pixel (%d,%d) outside the %dx%d grid", i, t[1], t[2], H4, W4),
+    if (t[1] < 0 || t[1] >= GH || t[2] < 0 || t[2] >= GW)
+      return snprintf(msg, cap, "%s: query %d: pixel (%d,%d) outside the %dx%d grid", hd.fn, i, t[1], t[2], GH, GW),
              IDC_ERR_ARG;
   }
   return IDC_OK;
+}
+
+static int caffe313_reccs_check(bool head, int n_img, int h, int w, int q, const int32_t* queries, float S, int K,
+                                int max_iter, int n_init, char* msg, size_t cap) {
+  const int rc = reccs_batch_check(kReccsHead313, head, n_img, h, w, q, queries, K, max_iter, n_init, msg, cap);
+  if (rc == IDC_OK && !std::isfinite(S))
+    return snprintf(msg, cap, "%s: S = %g is not finite", kReccsHead313.fn, (double)S), IDC_ERR_ARG;
+  return rc;
+}
+
+// The context's batched-suggestion scratch, room for q queries.  Grows stream-ordered: neither the release nor the
+// allocation waits for the device.
+static cudaError_t reccs_batch_scratch(Ctx* c, int q, cudaStream_t st) {
+  if (q <= c->reccs_batch_q) return cudaSuccess;
+  if (c->d_reccs_batch.get()) {
+    const cudaError_t e = cudaFreeAsync(c->d_reccs_batch.release(), st);
+    if (e != cudaSuccess) return e;
+  }
+  c->reccs_batch_q = 0;
+  const cudaError_t e = cudaMallocAsync(reinterpret_cast<void**>(c->d_reccs_batch.put()), reccs_batch_scratch_bytes(q), st);
+  if (e == cudaSuccess) c->reccs_batch_q = q;
+  return e;
 }
 
 int idc_ab_reccs_batch(idc_ctx* c, int q, const int32_t* queries_host, int K, int max_iter, int n_init,
@@ -1461,17 +1493,13 @@ int idc_ab_reccs_batch(idc_ctx* c, int q, const int32_t* queries_host, int K, in
                        void* stream) {
   if (!c) return IDC_ERR_ARG;
   char msg[256];
-  const int rc = reccs_batch_check(c->dist, c->last_n, c->H, c->W, q, queries_host, K, max_iter, n_init, msg, sizeof(msg));
+  const int rc = reccs_batch_check(kReccsHead529, c->dist, c->last_n, c->H, c->W, q, queries_host, K, max_iter, n_init,
+                                   msg, sizeof(msg));
   if (rc != IDC_OK) return fail(c, rc, "%s", msg);
   if (!centers_dev) return fail(c, IDC_ERR_ARG, "idc_ab_reccs_batch: NULL centers");
   const cudaStream_t st = (cudaStream_t)stream;
   CUDA_TRY(c, cudaSetDevice(c->dev));
-  if (q > c->reccs_batch_q) {   // grow, stream-ordered: neither the release nor the allocation waits for the device
-    if (c->d_reccs_batch.get()) CUDA_TRY(c, cudaFreeAsync(c->d_reccs_batch.release(), st));
-    c->reccs_batch_q = 0;
-    CUDA_TRY(c, cudaMallocAsync(reinterpret_cast<void**>(c->d_reccs_batch.put()), reccs_batch_scratch_bytes(q), st));
-    c->reccs_batch_q = q;
-  }
+  CUDA_TRY(c, reccs_batch_scratch(c, q, st));
   CUDA_TRY(c, launch_reccs_batch(c, q, queries_host, pts_host, K, max_iter, n_init, c->d_reccs_batch.get(), centers_dev,
                                  conf_dev, iters_dev, pmf_dev, st));
   return IDC_OK;
@@ -1480,7 +1508,32 @@ int idc_ab_reccs_batch(idc_ctx* c, int q, const int32_t* queries_host, int K, in
 int idc_ab_reccs_batch_check(int has_head, int n_img, int h, int w, int q, const int32_t* queries, int K, int max_iter,
                              int n_init, char* msg, size_t msg_bytes) {
   char buf[256];
-  const int rc = reccs_batch_check(has_head != 0, n_img, h, w, q, queries, K, max_iter, n_init, buf, sizeof(buf));
+  const int rc = reccs_batch_check(kReccsHead529, has_head != 0, n_img, h, w, q, queries, K, max_iter, n_init, buf,
+                                   sizeof(buf));
+  if (rc != IDC_OK && msg && msg_bytes) snprintf(msg, msg_bytes, "%s", buf);
+  return rc;
+}
+
+int idc_caffe313_reccs_batch(idc_ctx* c, int q, const int32_t* queries_host, float S, int K, int max_iter, int n_init,
+                             float* centers_dev, float* conf_dev, int32_t* iters_dev, float* pmf_dev, void* stream) {
+  if (!c) return IDC_ERR_ARG;
+  char msg[256];
+  const int rc = caffe313_reccs_check(c->caffe313, c->last_n, c->H, c->W, q, queries_host, S, K, max_iter, n_init, msg,
+                                      sizeof(msg));
+  if (rc != IDC_OK) return fail(c, rc, "%s", msg);
+  if (!centers_dev) return fail(c, IDC_ERR_ARG, "idc_caffe313_reccs_batch: NULL centers");
+  const cudaStream_t st = (cudaStream_t)stream;
+  CUDA_TRY(c, cudaSetDevice(c->dev));
+  CUDA_TRY(c, reccs_batch_scratch(c, q, st));
+  CUDA_TRY(c, launch_caffe313_reccs_batch(c, q, queries_host, S, K, max_iter, n_init, c->d_reccs_batch.get(),
+                                          centers_dev, conf_dev, iters_dev, pmf_dev, st));
+  return IDC_OK;
+}
+
+int idc_caffe313_reccs_batch_check(int has_head, int n_img, int h, int w, int q, const int32_t* queries, float S, int K,
+                                   int max_iter, int n_init, char* msg, size_t msg_bytes) {
+  char buf[256];
+  const int rc = caffe313_reccs_check(has_head != 0, n_img, h, w, q, queries, S, K, max_iter, n_init, buf, sizeof(buf));
   if (rc != IDC_OK && msg && msg_bytes) snprintf(msg, msg_bytes, "%s", buf);
   return rc;
 }

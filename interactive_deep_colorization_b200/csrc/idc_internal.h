@@ -327,6 +327,11 @@ inline size_t reccs_batch_scratch_bytes(int q) {
 cudaError_t launch_reccs_batch(Ctx* c, int q, const int32_t* queries, const float* pts, int K, int max_iter, int n_init,
                                char* scratch, float* centers, float* conf, int32_t* iters, float* pmf_out,
                                cudaStream_t st);
+// idc_caffe313_reccs_batch on the device: the same scratch and outputs, queries (img, y, x) at full resolution, the pmf
+// of each query dist_ab_S of the 313-bin logits (zero-padded to 529), the points the context's pts313 (zero-padded)
+cudaError_t launch_caffe313_reccs_batch(Ctx* c, int q, const int32_t* queries, float S, int K, int max_iter, int n_init,
+                                        char* scratch, float* centers, float* conf, int32_t* iters, float* pmf_out,
+                                        cudaStream_t st);
 cudaError_t launch_global_stats(int h, int w, const uint8_t* rgb, const float* pts, float* out316, cudaStream_t st);
 cudaError_t launch_rgb2lab(int n, int h, int w, const uint8_t* rgb, double* lab, cudaStream_t st);
 cudaError_t launch_render_planes(const double* ab, int ab_order, int ab_f32, const double* mask, int mask_f32, int l_mode,

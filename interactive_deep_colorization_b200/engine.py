@@ -464,6 +464,30 @@ class LhnContext(object):
         _lib.check(self.h, self.lib.idc_caffe313_dist_map(self.h, int(n), float(S), out.data_ptr(), st))
         return out
 
+    def caffe313_reccs_batch(self, queries, K=5, S=0.2, max_iter=100, n_init=8, out=None, out_pmf=None):
+        """Colour suggestions of the 313-bin head at many full-resolution pixels of the last forward's images in one
+        device pass (idc_caffe313_reccs_batch): queries int [Q,3] rows (img, y, x) -> (centres [Q,K,2] float32, mass
+        [Q,K] float32, Lloyd iterations [Q] int32) torch CUDA tensors, asynchronous on torch's current stream.  Query i
+        equals ColorizeImageB200CaffeDist.get_ab_reccs(y, x, K)'s device k-means on the same forward bit for bit: the
+        pmf caffe313_dist_pixel(img, y, x, S) and the bin centres, both zero-padded to 529.  Needs caffe313=True.  out:
+        optional (centres, mass, iterations) tensors to write into (mass / iterations may be None).  out_pmf: optional
+        float32 CUDA tensor [Q,529] that receives each query's padded pmf."""
+        import torch
+        q = np.ascontiguousarray(queries, np.int32).reshape(-1, 3)
+        dev = torch.device("cuda:%d" % self.device)
+        if out is None:
+            n, k = q.shape[0], max(int(K), 0)
+            out = (torch.empty((n, k, 2), dtype=torch.float32, device=dev), torch.empty((n, k), dtype=torch.float32, device=dev),
+                   torch.empty((n,), dtype=torch.int32, device=dev))
+        centers, conf, iters = out
+        st = torch.cuda.current_stream(dev).cuda_stream
+        _lib.check(self.h, self.lib.idc_caffe313_reccs_batch(self.h, int(q.shape[0]), _np_ptr(q), float(S), int(K),
+                                                             int(max_iter), int(n_init), centers.data_ptr(),
+                                                             None if conf is None else conf.data_ptr(),
+                                                             None if iters is None else iters.data_ptr(),
+                                                             None if out_pmf is None else out_pmf.data_ptr(), st))
+        return centers, conf, iters
+
     def dist_negentropy(self, img=0):
         """sum_k d * log(d) over the 529 bins of the resident distribution of image img -> [H/4, W/4] float32 (the
         reference's compute_entropy statement before its x4 upsample); only this plane leaves the device."""

@@ -34,6 +34,9 @@ mask planes and glob rows.
 colours every photo with its hints as `colorize(hints=...)` does and also answers the GUI palette's question, the K
 colour suggestions get_ab_reccs(h, w, K) gives, at each photo's query points, on the distribution of that photo's own
 forward: the colorize pass with idc_ab_reccs_batch right after idc_forward (every query of the batch in one pass).
+A Caffe colorizer made with caffe_dist=True does the same with the checkpoint's 313-bin head, as the Caffe GUI pairs
+ColorizeImageCaffe with ColorizeImageCaffeDist on one checkpoint: the regression head gives the colour result and the
+313-bin logits of the same forward give each query's suggestions (idc_caffe313_reccs_batch, at full-resolution pixels).
 """
 import collections
 import concurrent.futures
@@ -173,6 +176,21 @@ def check_conditions(conditions, batch):
     return _check_one_pass(conditions, "condition", batch)
 
 
+# The Caffe distribution head's weights (include/idc_b200.h, IDC_FLAG_CAFFE313); caffe.pts_in_hull comes with the package.
+CAFFE313_KEYS = tuple("caffe.%s.%s" % (layer, p) for layer in ("conv3_pred", "conv4_pred", "conv5_pred", "conv6_pred",
+                                                               "conv7_pred", "conv8_pred", "pred_313")
+                      for p in ("weight", "bias"))
+CAFFE_DIST_S = 0.2            # dist_ab_S's softening, the S every caller of the Caffe distribution model passes (prep_net)
+
+
+def reccs_queries(points, caffe313):
+    """Per photo of a batch an int [P,2] array of (h, w) network pixels -> int32 [sum P, 3] queries, photo by photo:
+    (i, h, w) for the Caffe 313-bin head (its distribution is per pixel), (i, h // 4, w // 4) for the 529-bin head (one
+    distribution per 4 x 4 cell)."""
+    return np.concatenate([np.zeros((0, 3), np.int32)] + [
+        np.column_stack([np.full(len(p), i), p if caffe313 else p // 4]).astype(np.int32) for i, p in enumerate(points)])
+
+
 def read_photo(path):
     """A photo as `load_image` reads it: cv2.imread(path, 1), BGR -> RGB."""
     import cv2
@@ -243,27 +261,45 @@ class PhotoColorizer(object):
                 caffe_scaled_state_dict, option tanh_scale = 100); a hint's mask of 1 is then the reference's mask x 110.
                 Not with maskcent.
     suggest     the context also carries the 529-bin distribution head, for `suggest` (the head runs beside the colour
-                result and leaves it as it is).  Not with caffe or global_hints: their distribution models (313 bins,
-                global hints) have no batched suggestions."""
+                result and leaves it as it is).  Not with caffe (use caffe_dist) or global_hints (the global model has
+                no distribution head).
+    caffe_dist  with caffe: the context also carries the checkpoint's Caffe 313-bin distribution head (the caffe.* keys
+                of include/idc_b200.h), for `suggest`, as ColorizeImageB200CaffeDist loads it; the colour result still
+                comes from the regression head and is what caffe=True alone gives.  Not with global_hints."""
 
     def __init__(self, state_dict, Xd=256, batch=32, device=0, maskcent=False, global_hints=False, engine="wgmma",
-                 max_batch_bytes=96 << 20, readahead=None, workers=4, calibrate=None, caffe=False, suggest=False):
+                 max_batch_bytes=96 << 20, readahead=None, workers=4, calibrate=None, caffe=False, suggest=False,
+                 caffe_dist=False):
         if Xd < 8 or Xd % 8:
             raise ValueError("Xd must be a multiple of 8, got %d" % Xd)
         if not 1 <= batch <= _lib.MAX_PHOTOS:
             raise ValueError("batch must be in [1, %d], got %d" % (_lib.MAX_PHOTOS, batch))
         if caffe and maskcent:
             raise ValueError("caffe=True takes no maskcent: the Caffe models do not centre the mask")
-        if suggest and (caffe or global_hints):
-            raise ValueError("suggest=True works with the 529-bin distribution head only, not with %s"
-                             % ("caffe=True" if caffe else "global_hints=True"))
+        if suggest and caffe:
+            raise ValueError("suggest=True works with the 529-bin distribution head only; a Caffe checkpoint's "
+                             "suggestions come from its 313-bin head: use caffe_dist=True")
+        if suggest and global_hints:
+            raise ValueError("suggest=True works with the 529-bin distribution head only, not with global_hints=True")
+        if caffe_dist and not caffe:
+            raise ValueError("caffe_dist=True needs caffe=True: the 313-bin head belongs to the Caffe checkpoint")
+        if caffe_dist and global_hints:
+            raise ValueError("caffe_dist=True excludes global_hints=True: the global model has no 313-bin head")
+        if caffe_dist:
+            missing = [k for k in CAFFE313_KEYS if k not in state_dict]
+            if missing:
+                raise ValueError("caffe_dist=True needs the checkpoint's 313-bin head: it has no %r" % missing[0])
         self.Xd, self.batch, self.device = int(Xd), int(batch), int(device)
         self.maskcent, self.global_hints, self.engine = bool(maskcent), bool(global_hints), engine
-        self.caffe, self.dist = bool(caffe), bool(suggest)
+        self.caffe, self.dist, self.caffe_dist = bool(caffe), bool(suggest), bool(caffe_dist)
         self.options = {"tanh_scale": 100} if self.caffe else None
         if self.caffe:
             from .colorize_image import caffe_scaled_state_dict
             state_dict = caffe_scaled_state_dict(state_dict)
+        if self.caffe_dist:                      # the bin centres, as ColorizeImageB200Caffe.prep_net adds them
+            import torch
+            from .prepost import pts_in_hull
+            state_dict["caffe.pts_in_hull"] = torch.from_numpy(pts_in_hull())
         self.max_batch_bytes = int(max_batch_bytes)
         self.readahead = int(readahead) if readahead else 2 * self.batch
         self.workers = int(workers)
@@ -274,12 +310,12 @@ class PhotoColorizer(object):
         X, dev, glob = self.Xd, self.device, self.global_hints
         return engine.resolve_calibration(calibrate, lambda photos: engine.measure_act_ranges(
             state_dict, engine.calibration_batch(photos, X, device=dev, global_hints=glob), X, X, device=dev,
-            maskcent=0.5 if self.maskcent else 0.0, global_hints=glob, options=self.options))
+            maskcent=0.5 if self.maskcent else 0.0, global_hints=glob, caffe313=self.caffe_dist, options=self.options))
 
     def _make_backend(self, state_dict):
         return _DeviceBatches(state_dict, self.Xd, self.batch, self.device, 0.5 if self.maskcent else 0.0,
                               self.global_hints, self.engine, self.max_batch_bytes, self.act_ranges, self.options,
-                              self.dist)
+                              self.dist, self.caffe_dist)
 
     def colorize(self, photos, hints=None, glob=None, psnr=False):
         """photos: a sequence of paths (read as load_image reads them) or HxWx3 uint8 RGB arrays.
@@ -306,13 +342,14 @@ class PhotoColorizer(object):
         PhotoResult and, at each of its points (h, w) (network coordinates, 0 <= h, w < Xd), the K suggestions
         get_ab_reccs(h, w, K, return_conf=True) of the single-image distribution model gives after net_forward with
         the photo's hints (8 restarts, 100 Lloyd iterations, the PyTorch wrapper's gamut grid), read from the
-        distribution of the forward that used those hints.  Needs suggest=True.
+        distribution of the forward that used those hints.  Needs suggest=True, or caffe_dist=True: then the answers
+        are ColorizeImageB200CaffeDist's (the 313-bin dist_ab_S at pixel (h, w) with S = 0.2, the 313 bin centres).
         photos, hints: as colorize (hints may be None, or None per photo).  points: one int [P,2] array of (h, w) per
         photo (P may be 0).  K in [1, 32].
         -> iterator of SuggestResult, in input order.  Argument errors raise ValueError here, before any device work
         (paths as in colorize)."""
-        if not self.dist:
-            raise ValueError("suggest needs PhotoColorizer(suggest=True)")
+        if not (self.dist or self.caffe_dist):
+            raise ValueError("suggest needs PhotoColorizer(suggest=True), or caffe_dist=True with caffe=True")
         n = len(photos)
         if isinstance(K, (bool, np.bool_)) or not isinstance(K, (int, np.integer)) or not 1 <= K <= 32:
             raise ValueError("K must be an integer in [1, 32], got %r" % (K,))
@@ -487,12 +524,12 @@ class _DeviceBatches(object):
     the system, the device memory to torch's caching allocator)."""
 
     def __init__(self, state_dict, X, batch, device, maskcent, global_hints, engine_name, max_bytes, act_ranges=None,
-                 options=None, dist=False):
+                 options=None, dist=False, caffe313=False):
         import torch
         self.torch, self.lib = torch, _lib.load()
-        self.X, self.batch, self.device, self.maskcent = X, batch, device, maskcent
+        self.X, self.batch, self.device, self.maskcent, self.caffe313 = X, batch, device, maskcent, caffe313
         self.ctx = engine.LhnContext(device=device, max_n=batch, H=X, W=X, engine=engine_name, global_hints=global_hints,
-                                     options=options, dist=dist)
+                                     options=options, dist=dist, caffe313=caffe313)
         self.ctx.load_state_dict(state_dict, act_ranges=act_ranges)
         dev = self.dev = torch.device("cuda:%d" % device)
         f32 = torch.float32
@@ -630,9 +667,8 @@ class _DeviceBatches(object):
         n = len(photos)
         s, table, nbytes = self._next_slot(photos)
         queries = None
-        if points is not None:   # one query (photo of the batch, y4, x4) per point, photo by photo
-            queries = np.concatenate([np.zeros((0, 3), np.int32)] + [
-                np.column_stack([np.full(len(p), i), p // 4]).astype(np.int32) for i, p in enumerate(points)])
+        if points is not None:   # one query per point, photo by photo
+            queries = reccs_queries(points, self.caffe313)
             if len(queries):
                 self._reccs_buffers(s, len(queries) * K)
         count = 0
@@ -664,12 +700,15 @@ class _DeviceBatches(object):
             self.ctx.forward_device(self.L_mc[:n], self.ab_in[:n], self.mask[:n], self.maskcent,
                                     glob=None if glob is None else s["glob"][:n], want_rgb=True,
                                     out_ab=s["ab"][:n], out_rgb=s["rgb"][:n])
-            if queries is not None:        # on this forward's class logits, before the next forward replaces them
+            if queries is not None:        # on this forward's logits, before the next forward replaces them
                 Q, M = len(queries), _lib.MAX_RECCS_QUERIES
                 for q0 in range(0, Q, M):
                     q1 = min(q0 + M, Q)
-                    self.ctx.ab_reccs_batch(queries[q0:q1], K, out=(s["cen"][q0 * K:q1 * K].view(q1 - q0, K, 2),
-                                                                    s["conf"][q0 * K:q1 * K].view(q1 - q0, K), None))
+                    out = (s["cen"][q0 * K:q1 * K].view(q1 - q0, K, 2), s["conf"][q0 * K:q1 * K].view(q1 - q0, K), None)
+                    if self.caffe313:
+                        self.ctx.caffe313_reccs_batch(queries[q0:q1], K, S=CAFFE_DIST_S, out=out)
+                    else:
+                        self.ctx.ab_reccs_batch(queries[q0:q1], K, out=out)
             _lib.check(None, lib.idc_rgb2lab_f64(self.device, n, X, X, s["rgb"].data_ptr(), self.lab.data_ptr(), sh))
             _lib.check(None, lib.idc_photo_render(self.device, n, table.ctypes.data, s["src"].data_ptr(), X,
                                                   self.lab.data_ptr(), s["src"].data_ptr(), sh))

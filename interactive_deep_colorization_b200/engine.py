@@ -84,12 +84,8 @@ def calibration_batch(images, X, hints=8, seed=0, device=0, global_hints=False):
         raise ValueError("calibration needs 1 to %d photos, got %d" % (_lib.MAX_PHOTOS, n))
     dev = torch.device("cuda:%d" % device)
     st = torch.cuda.current_stream(dev).cuda_stream
-    table = np.zeros(n, _lib.PHOTO_DTYPE)
-    off = 0
-    for i, a in enumerate(imgs):
-        table[i] = (off, a.shape[0], a.shape[1])
-        off += a.shape[0] * a.shape[1]
-    src = torch.from_numpy(np.concatenate([a.reshape(-1) for a in imgs])).to(dev)
+    table, src = P.pack_photos(imgs)
+    src = torch.from_numpy(src).to(dev)
     L_mc = torch.empty((n, 1, X, X), dtype=torch.float32, device=dev)
     rgb = torch.empty((n, X, X, 3), dtype=torch.uint8, device=dev)
     lab = torch.empty((n, 3, X, X), dtype=torch.float64, device=dev)
@@ -97,22 +93,21 @@ def calibration_batch(images, X, hints=8, seed=0, device=0, global_hints=False):
     _lib.check(None, lib.idc_rgb2lab_f64(device, n, X, X, rgb.data_ptr(), lab.data_ptr(), st))
     own_ab = lab[:, 1:].cpu().numpy()
     rng = np.random.RandomState(seed)
-    rects = []
+    rects = [[] for _ in range(n)]
     for i in range(1, n, 2):
         for _ in range(hints):
             y, x, p = int(rng.randint(X)), int(rng.randint(X)), int(rng.randint(5))     # (2p+1)-pixel square, p = 0..4
-            rects.append((i, max(y - p, 0), max(x - p, 0), min(y + p, X - 1), min(x + p, X - 1),
-                          own_ab[i, 0, y, x], own_ab[i, 1, y, x]))
-    if len(rects) > _lib.MAX_HINTS:
-        raise ValueError("%d calibration hints, at most %d" % (len(rects), _lib.MAX_HINTS))
-    block = np.zeros(_lib.HINT_HDR_BYTES + len(rects) * _lib.HINT_DTYPE.itemsize, np.uint8)
-    block[:4].view(np.int32)[0] = len(rects)
-    if rects:
-        block[_lib.HINT_HDR_BYTES:] = as_hints(rects).view(np.uint8)
+            rects[i].append((i, max(y - p, 0), max(x - p, 0), min(y + p, X - 1), min(x + p, X - 1),
+                             own_ab[i, 0, y, x], own_ab[i, 1, y, x]))
+    count = sum(map(len, rects))
+    if count > _lib.MAX_HINTS:
+        raise ValueError("%d calibration hints, at most %d" % (count, _lib.MAX_HINTS))
+    block = np.empty(P.HINT_BLOCK_BYTES, np.uint8)
+    block = block[:P.pack_hints([as_hints(r) for r in rects], block)]
     d_block = torch.from_numpy(block).to(dev)
     ab = torch.empty((n, 2, X, X), dtype=torch.float32, device=dev)
     mask = torch.empty((n, 1, X, X), dtype=torch.float32, device=dev)
-    _lib.check(None, lib.idc_hint_raster(device, n, X, X, len(rects), d_block.data_ptr(), ab.data_ptr(), mask.data_ptr(), st))
+    _lib.check(None, lib.idc_hint_raster(device, n, X, X, count, d_block.data_ptr(), ab.data_ptr(), mask.data_ptr(), st))
     if not global_hints:
         return L_mc, ab, mask
     from . import prepost

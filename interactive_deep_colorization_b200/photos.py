@@ -43,6 +43,7 @@ import concurrent.futures
 import ctypes
 import math
 import os
+import weakref
 
 import numpy as np
 
@@ -242,6 +243,51 @@ def read_ahead(sources, load, depth, workers):
                 pending.append(pool.submit(load, s))
                 break
             yield r
+
+
+def pack_photos(imgs, out=None):
+    """HxWx3 uint8 photos -> (table, out): the idc_photo table of the batch (PHOTO_DTYPE [n]; photo i's first pixel
+    `off` comes right after photo i-1's last) and the photos packed back to back at those offsets into the uint8
+    buffer `out` (one of exactly their size when None)."""
+    if out is None:
+        out = np.empty(sum(a.nbytes for a in imgs), np.uint8)
+    table = np.zeros(len(imgs), _lib.PHOTO_DTYPE)
+    off = 0
+    for i, a in enumerate(imgs):
+        h, w = a.shape[:2]
+        table[i] = off, h, w
+        out[off * 3:(off + h * w) * 3] = a.reshape(-1)
+        off += h * w
+    return table, out
+
+
+HINT_BLOCK_BYTES = _lib.HINT_HDR_BYTES + _lib.MAX_HINTS * _lib.HINT_DTYPE.itemsize      # the largest hint block
+
+
+def pack_hints(hints, out, levels=None, stride=None):
+    """idc_hint_raster blocks, each a 16-byte header {count, 0, 0, 0} and then `count` idc_hint records (HINT_DTYPE),
+    written into the uint8 buffer `out` -> the length of one block.
+    Without levels, one block: hints holds one hint list (or None) per image of a batch, and each record gets its
+    list's position as `img`; no lists, or only empty ones, make an empty block.
+    With levels, len(hints) * len(levels) blocks `stride` bytes apart: block i * len(levels) + j holds the first
+    levels[j] records of hints[i] as they are.  The default stride is the header plus max(levels) records, rounded up
+    to 16 bytes; -> the stride."""
+    hdr, rec = _lib.HINT_HDR_BYTES, _lib.HINT_DTYPE.itemsize
+    if levels is None:
+        lists = [np.zeros(0, _lib.HINT_DTYPE) if h is None else h for h in hints]
+        block = np.concatenate([np.zeros(0, _lib.HINT_DTYPE)] + lists)
+        block["img"] = np.repeat(np.arange(len(lists)), [len(h) for h in lists])
+        out[:hdr].view(np.int32)[:] = len(block), 0, 0, 0
+        out[hdr:hdr + block.nbytes] = block.view(np.uint8)
+        return hdr + block.nbytes
+    if stride is None:
+        stride = hdr + (max(levels) * rec + 15) // 16 * 16
+    raw = np.stack(hints).view(np.uint8)
+    blocks = out[:len(raw) * len(levels) * stride].reshape(len(raw), len(levels), stride)
+    blocks[:, :, :hdr].view(np.int32)[:] = [(c, 0, 0, 0) for c in levels]
+    for j, c in enumerate(levels):
+        blocks[:, j, hdr:hdr + c * rec] = raw[:, :c * rec]
+    return stride
 
 
 class PhotoColorizer(object):
@@ -490,22 +536,106 @@ class PhotoColorizer(object):
 
 
 class _HostBuffer(object):
-    """Page-locked host bytes from idc_host_alloc, seen as a numpy array and a torch tensor; free() returns them to the
-    system (torch's own pinned allocator would keep them cached for the life of the process)."""
+    """Page-locked host bytes from idc_host_alloc, seen as a torch tensor; free() returns them to the system (torch's
+    own pinned allocator would keep them cached for the life of the process)."""
 
     def __init__(self, lib, nbytes):
         import torch
         self.lib, self.ptr = lib, lib.idc_host_alloc(nbytes)
         if not self.ptr:
             raise _lib.IdcError(-2, "idc_host_alloc(%d) failed" % nbytes)
-        self.array = np.frombuffer((ctypes.c_char * nbytes).from_address(self.ptr), dtype=np.uint8)
-        self.tensor = torch.from_numpy(self.array)
+        self.tensor = torch.from_numpy(np.frombuffer((ctypes.c_char * nbytes).from_address(self.ptr), dtype=np.uint8))
 
     def free(self):
         if self.ptr:
-            self.array = self.tensor = None
+            self.tensor = None
             self.lib.idc_host_free(self.ptr)
             self.ptr = None
+
+
+class _Twin(object):
+    """A buffer of _DeviceBatches: `rows` rows of shape `row` on the device and, as HostStaging pairs them on the C
+    side, page-locked host copies of the same layout (_HostBuffer).  hosts=1: h_in and h_out are one copy; hosts=2:
+    the device rows are uploaded from h_in and downloaded into h_out; hosts=0: device only."""
+
+    def __init__(self, owner, row, dtype, rows=0, hosts=1, init=None):
+        self.owner = weakref.proxy(owner)           # no cycle: the buffers go when their _DeviceBatches does
+        self.row, self.dtype, self.hosts = tuple(row), dtype, hosts
+        self.rows, self.dev, self.h_in, self.h_out, self._bufs = 0, None, None, None, ()
+        self.grow(rows, init=init)
+
+    def grow(self, rows, cap=None, init=None):
+        """Room for `rows` rows, allocated again only while no enqueued work uses the buffer.  With cap the buffer
+        holds exactly cap rows whenever rows fits in cap (so a buffer grown past cap shrinks back) and exactly `rows`
+        otherwise.  Without cap it only grows: to exactly `rows` on the device, while its host copies, once they have
+        to grow, at least double, so that a buffer that grows batch by batch seldom frees page-locked memory
+        (idc_host_free waits for the whole device).  init: a host array the new device rows are copied from.  Every
+        buffer of _DeviceBatches is allocated here, and the pipeline's streams are ordered after it."""
+        if cap is not None and rows <= cap:
+            if self.rows == cap:
+                return
+            rows = cap
+        elif self.rows >= rows:
+            return
+        o, torch = self.owner, self.owner.torch
+        self.dev = None
+        if init is None:
+            self.dev = torch.empty((rows,) + self.row, dtype=self.dtype, device=o.dev)
+        else:
+            self.dev = torch.from_numpy(init).to(o.dev)
+        nbytes = self.dev.numel() * self.dev.element_size()
+        have = self._bufs[0].tensor.numel() if self._bufs else 0
+        if cap is not None or have < nbytes:
+            for b in self._bufs:
+                b.free()
+            size = nbytes if cap is not None or not have else max(nbytes, 2 * have)
+            self._bufs = tuple(_HostBuffer(o.lib, size) for _ in range(self.hosts))
+        views = [b.tensor[:nbytes].view(self.dtype).view(self.dev.shape) for b in self._bufs]
+        if views:
+            self.h_in, self.h_out = views[0], views[-1]
+        self.rows = rows
+        o._after_alloc()
+
+    def upload(self, n):
+        self.dev[:n].copy_(self.h_in[:n], non_blocking=True)
+
+    def download(self, n):
+        self.h_out[:n].copy_(self.dev[:n], non_blocking=True)
+
+    def free(self):
+        """Return the host copies to the system and the device rows to torch's caching allocator."""
+        for b in self._bufs:
+            b.free()
+        self.rows, self.dev, self.h_in, self.h_out, self._bufs = 0, None, None, None, ()
+
+
+class _Slot(object):
+    """One of the two buffer sets of _DeviceBatches, with the events of the batch in it.  The buffers of a pass kind
+    that not every colorizer runs start empty and grow on the first batch that needs them."""
+
+    def __init__(self, b):
+        torch, X, n = b.torch, b.X, b.batch
+        u8, f32 = torch.uint8, torch.float32
+        self.serial = 0                                   # serial number of the batch the slot holds
+        # the packed photos, uploaded from h_in, rendered over in place and downloaded into h_out: max_bytes, or more
+        # for the one batch of a larger photo
+        self.src = _Twin(b, (), u8, hosts=2)
+        self.hints = _Twin(b, (), u8, HINT_BLOCK_BYTES)
+        self.glob = _Twin(b, (316,), f32, n)
+        self.img_rgb = _Twin(b, (X, X, 3), u8, n, hosts=0)
+        self.ab = _Twin(b, (2, X, X), f32, n)
+        self.rgb = _Twin(b, (X, X, 3), u8, n)
+        self.sse = _Twin(b, (), torch.int64, n)
+        self.stats = _Twin(b, (316,), f32, n)
+        self.cen = _Twin(b, (2,), f32)                    # suggest: queries x K centres and their masses
+        self.conf = _Twin(b, (), f32)
+        self.blocks = _Twin(b, (), u8)                    # reveal sweeps: one hint block per forward image
+        self.ev_in, self.ev_comp, self.ev_out = (torch.cuda.Event() for _ in range(3))
+
+    def free(self):
+        for t in vars(self).values():
+            if isinstance(t, _Twin):
+                t.free()
 
 
 # What a _DeviceBatches submit returns and its collect takes: the slot, the serial number of the batch in it, the
@@ -514,38 +644,38 @@ _Batch = collections.namedtuple("_Batch", "slot serial n V info")
 
 
 class _DeviceBatches(object):
-    """Device side of PhotoColorizer: one LhnContext (max_n = batch) and two slots of batch buffers.  submit() packs and
-    enqueues a batch on slot k % 2 and returns; collect() waits for that batch's copies and returns its results.
+    """Device side of PhotoColorizer: one LhnContext (max_n = batch) and two _Slots of batch buffers.  submit() packs
+    and enqueues a batch on slot k % 2 and returns; collect() waits for that batch's copies and returns its results.
     submit() first waits until the slot's previous batch is off the device, so a slot is never overwritten while a
     kernel or a copy still uses it, whether or not that batch was collected; collecting a batch whose slot has been
     reused since raises instead of returning another batch's pixels.
     The source / result buffers of a slot hold max_bytes; a batch of one larger photo grows them for that batch, and
-    the slot's next batch that fits, or close(), returns them to max_bytes (the page-locked host memory goes back to
-    the system, the device memory to torch's caching allocator)."""
+    the slot's next batch that fits returns them to max_bytes.  close() returns every page-locked buffer to the system
+    and the device memory to torch's caching allocator."""
 
     def __init__(self, state_dict, X, batch, device, maskcent, global_hints, engine_name, max_bytes, act_ranges=None,
                  options=None, dist=False, caffe313=False):
         import torch
+        from . import prepost
         self.torch, self.lib = torch, _lib.load()
         self.X, self.batch, self.device, self.maskcent, self.caffe313 = X, batch, device, maskcent, caffe313
         self.ctx = engine.LhnContext(device=device, max_n=batch, H=X, W=X, engine=engine_name, global_hints=global_hints,
                                      options=options, dist=dist, caffe313=caffe313)
         self.ctx.load_state_dict(state_dict, act_ranges=act_ranges)
-        dev = self.dev = torch.device("cuda:%d" % device)
+        self.dev = torch.device("cuda:%d" % device)
+        self.s_in, self.s_comp, self.s_out = (torch.cuda.Stream(self.dev) for _ in range(3))
         f32 = torch.float32
         # used by the compute stream only: one copy
-        self.L_mc = torch.empty((batch, 1, X, X), dtype=f32, device=dev)
-        self.ab_in = torch.empty((batch, 2, X, X), dtype=f32, device=dev)
-        self.mask = torch.empty((batch, 1, X, X), dtype=f32, device=dev)
-        self.lab = torch.empty((batch, 3, X, X), dtype=torch.float64, device=dev)
-        from . import prepost
-        self.pts313 = torch.from_numpy(prepost.pts_in_hull()).to(dev)        # the 313 ab bin centres
-        self._keep = {}                                                       # conditions -> _glob_keep's masks
-        self.zero = torch.zeros((), dtype=f32, device=dev)
+        self.L_mc, self.ab_in, self.mask = (_Twin(self, (c, X, X), f32, batch, hosts=0).dev for c in (1, 2, 1))
+        self.lab = _Twin(self, (3, X, X), torch.float64, batch, hosts=0).dev
+        # a sweep's prepared photos before they are repeated per level or condition, made on the first sweep
+        self.L_photo = _Twin(self, (1, X, X), f32, hosts=0)
+        self.rgb_photo = _Twin(self, (X, X, 3), torch.uint8, hosts=0)
+        self.pts313 = _Twin(self, (2,), f32, 313, hosts=0, init=prepost.pts_in_hull()).dev    # the 313 ab bin centres
+        self.zero = _Twin(self, (), f32, 1, hosts=0, init=np.zeros(1, np.float32)).dev[0]
+        self.keep = {}                          # conditions -> [C,316] bool: the entries each keeps (_GLOB_KEEP)
         self.max_bytes = max_bytes
-        self.slots = [self._slot() for _ in range(2)]
-        self.s_in, self.s_comp, self.s_out = (torch.cuda.Stream(dev) for _ in range(3))
-        self._after_alloc()
+        self.slots = [_Slot(self) for _ in range(2)]
         self.k = 0
 
     def _after_alloc(self):
@@ -555,91 +685,48 @@ class _DeviceBatches(object):
         for st in (self.s_in, self.s_comp, self.s_out):
             st.wait_stream(cur)
 
-    def _slot(self):
-        torch, X, n, dev = self.torch, self.X, self.batch, self.dev
-        pin = lambda shape, dt: torch.empty(shape, dtype=dt, pin_memory=True)
-        hint_bytes = _lib.HINT_HDR_BYTES + _lib.MAX_HINTS * _lib.HINT_DTYPE.itemsize
-        return {"cap": 0, "batch": 0,                                # batch: serial number of the batch the slot holds
-                "src": None, "h_src": None, "h_full": None,      # sized by _reserve
-                "hints": torch.empty((hint_bytes,), dtype=torch.uint8, device=dev), "h_hints": pin((hint_bytes,), torch.uint8),
-                "glob": torch.empty((n, 316), dtype=torch.float32, device=dev), "h_glob": pin((n, 316), torch.float32),
-                "img_rgb": torch.empty((n, X, X, 3), dtype=torch.uint8, device=dev),
-                "ab": torch.empty((n, 2, X, X), dtype=torch.float32, device=dev), "h_ab": pin((n, 2, X, X), torch.float32),
-                "rgb": torch.empty((n, X, X, 3), dtype=torch.uint8, device=dev), "h_rgb": pin((n, X, X, 3), torch.uint8),
-                "sse": torch.empty((n,), dtype=torch.int64, device=dev), "h_sse": pin((n,), torch.int64),
-                "stats": torch.empty((n, 316), dtype=torch.float32, device=dev), "h_stats": pin((n, 316), torch.float32),
-                "ev_in": torch.cuda.Event(), "ev_comp": torch.cuda.Event(), "ev_out": torch.cuda.Event()}
-
-    def _free_big(self, s):
-        for k in ("h_src", "h_full"):
-            if s[k] is not None:
-                s[k].free()
-        s["src"] = s["h_src"] = s["h_full"] = None
-        s["cap"] = 0
-
-    def _reserve(self, s, nbytes):
-        """Source / result buffers of slot s for nbytes: max_bytes, or exactly nbytes for a larger batch.  The slot is
-        idle (submit waited for it)."""
-        if s["cap"] >= nbytes and (s["cap"] == self.max_bytes or nbytes > self.max_bytes):
-            return
-        cap = max(nbytes, self.max_bytes)
-        self._free_big(s)
-        s["src"] = self.torch.empty((cap,), dtype=self.torch.uint8, device=self.dev)
-        s["h_src"], s["h_full"] = _HostBuffer(self.lib, cap), _HostBuffer(self.lib, cap)
-        s["cap"] = cap
-        self._after_alloc()
-
     def _next_slot(self, photos):
         """The next slot, once its previous batch (if any) is off the device: render, D2H, all; the batch's photo table,
         and the photos packed back to back into the slot's page-locked source buffer -> (slot, table, nbytes)."""
         s = self.slots[self.k % 2]
         self.k += 1
-        s["ev_out"].synchronize()
-        s["batch"] = self.k
-        table = np.zeros(len(photos), _lib.PHOTO_DTYPE)
-        off = 0
-        for i, a in enumerate(photos):
-            table[i] = (off, a.shape[0], a.shape[1])
-            off += a.shape[0] * a.shape[1]
-        nbytes = off * 3
-        self._reserve(s, nbytes)
-        h_src = s["h_src"].array
-        for i, a in enumerate(photos):
-            o = int(table[i]["off"]) * 3
-            h_src[o:o + a.nbytes] = a.reshape(-1)
-        return s, table, nbytes
+        s.ev_out.synchronize()
+        s.serial = self.k
+        nbytes = sum(a.nbytes for a in photos)
+        s.src.grow(nbytes, cap=self.max_bytes)
+        return s, pack_photos(photos, s.src.h_in.numpy())[0], nbytes
 
-    def _upload_photos(self, s, nbytes, pairs=()):
-        """H2D of the packed photos and the (device, host) pairs on the copy stream; the compute stream waits for it."""
+    def _upload_photos(self, s, nbytes, *bufs):
+        """H2D of the packed photos and of the first rows of each (buffer, rows) on the copy stream; the compute stream
+        waits for it."""
         with self.torch.cuda.stream(self.s_in):
-            s["src"][:nbytes].copy_(s["h_src"].tensor[:nbytes], non_blocking=True)
-            for d, h in pairs:
-                d.copy_(h, non_blocking=True)
-            s["ev_in"].record(self.s_in)
-        self.s_comp.wait_event(s["ev_in"])
+            for t, n in ((s.src, nbytes),) + bufs:
+                t.upload(n)
+            s.ev_in.record(self.s_in)
+        self.s_comp.wait_event(s.ev_in)
 
-    def _download(self, s, pairs):
-        """After the work enqueued on the compute stream so far: D2H of the (device, host) pairs on the copy stream,
-        then ev_out, which the slot's next batch and the collect wait for."""
-        s["ev_comp"].record(self.s_comp)
+    def _download(self, s, *bufs):
+        """After the work enqueued on the compute stream so far: D2H of the first rows of each (buffer, rows) on the
+        copy stream, then ev_out, which the slot's next batch and the collect wait for."""
+        s.ev_comp.record(self.s_comp)
         with self.torch.cuda.stream(self.s_out):
-            self.s_out.wait_event(s["ev_comp"])
-            for d, h in pairs:
-                h.copy_(d, non_blocking=True)
-            s["ev_out"].record(self.s_out)
+            self.s_out.wait_event(s.ev_comp)
+            for t, n in bufs:
+                t.download(n)
+            s.ev_out.record(self.s_out)
 
     def _finish(self, token):
         """Wait for a submitted batch's D2H -> its slot.  Raise if the slot has taken a later batch since."""
         s = token.slot
-        if s["batch"] != token.serial:
+        if s.serial != token.serial:
             raise RuntimeError("this batch's buffers were reused by a later batch: iterate one result iterator at a "
                                "time per PhotoColorizer")
-        s["ev_out"].synchronize()
+        s.ev_out.synchronize()
         return s
 
     def _prep(self, s, n, table, L, rgb):
         """idc_photo_prep of the slot's n photos into L [n,1,X,X] and, unless rgb is None, rgb [n,X,X,3]."""
-        _lib.check(None, self.lib.idc_photo_prep(self.device, n, table.ctypes.data, s["src"].data_ptr(), self.X,
+        _lib.check(None, self.lib.idc_photo_prep(self.device, n, table.ctypes.data, s.src.dev.data_ptr(), self.X,
                                                  L.data_ptr(), None if rgb is None else rgb.data_ptr(),
                                                  self.s_comp.cuda_stream))
 
@@ -647,155 +734,102 @@ class _DeviceBatches(object):
         """_prep, then each photo's [316] statistics row from rgb into the slot's stats (idc_global_stats_batch)."""
         self._prep(s, n, table, L, rgb)
         _lib.check(None, self.lib.idc_global_stats_batch(self.device, n, self.X, self.X, rgb.data_ptr(),
-                                                         self.pts313.data_ptr(), s["stats"].data_ptr(),
+                                                         self.pts313.data_ptr(), s.stats.dev.data_ptr(),
                                                          self.s_comp.cuda_stream))
-
-    def _reccs_buffers(self, s, size):
-        """Slot s's suggestion outputs, room for `size` centres (queries x K): device and page-locked host.  The slot is
-        idle (submit waited for it)."""
-        if s.get("rc_cap", 0) < size:
-            torch, dev = self.torch, self.dev
-            s["cen"] = torch.empty((size, 2), dtype=torch.float32, device=dev)
-            s["conf"] = torch.empty((size,), dtype=torch.float32, device=dev)
-            s["h_cen"] = torch.empty((size, 2), dtype=torch.float32, pin_memory=True)
-            s["h_conf"] = torch.empty((size,), dtype=torch.float32, pin_memory=True)
-            s["rc_cap"] = size
-            self._after_alloc()
 
     def submit(self, photos, hints, glob, psnr, points=None, K=0):
         torch, lib, X = self.torch, self.lib, self.X
         n = len(photos)
         s, table, nbytes = self._next_slot(photos)
-        queries = None
-        if points is not None:   # one query per point, photo by photo
-            queries = reccs_queries(points, self.caffe313)
-            if len(queries):
-                self._reccs_buffers(s, len(queries) * K)
-        count = 0
-        if hints is not None:
-            lists = []
-            for i, h in enumerate(hints):
-                if h is not None and h.shape[0]:
-                    h = h.copy()
-                    h["img"] = i
-                    lists.append(h)
-            block = np.concatenate(lists) if lists else np.zeros(0, _lib.HINT_DTYPE)
-            count = block.shape[0]
-        hb = s["h_hints"].numpy()
-        hb[:_lib.HINT_HDR_BYTES].view(np.int32)[:] = (count, 0, 0, 0)
-        if count:
-            hb[_lib.HINT_HDR_BYTES:_lib.HINT_HDR_BYTES + block.nbytes] = block.view(np.uint8)
+        queries = None if points is None else reccs_queries(points, self.caffe313)    # one per point, photo by photo
+        QK = 0 if queries is None else len(queries) * K
+        s.cen.grow(QK)
+        s.conf.grow(QK)
+        hints = hints or []
+        count = sum(len(h) for h in hints if h is not None)
+        up = [(s.hints, pack_hints(hints, s.hints.h_in.numpy()))]
         if glob is not None:
-            s["h_glob"].numpy()[:n] = np.stack(glob)
-        hint_len = _lib.HINT_HDR_BYTES + count * _lib.HINT_DTYPE.itemsize
-        self._upload_photos(s, nbytes, [(s["hints"][:hint_len], s["h_hints"][:hint_len])]
-                            + ([] if glob is None else [(s["glob"][:n], s["h_glob"][:n])]))
+            s.glob.h_in.numpy()[:n] = np.stack(glob)
+            up.append((s.glob, n))
+        self._upload_photos(s, nbytes, *up)
 
         st = self.s_comp
         sh = st.cuda_stream
         with torch.cuda.stream(st):
-            self._prep(s, n, table, self.L_mc, s["img_rgb"] if psnr else None)
-            _lib.check(None, lib.idc_hint_raster(self.device, n, X, X, count, s["hints"].data_ptr(), self.ab_in.data_ptr(),
-                                                 self.mask.data_ptr(), sh))
+            self._prep(s, n, table, self.L_mc, s.img_rgb.dev if psnr else None)
+            _lib.check(None, lib.idc_hint_raster(self.device, n, X, X, count, s.hints.dev.data_ptr(),
+                                                 self.ab_in.data_ptr(), self.mask.data_ptr(), sh))
             self.ctx.forward_device(self.L_mc[:n], self.ab_in[:n], self.mask[:n], self.maskcent,
-                                    glob=None if glob is None else s["glob"][:n], want_rgb=True,
-                                    out_ab=s["ab"][:n], out_rgb=s["rgb"][:n])
+                                    glob=None if glob is None else s.glob.dev[:n], want_rgb=True,
+                                    out_ab=s.ab.dev[:n], out_rgb=s.rgb.dev[:n])
             if queries is not None:        # on this forward's logits, before the next forward replaces them
                 Q, M = len(queries), _lib.MAX_RECCS_QUERIES
                 for q0 in range(0, Q, M):
                     q1 = min(q0 + M, Q)
-                    out = (s["cen"][q0 * K:q1 * K].view(q1 - q0, K, 2), s["conf"][q0 * K:q1 * K].view(q1 - q0, K), None)
+                    out = (s.cen.dev[q0 * K:q1 * K].view(q1 - q0, K, 2), s.conf.dev[q0 * K:q1 * K].view(q1 - q0, K),
+                           None)
                     if self.caffe313:
                         self.ctx.caffe313_reccs_batch(queries[q0:q1], K, S=CAFFE_DIST_S, out=out)
                     else:
                         self.ctx.ab_reccs_batch(queries[q0:q1], K, out=out)
-            _lib.check(None, lib.idc_rgb2lab_f64(self.device, n, X, X, s["rgb"].data_ptr(), self.lab.data_ptr(), sh))
-            _lib.check(None, lib.idc_photo_render(self.device, n, table.ctypes.data, s["src"].data_ptr(), X,
-                                                  self.lab.data_ptr(), s["src"].data_ptr(), sh))
+            _lib.check(None, lib.idc_rgb2lab_f64(self.device, n, X, X, s.rgb.dev.data_ptr(), self.lab.data_ptr(), sh))
+            _lib.check(None, lib.idc_photo_render(self.device, n, table.ctypes.data, s.src.dev.data_ptr(), X,
+                                                  self.lab.data_ptr(), s.src.dev.data_ptr(), sh))
             if psnr:
-                _lib.check(None, lib.idc_rgb_sse(self.device, n, X, X, s["img_rgb"].data_ptr(), s["rgb"].data_ptr(),
-                                                 s["sse"].data_ptr(), sh))
+                _lib.check(None, lib.idc_rgb_sse(self.device, n, X, X, s.img_rgb.dev.data_ptr(), s.rgb.dev.data_ptr(),
+                                                 s.sse.dev.data_ptr(), sh))
 
-        pairs = [(s["src"][:nbytes], s["h_full"].tensor[:nbytes]), (s["ab"][:n], s["h_ab"][:n]),
-                 (s["rgb"][:n], s["h_rgb"][:n])]
+        down = [(s.src, nbytes), (s.ab, n), (s.rgb, n)]
         if psnr:
-            pairs.append((s["sse"][:n], s["h_sse"][:n]))
-        if queries is not None and len(queries):
-            QK = len(queries) * K
-            pairs += [(s["cen"][:QK], s["h_cen"][:QK]), (s["conf"][:QK], s["h_conf"][:QK])]
-        self._download(s, pairs)
-        return _Batch(s, s["batch"], n, 1, (table, psnr, None if points is None else [len(p) for p in points], K))
+            down.append((s.sse, n))
+        if QK:
+            down += [(s.cen, QK), (s.conf, QK)]
+        self._download(s, *down)
+        return _Batch(s, s.serial, n, 1, (table, psnr, None if points is None else [len(p) for p in points], K))
 
     def collect(self, token):
         s = self._finish(token)
         table, psnr, counts, K = token.info
-        full, ab, rgb, sse = s["h_full"].array, s["h_ab"].numpy(), s["h_rgb"].numpy(), s["h_sse"].numpy()
+        full, ab, rgb, sse = (t.h_out.numpy() for t in (s.src, s.ab, s.rgb, s.sse))
         out = [PhotoResult(full[off * 3:(off + h * w) * 3].reshape(h, w, 3).copy(), rgb[i].copy(), ab[i].copy(),
                            _psnr(sse[i], self.X) if psnr else None)
                for i, (off, h, w) in enumerate(table.tolist())]
         if counts is None:
             return out
         Q = sum(counts)
-        cen = s["h_cen"].numpy()[:Q * K].reshape(Q, K, 2) if Q else np.zeros((0, K, 2), np.float32)
-        conf = s["h_conf"].numpy()[:Q * K].reshape(Q, K) if Q else np.zeros((0, K), np.float32)
+        cen = s.cen.h_out.numpy()[:Q * K].reshape(Q, K, 2) if Q else np.zeros((0, K, 2), np.float32)
+        conf = s.conf.h_out.numpy()[:Q * K].reshape(Q, K) if Q else np.zeros((0, K), np.float32)
         ends = np.cumsum(counts)
         # float64 like get_ab_reccs (centers.astype(np.float64), conf.astype(np.float64))
         return [SuggestResult(r, cen[e - c:e].astype(np.float64), conf[e - c:e].astype(np.float64))
                 for r, c, e in zip(out, counts, ends)]
 
-    def _photo_buffers(self):
-        """The prepared photos of a sweep before they are repeated per level or condition (compute stream only, one
-        copy), made on the first sweep."""
-        if getattr(self, "L_photo", None) is None:
-            torch, X, n, dev = self.torch, self.X, self.batch, self.dev
-            self.L_photo = torch.empty((n, 1, X, X), dtype=torch.float32, device=dev)
-            self.rgb_photo = torch.empty((n, X, X, 3), dtype=torch.uint8, device=dev)
-            self._after_alloc()
-
-    def _reveal_buffers(self):
-        """Buffers of reveal sweeps, made on the first one: _photo_buffers and, per slot, room for `batch` hint blocks
-        of IDC_MAX_HINTS hints each."""
-        self._photo_buffers()
-        if "blocks" not in self.slots[0]:
-            torch, n, dev = self.torch, self.batch, self.dev
-            nb = n * (_lib.HINT_HDR_BYTES + _lib.MAX_HINTS * _lib.HINT_DTYPE.itemsize)
-            for s in self.slots:
-                s["blocks"] = torch.empty((nb,), dtype=torch.uint8, device=dev)
-                s["h_blocks"] = torch.empty((nb,), dtype=torch.uint8, pin_memory=True)
-            self._after_alloc()
-
-    def _glob_keep(self, conditions):
-        """[C,316] bool device tensor: the entries of a statistics row each condition keeps (_GLOB_KEEP)."""
-        if conditions not in self._keep:
-            self._keep[conditions] = self.torch.from_numpy(np.stack([_GLOB_KEEP[c] for c in conditions])).to(self.dev)
-            self._after_alloc()
-        return self._keep[conditions]
-
     def _submit_sweep(self, photos, V, fill):
         """One device pass of a sweep: photo i of the batch is forward images i*V .. i*V+V-1 (V variants: the levels or
         the conditions), each with the photo's prepared L and img_rgb.  fill(s, m, table, nbytes) uploads the batch,
         preps its m photos into L_photo / rgb_photo and makes the forward's ab / mask planes on the compute stream; it
-        returns the forward's glob rows (or None) and the (device, host) pairs it adds to the D2H of ab, rgb and SSE."""
+        returns the forward's glob rows (or None) and the (buffer, rows) it adds to the D2H of ab, rgb and SSE."""
         torch, lib, X = self.torch, self.lib, self.X
         m = len(photos)
         N = m * V
+        self.L_photo.grow(self.batch)
+        self.rgb_photo.grow(self.batch)
         s, table, nbytes = self._next_slot(photos)
         glob, extra = fill(s, m, table, nbytes)
         with torch.cuda.stream(self.s_comp):
-            self.L_mc[:N].view(m, V, 1, X, X).copy_(self.L_photo[:m, None].expand(m, V, 1, X, X))
-            s["img_rgb"][:N].view(m, V, X, X, 3).copy_(self.rgb_photo[:m, None].expand(m, V, X, X, 3))
+            self.L_mc[:N].view(m, V, 1, X, X).copy_(self.L_photo.dev[:m, None].expand(m, V, 1, X, X))
+            s.img_rgb.dev[:N].view(m, V, X, X, 3).copy_(self.rgb_photo.dev[:m, None].expand(m, V, X, X, 3))
             self.ctx.forward_device(self.L_mc[:N], self.ab_in[:N], self.mask[:N], self.maskcent, glob=glob,
-                                    want_rgb=True, out_ab=s["ab"][:N], out_rgb=s["rgb"][:N])
-            _lib.check(None, lib.idc_rgb_sse(self.device, N, X, X, s["img_rgb"].data_ptr(), s["rgb"].data_ptr(),
-                                             s["sse"].data_ptr(), self.s_comp.cuda_stream))
-        self._download(s, [(s["ab"][:N], s["h_ab"][:N]), (s["rgb"][:N], s["h_rgb"][:N]),
-                           (s["sse"][:N], s["h_sse"][:N])] + extra)
-        return _Batch(s, s["batch"], m, V, None)
+                                    want_rgb=True, out_ab=s.ab.dev[:N], out_rgb=s.rgb.dev[:N])
+            _lib.check(None, lib.idc_rgb_sse(self.device, N, X, X, s.img_rgb.dev.data_ptr(), s.rgb.dev.data_ptr(),
+                                             s.sse.dev.data_ptr(), self.s_comp.cuda_stream))
+        self._download(s, (s.ab, N), (s.rgb, N), (s.sse, N), *extra)
+        return _Batch(s, s.serial, m, V, None)
 
     def _collect_sweep(self, token):
         """A sweep's results -> per photo (psnr float64 [V], ab float32 [V,2,X,X], rgb uint8 [V,X,X,3])."""
         s, V = self._finish(token), token.V
-        ab, rgb, sse = s["h_ab"].numpy(), s["h_rgb"].numpy(), s["h_sse"].numpy()
+        ab, rgb, sse = (t.h_out.numpy() for t in (s.ab, s.rgb, s.sse))
         out = []
         for i in range(token.n):
             k = slice(i * V, (i + 1) * V)
@@ -806,27 +840,20 @@ class _DeviceBatches(object):
         """One device pass of a reveal sweep: image i*L+j of the sweep (L = len(levels)) has the first levels[j] rows of
         points[i] as hints, coloured with the mean ground-truth ab under each (idc_hint_fill_mean)."""
         lib, X, L = self.lib, self.X, len(levels)
-        self._reveal_buffers()
-        # hint blocks, one per forward image, in idc_hint_raster's layout; the colours are filled on the device
-        stride = _lib.HINT_HDR_BYTES + (max(levels) * _lib.HINT_DTYPE.itemsize + 15) // 16 * 16
+        # the points as hint rectangles; their colours are filled on the device
+        pts = np.stack(points)
+        rects = np.zeros(pts.shape[:2], _lib.HINT_DTYPE)
+        rects["y0"], rects["x0"] = pts[..., 0], pts[..., 1]
+        rects["y1"], rects["x1"] = pts[..., 0] + pts[..., 2] - 1, pts[..., 1] + pts[..., 2] - 1
 
         def fill(s, m, table, nbytes):
             N = m * L
-            hb = s["h_blocks"].numpy()[:N * stride].reshape(N, stride)
-            for i, pts in enumerate(points):
-                rect = np.zeros(max(levels), _lib.HINT_DTYPE)
-                rect["y0"], rect["x0"] = pts[:, 0], pts[:, 1]
-                rect["y1"], rect["x1"] = pts[:, 0] + pts[:, 2] - 1, pts[:, 1] + pts[:, 2] - 1
-                raw = rect.view(np.uint8)
-                for j, c in enumerate(levels):
-                    row = hb[i * L + j]
-                    row[:_lib.HINT_HDR_BYTES].view(np.int32)[:] = (c, 0, 0, 0)
-                    row[_lib.HINT_HDR_BYTES:_lib.HINT_HDR_BYTES + c * _lib.HINT_DTYPE.itemsize] = \
-                        raw[:c * _lib.HINT_DTYPE.itemsize]
-            self._upload_photos(s, nbytes, [(s["blocks"][:N * stride], s["h_blocks"][:N * stride])])
-            sh, blocks = self.s_comp.cuda_stream, s["blocks"].data_ptr()
-            self._prep(s, m, table, self.L_photo, self.rgb_photo)
-            _lib.check(None, lib.idc_rgb2lab_f64(self.device, m, X, X, self.rgb_photo.data_ptr(), self.lab.data_ptr(), sh))
+            s.blocks.grow(self.batch * HINT_BLOCK_BYTES)
+            stride = pack_hints(rects, s.blocks.h_in.numpy(), levels)
+            self._upload_photos(s, nbytes, (s.blocks, N * stride))
+            sh, blocks, rgb = self.s_comp.cuda_stream, s.blocks.dev.data_ptr(), self.rgb_photo.dev
+            self._prep(s, m, table, self.L_photo.dev, rgb)
+            _lib.check(None, lib.idc_rgb2lab_f64(self.device, m, X, X, rgb.data_ptr(), self.lab.data_ptr(), sh))
             _lib.check(None, lib.idc_hint_fill_mean(self.device, N, L, X, self.lab.data_ptr(), blocks, stride, sh))
             for b in range(N):
                 _lib.check(None, lib.idc_hint_raster(self.device, 1, X, X, levels[b % L], blocks + b * stride,
@@ -843,46 +870,47 @@ class _DeviceBatches(object):
         n = len(photos)
         s, table, nbytes = self._next_slot(photos)
         self._upload_photos(s, nbytes)
-        self._prep_stats(s, n, table, self.L_mc, s["img_rgb"])
-        self._download(s, [(s["stats"][:n], s["h_stats"][:n])])
-        return _Batch(s, s["batch"], n, 1, None)
+        self._prep_stats(s, n, table, self.L_mc, s.img_rgb.dev)
+        self._download(s, (s.stats, n))
+        return _Batch(s, s.serial, n, 1, None)
 
     def collect_stats(self, token):
-        return [r.copy() for r in self._finish(token)["h_stats"].numpy()[:token.n]]
+        return [r.copy() for r in self._finish(token).stats.h_out.numpy()[:token.n]]
 
     def submit_glob(self, photos, conditions):
         """One device pass of a global-hints sweep: image i*C+j of the sweep (C = len(conditions)) has no local hints
         and glob_vector(stats_i, conditions[j]), stats_i being photo i's own statistics."""
         torch, X, C = self.torch, self.X, len(conditions)
-        self._photo_buffers()
-        keep = self._glob_keep(conditions)
+        if conditions not in self.keep:
+            self.keep[conditions] = _Twin(self, (316,), torch.bool, C, hosts=0,
+                                          init=np.stack([_GLOB_KEEP[c] for c in conditions])).dev
+        keep = self.keep[conditions]
 
         def fill(s, m, table, nbytes):
             N = m * C
-            s["h_hints"].numpy()[:_lib.HINT_HDR_BYTES].view(np.int32)[:] = 0        # an empty hint block: zero planes
-            self._upload_photos(s, nbytes, [(s["hints"][:_lib.HINT_HDR_BYTES], s["h_hints"][:_lib.HINT_HDR_BYTES])])
+            self._upload_photos(s, nbytes, (s.hints, pack_hints([], s.hints.h_in.numpy())))    # empty: zero planes
             with torch.cuda.stream(self.s_comp):
-                self._prep_stats(s, m, table, self.L_photo, self.rgb_photo)
+                self._prep_stats(s, m, table, self.L_photo.dev, self.rgb_photo.dev)
                 # glob rows: each entry of the photo's row copied or 0 (exact, as glob_vector)
-                torch.where(keep[None], s["stats"][:m, None], self.zero, out=s["glob"][:N].view(m, C, 316))
-                _lib.check(None, self.lib.idc_hint_raster(self.device, N, X, X, 0, s["hints"].data_ptr(),
+                torch.where(keep[None], s.stats.dev[:m, None], self.zero, out=s.glob.dev[:N].view(m, C, 316))
+                _lib.check(None, self.lib.idc_hint_raster(self.device, N, X, X, 0, s.hints.dev.data_ptr(),
                                                           self.ab_in.data_ptr(), self.mask.data_ptr(),
                                                           self.s_comp.cuda_stream))
-            return s["glob"][:N], [(s["stats"][:m], s["h_stats"][:m])]
+            return s.glob.dev[:N], [(s.stats, m)]
 
         return self._submit_sweep(photos, C, fill)
 
     def collect_glob(self, token):
-        out, stats = self._collect_sweep(token), token.slot["h_stats"].numpy()
+        out, stats = self._collect_sweep(token), token.slot.stats.h_out.numpy()
         return [GlobalSweepResult(p, ab, rgb, stats[i].copy()) for i, (p, ab, rgb) in enumerate(out)]
 
     def discard(self, token):
         """Wait for a batch nobody will collect (its results are dropped), unless its slot was reused since."""
-        if token.slot["batch"] == token.serial:
+        if token.slot.serial == token.serial:
             self._finish(token)
 
     def close(self):
         self.torch.cuda.synchronize(self.dev)
         for s in self.slots:
-            self._free_big(s)
+            s.free()
         self.ctx.close()

@@ -48,12 +48,8 @@ def _single(photo, X):
 
 
 def _pack(imgs):
-    table = np.zeros(len(imgs), _lib.PHOTO_DTYPE)
-    off = 0
-    for i, a in enumerate(imgs):
-        table[i] = (off, a.shape[0], a.shape[1])
-        off += a.shape[0] * a.shape[1]
-    return table, torch.from_numpy(np.concatenate([a.reshape(-1) for a in imgs])).cuda()
+    table, src = photos.pack_photos(imgs)
+    return table, torch.from_numpy(src).cuda()
 
 
 @pytest.mark.parametrize("X", [64, 256])
@@ -198,7 +194,7 @@ def test_abandoned_interleaved_and_oversized_batches(photo_set, sd):
     pc = photos.PhotoColorizer(sd, Xd=X, batch=4, max_batch_bytes=budget)
     seq = [photo_set[0], photo_set[-1], photo_set[1], photo_set[2]]     # 0.9 MB, 54 MB alone, then two one-photo batches
     res = list(pc.colorize(seq))
-    assert [s["cap"] for s in pc._backend.slots] == [budget, budget]
+    assert [s.src.rows for s in pc._backend.slots] == [budget, budget]
     for a, r in zip(seq, res):
         want = prepost.fullres_rgb_gpu(prepost.rgb2lab_gpu(r.rgb)[1:], _single(a, X)[2])
         assert np.array_equal(r.fullres, want), a.shape

@@ -69,12 +69,8 @@ def test_fill_and_raster_equal_numpy_painting(photo_set, X):
     lib = _lib.load()
     imgs = photo_set[:4]
     n, L = len(imgs), len(LEVELS)
-    table = np.zeros(n, _lib.PHOTO_DTYPE)
-    off = 0
-    for i, a in enumerate(imgs):
-        table[i] = (off, a.shape[0], a.shape[1])
-        off += a.shape[0] * a.shape[1]
-    src = torch.from_numpy(np.concatenate([a.reshape(-1) for a in imgs])).cuda()
+    table, src = photos.pack_photos(imgs)
+    src = torch.from_numpy(src).cuda()
     L_mc = torch.empty((n, 1, X, X), device="cuda")
     rgb = torch.empty((n, X, X, 3), dtype=torch.uint8, device="cuda")
     lab = torch.empty((n, 3, X, X), dtype=torch.float64, device="cuda")
@@ -84,16 +80,14 @@ def test_fill_and_raster_equal_numpy_painting(photo_set, X):
     # blocks in the sweep's layout, with a stride that is not a multiple of 16 and stale colours to be overwritten
     pts = [photos.reveal_points(X, 1024, 11, i) for i in range(n)]
     stride = _lib.HINT_HDR_BYTES + 1024 * _lib.HINT_DTYPE.itemsize + 4
-    host = np.zeros((n * L, stride), np.uint8)
-    for i in range(n):
-        for j, c in enumerate(LEVELS):
-            h = np.zeros(c, _lib.HINT_DTYPE)
-            p = pts[i][:c]
-            h["y0"], h["x0"], h["y1"], h["x1"] = p[:, 0], p[:, 1], p[:, 0] + p[:, 2] - 1, p[:, 1] + p[:, 2] - 1
-            h["a"], h["b"] = 77.0, -77.0
-            host[i * L + j, :16].view(np.int32)[:] = (c, 0, 0, 0)
-            host[i * L + j, 16:16 + h.nbytes] = h.view(np.uint8)
-    blocks = torch.from_numpy(host.reshape(-1)).cuda()
+    host = np.zeros(n * L * stride, np.uint8)
+    rects = np.zeros((n, 1024), _lib.HINT_DTYPE)
+    p = np.stack(pts)
+    rects["y0"], rects["x0"] = p[..., 0], p[..., 1]
+    rects["y1"], rects["x1"] = p[..., 0] + p[..., 2] - 1, p[..., 1] + p[..., 2] - 1
+    rects["a"], rects["b"] = 77.0, -77.0
+    assert photos.pack_hints(rects, host, LEVELS, stride) == stride
+    blocks = torch.from_numpy(host).cuda()
     N = n * L
     ab = torch.full((N, 2, X, X), 5.0, device="cuda")
     mask = torch.full((N, 1, X, X), 5.0, device="cuda")

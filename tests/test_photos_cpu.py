@@ -2,6 +2,7 @@
 argument checks of the batched-photo C ABI entries, which return IDC_ERR_ARG before any device call."""
 import ctypes
 import os
+import struct
 
 import numpy as np
 import pytest
@@ -290,3 +291,83 @@ def test_photo_dtype_matches_header():
     assert "#define IDC_MAX_PHOTO_SIDE %d" % _lib.MAX_PHOTO_SIDE in src
     assert "#define IDC_MAX_PHOTO_X %d" % _lib.MAX_PHOTO_X in src
     assert _lib.PHOTO_DTYPE.itemsize == 16
+
+
+# ---- the two wire formats a batch feeds the kernels, restated byte by byte ----
+def test_pack_photos_writes_the_photo_table_and_packs_the_pixels():
+    rs = np.random.RandomState(3)
+    imgs = [rs.randint(0, 256, (h, w, 3)).astype(np.uint8) for h, w in ((3, 5), (1, 1), (7, 2), (2, 9))]
+    table, out = photos.pack_photos(imgs)
+    want, off = b"", 0
+    for a in imgs:                               # idc_photo: int64 off (in pixels), int32 h, int32 w
+        want += struct.pack("<qii", off, a.shape[0], a.shape[1])
+        off += a.shape[0] * a.shape[1]
+    assert table.dtype == _lib.PHOTO_DTYPE and table.tobytes() == want
+    assert out.dtype == np.uint8 and out.tobytes() == b"".join(a.tobytes() for a in imgs)
+    big = np.full(out.size + 10, 0xAB, np.uint8)          # into a larger buffer: its head only
+    t2, o2 = photos.pack_photos(imgs, big)
+    assert o2 is big and t2.tobytes() == want and big[:out.size].tobytes() == out.tobytes()
+    assert (big[out.size:] == 0xAB).all()
+
+
+def _hint_list(rs, k):
+    h = np.zeros(k, _lib.HINT_DTYPE)
+    for f in ("y0", "x0", "y1", "x1"):
+        h[f] = rs.randint(-5, 300, k)
+    h["a"], h["b"] = rs.uniform(-110, 110, k), rs.uniform(-110, 110, k)
+    h["img"] = 99                                          # replaced by the list's position when tagged
+    return h
+
+
+def _records(h, img=None):
+    # idc_hint: int32 img, y0, x0, y1, x1, float32 a, b
+    return b"".join(struct.pack("<5i2f", r["img"] if img is None else img, r["y0"], r["x0"], r["y1"], r["x1"],
+                                r["a"], r["b"]) for r in h)
+
+
+def _header(count):
+    return struct.pack("<4i", count, 0, 0, 0)
+
+
+def test_pack_hints_writes_one_tagged_block():
+    rs = np.random.RandomState(4)
+    lists = [_hint_list(rs, 3), None, _hint_list(rs, 0), _hint_list(rs, 2)]
+    out = np.full(photos.HINT_BLOCK_BYTES, 0xCD, np.uint8)
+    n = photos.pack_hints(lists, out)
+    want = _header(5) + _records(lists[0], 0) + _records(lists[3], 3)
+    assert n == len(want) == 16 + 5 * 28 and out[:n].tobytes() == want
+    assert (out[n:] == 0xCD).all()
+    assert lists[0]["img"].tolist() == [99] * 3                        # the caller's lists are left as they are
+    for empty in ([], [None, None], [_hint_list(rs, 0)]):
+        out[:] = 0xCD
+        assert photos.pack_hints(empty, out) == 16
+        assert out[:16].tobytes() == _header(0) and (out[16:] == 0xCD).all()
+    full = [_hint_list(rs, _lib.MAX_HINTS - 24), None, _hint_list(rs, 24)]          # the largest block
+    assert photos.pack_hints(full, out) == photos.HINT_BLOCK_BYTES == 16 + _lib.MAX_HINTS * 28
+    assert out.tobytes() == _header(_lib.MAX_HINTS) + _records(full[0], 0) + _records(full[2], 2)
+
+
+def test_pack_hints_writes_strided_level_blocks():
+    rs = np.random.RandomState(5)
+    recs = np.stack([_hint_list(rs, 10) for _ in range(3)])
+    recs["img"] = 0
+    levels = (0, 1, 10, 4)
+    # default stride: header + max(levels) records rounded up to 16 bytes
+    for lv, stride in ((levels, 16 + 288), ((4, 1), 16 + 112), ((5,), 16 + 144), ((0,), 16)):
+        out = np.full(3 * len(lv) * stride + 7, 0xCD, np.uint8)
+        assert photos.pack_hints(recs, out, lv) == stride
+        for i in range(3):
+            for j, c in enumerate(lv):
+                b = (i * len(lv) + j) * stride
+                want = _header(c) + _records(recs[i, :c])
+                assert out[b:b + len(want)].tobytes() == want, (lv, i, j)
+        assert (out[3 * len(lv) * stride:] == 0xCD).all()
+    # a given stride, not a multiple of 16; the records go as they are, img included
+    recs[1]["img"] = 7
+    stride = 16 + 10 * 28 + 4
+    out = np.zeros(3 * len(levels) * stride, np.uint8)
+    assert photos.pack_hints(list(recs), out, levels, stride) == stride
+    for i in range(3):
+        for j, c in enumerate(levels):
+            b = (i * len(levels) + j) * stride
+            assert out[b:b + 16 + c * 28].tobytes() == _header(c) + _records(recs[i, :c]), (i, j)

@@ -54,15 +54,11 @@ def timed(fn):
 def kernel_ms(imgs, X, iters):
     """Mean device time of one idc_photo_prep and one idc_photo_render launch over the batch `imgs`."""
     import torch
-    from interactive_deep_colorization_b200 import _lib
+    from interactive_deep_colorization_b200 import _lib, photos
     lib = _lib.load()
     n = len(imgs)
-    table = np.zeros(n, _lib.PHOTO_DTYPE)
-    off = 0
-    for i, a in enumerate(imgs):
-        table[i] = (off, a.shape[0], a.shape[1])
-        off += a.shape[0] * a.shape[1]
-    src = torch.from_numpy(np.concatenate([a.reshape(-1) for a in imgs])).cuda()
+    table, src = photos.pack_photos(imgs)
+    src = torch.from_numpy(src).cuda()
     out = torch.empty_like(src)
     L = torch.empty((n, 1, X, X), dtype=torch.float32, device="cuda")
     lab = torch.rand((n, 3, X, X), dtype=torch.float64, device="cuda") * 60 - 30

@@ -286,7 +286,10 @@ int idc_rgb2lab_f64(int device, int n, int h, int w, const uint8_t* rgb, double*
 /* f3: global statistics of a reference image (models/global_model/global_stats.prototxt:1-244; NNEncLayer with
  * NN=1, caffe_files/caffe_traininglayers.py:161-196; usage DemoGlobalHistogramTransfer.ipynb:176-182):
  * uint8 RGB [h,w,3] (h,w multiples of 4) + the 313 ab bin centres [313,2] -> out[316] =
- * [313-bin histogram of the 4x4-pooled ab, 1, mean HSV saturation, 1] = the `glob` input of idc_forward. DEVICE ptrs. */
+ * [313-bin histogram of the 4x4-pooled ab, 1, mean HSV saturation, 1] = the `glob` input of idc_forward. DEVICE ptrs.
+ * The histogram is idc_global_stats_batch's bit for bit (the same cell rule); s_avg is summed in another fixed order.
+ * The same bytes on every run.  Its scratch is allocated and released stream-ordered (cudaMallocAsync /
+ * cudaFreeAsync): the call does not wait for the device. */
 int idc_global_stats(int device, int h, int w, const uint8_t* rgb, const float* pts313, float* out316, void* stream);
 /* f1, get_img_fullres (:123-131): scipy.ndimage.zoom(order=1) of ab [2,h_in,w_in] float64 to [h,w], then
  * lab2rgb_transpose with the full-resolution L [h,w] -> uint8 [h,w,3].  The same call as

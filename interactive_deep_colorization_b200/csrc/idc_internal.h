@@ -411,6 +411,39 @@ __device__ __forceinline__ void rgb_u8_to_lab(const uint8_t* px, double& l, doub
   b = 200.0 * (fy - fz);
 }
 
+// One 4x4 cell (cy, cx) of the global-hints statistics (global_stats.prototxt) of the uint8 RGB image img, w pixels
+// wide: the cell's ab is the float64 row-major sum of its 16 pixels (rgb_u8_to_lab) from -0.0 / 16, rounded once to
+// float32, and its bin the first minimum of the float32 ((a - pa)^2 + (b - pb)^2) over the 313 centres with every
+// operation rounded separately (numpy's order, no FMA).  The 16 pixels' skimage HSV saturation is added to sat in the
+// same order.  global_stats_kernel and global_stats_batch_kernel both call it, so they bin every cell alike.
+__device__ __forceinline__ int stats_cell(const uint8_t* __restrict__ img, int w, int cy, int cx, const float2* bins,
+                                          double& sat) {
+  double sa = -0.0, sb = -0.0;
+  for (int dy = 0; dy < 4; ++dy) {
+    const uint8_t* row = img + ((size_t)(cy * 4 + dy) * w + cx * 4) * 3;
+    for (int dx = 0; dx < 4; ++dx) {
+      const uint8_t* px = row + dx * 3;
+      double l, a, b;
+      rgb_u8_to_lab(px, l, a, b);
+      sa = __dadd_rn(sa, a);
+      sb = __dadd_rn(sb, b);
+      // skimage rgb2hsv: S = (max - min) / max of the /255 values, 0 where max = 0
+      const double r8 = px[0] / 255.0, g8 = px[1] / 255.0, b8 = px[2] / 255.0;
+      const double mx = fmax(r8, fmax(g8, b8)), mn = fmin(r8, fmin(g8, b8));
+      sat = __dadd_rn(sat, mx > 0.0 ? __ddiv_rn(__dsub_rn(mx, mn), mx) : 0.0);
+    }
+  }
+  const float a = __double2float_rn(__ddiv_rn(sa, 16.0)), b = __double2float_rn(__ddiv_rn(sb, 16.0));
+  int best = 0;
+  float bd = 0.f;
+  for (int k = 0; k < 313; ++k) {
+    const float da = __fsub_rn(a, bins[k].x), db = __fsub_rn(b, bins[k].y);
+    const float d = __fadd_rn(__fmul_rn(da, da), __fmul_rn(db, db));
+    if (k == 0 || d < bd) { bd = d; best = k; }
+  }
+  return best;
+}
+
 // OpenCV's source coordinate of output d, (float)((d + 0.5) * scale - 0.5) (modules/imgproc/src/resize.cpp), with the
 // multiply and the subtract rounded separately as on the host (nvcc would fuse them).
 __device__ __forceinline__ float cv_src_coord(int d, double scale) {

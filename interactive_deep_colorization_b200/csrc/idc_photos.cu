@@ -133,14 +133,13 @@ __global__ void __launch_bounds__(kFillThreads) hint_fill_mean_kernel(int levels
 }
 
 // grid n, one CTA per image: global_stats.prototxt (rgb2lab -> 4x4 average pool of ab -> nearest of the 313 bins ->
-// global average; mean HSV saturation) for image blockIdx.x of rgb [n,h,w,3].  Thread t takes cells t, t + T, ...; a
-// cell's ab is the float64 row-major sum of its 16 pixels / 16, rounded once to float32, and its bin the first minimum
-// of the float32 ((a - pa)^2 + (b - pb)^2) with every operation rounded separately (numpy's order, no FMA).  Bin counts
-// are integer shared-memory atomics; the saturation partials are reduced in a fixed tree.  Nothing depends on n or on
+// global average; mean HSV saturation) for image blockIdx.x of rgb [n,h,w,3].  Thread t takes cells t, t + T, ...,
+// each through stats_cell (idc_internal.h), the routine of the single-image global_stats_kernel.  Bin counts are
+// integer shared-memory atomics; the saturation partials are reduced in a fixed tree.  Nothing depends on n or on
 // where the image sits in the batch, so a row is identical bit for bit in any batch and on every run.
 constexpr int kStatsThreads = 512;
 
-__global__ void __launch_bounds__(kStatsThreads) global_stats_batch_kernel(int h, int w, const uint8_t* __restrict__ rgb,
+__global__ void __launch_bounds__(kStatsThreads, 1) global_stats_batch_kernel(int h, int w, const uint8_t* __restrict__ rgb,
                                                                            const float* __restrict__ pts,
                                                                            float* __restrict__ out) {
   __shared__ int count[313];
@@ -156,30 +155,7 @@ __global__ void __launch_bounds__(kStatsThreads) global_stats_batch_kernel(int h
   double sat = 0.0;
   for (int c = threadIdx.x; c < cells; c += kStatsThreads) {
     const int cy = c / w4, cx = c - cy * w4;
-    double sa = -0.0, sb = -0.0;
-    for (int dy = 0; dy < 4; ++dy) {
-      const uint8_t* row = img + ((size_t)(cy * 4 + dy) * w + cx * 4) * 3;
-      for (int dx = 0; dx < 4; ++dx) {
-        const uint8_t* px = row + dx * 3;
-        double l, a, b;
-        rgb_u8_to_lab(px, l, a, b);
-        sa = __dadd_rn(sa, a);
-        sb = __dadd_rn(sb, b);
-        // skimage rgb2hsv: S = (max - min) / max of the /255 values, 0 where max = 0
-        const double r8 = px[0] / 255.0, g8 = px[1] / 255.0, b8 = px[2] / 255.0;
-        const double mx = fmax(r8, fmax(g8, b8)), mn = fmin(r8, fmin(g8, b8));
-        sat = __dadd_rn(sat, mx > 0.0 ? __ddiv_rn(__dsub_rn(mx, mn), mx) : 0.0);
-      }
-    }
-    const float a = __double2float_rn(__ddiv_rn(sa, 16.0)), b = __double2float_rn(__ddiv_rn(sb, 16.0));
-    int best = 0;
-    float bd = 0.f;
-    for (int k = 0; k < 313; ++k) {
-      const float da = __fsub_rn(a, bins[k].x), db = __fsub_rn(b, bins[k].y);
-      const float d = __fadd_rn(__fmul_rn(da, da), __fmul_rn(db, db));
-      if (k == 0 || d < bd) { bd = d; best = k; }
-    }
-    atomicAdd(&count[best], 1);
+    atomicAdd(&count[stats_cell(img, w, cy, cx, bins, sat)], 1);
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) sat = __dadd_rn(sat, __shfl_xor_sync(0xffffffffu, sat, o));

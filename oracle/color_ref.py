@@ -24,13 +24,18 @@ def _as_float(img):
     return img.astype(np.float64)
 
 
-def rgb2lab(rgb):
+def rgb2xyz_white(rgb):
+    """rgb2lab's intermediate: XYZ / the D65 white point, the values lab_f's 0.008856 branch tests."""
     arr = _as_float(rgb).copy()
     m = arr > 0.04045
     arr[m] = np.power((arr[m] + 0.055) / 1.055, 2.4)
     arr[~m] /= 12.92
     xyz = arr @ XYZ_FROM_RGB.T
-    xyz = xyz / WHITE_D65_2
+    return xyz / WHITE_D65_2
+
+
+def rgb2lab(rgb):
+    xyz = rgb2xyz_white(rgb)
     m = xyz > 0.008856
     xyz[m] = np.cbrt(xyz[m])
     xyz[~m] = 7.787 * xyz[~m] + 16.0 / 116.0
@@ -41,7 +46,8 @@ def rgb2lab(rgb):
     return np.concatenate([v[..., np.newaxis] for v in (L, a, b)], axis=-1)
 
 
-def lab2rgb(lab):
+def lab2linear(lab):
+    """lab2rgb's intermediate: linear RGB, the values the 0.0031308 gamma branch tests."""
     lab = np.asarray(lab, dtype=np.float64)
     L, a, b = lab[..., 0], lab[..., 1], lab[..., 2]
     y = (L + 16.0) / 116.0
@@ -53,7 +59,11 @@ def lab2rgb(lab):
     out[m] = np.power(out[m], 3.0)
     out[~m] = (out[~m] - 16.0 / 116.0) / 7.787
     out *= WHITE_D65_2
-    arr = out @ RGB_FROM_XYZ.T
+    return out @ RGB_FROM_XYZ.T
+
+
+def lab2rgb(lab):
+    arr = lab2linear(lab)
     m = arr > 0.0031308
     arr[m] = 1.055 * np.power(arr[m], 1.0 / 2.4) - 0.055
     arr[~m] *= 12.92

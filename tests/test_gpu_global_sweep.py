@@ -97,9 +97,8 @@ def test_kernel_vs_oracle_and_single_image_kernel(photo_set, X):
         assert got[i, 313] == 1 and got[i, 315] == 1
         assert abs(float(got[i, 314]) - float(ref[314])) <= np.spacing(np.float32(ref[314])), (X, i)
         one = prepost.global_stats_gpu(img)                     # the single-image, many-CTA kernel
-        c_one = np.rint(one[:313].astype(np.float64) * cells).astype(np.int64)
-        assert np.abs(c_got - c_one).sum() // 2 <= near, (X, i)
-        assert abs(float(got[i, 314]) - float(one[314])) <= 4 * np.spacing(np.float32(one[314])), (X, i)
+        assert one[:313].tobytes() == got[i, :313].tobytes(), (X, i)      # one cell routine: the same bins
+        assert abs(float(got[i, 314]) - float(one[314])) <= 2 * np.spacing(np.float32(one[314])), (X, i)
         print("X=%d photo %d: %d cells moved against the oracle (%d near a boundary)" % (X, i, moved, near))
 
 

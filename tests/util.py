@@ -76,19 +76,24 @@ def small_batch(n=2, X=64, seed=100):
     return synth.synthetic_batch(n, X, seed=seed, max_hints=4)
 
 
-def render_edges(rgb255, margin=1e-9):
+def render_edges(rgb255, margin=1e-9, unclipped=None):
     """Values of a float64 render before its truncating cast (255 * clip(lab2rgb(lab), 0, 1)) that lie within `margin`
     of an integer strictly inside (0, 255).  Only there can a last-ulp difference between CUDA's pow / cbrt and glibc's
-    flip the cast; clipped values are exact on every path."""
+    flip the cast; values clipped from well outside [0, 1] are exact on every path.  unclipped (optional): the same
+    render before the clip, 255 * lab2rgb(lab); values it puts within `margin` of 255 are edges too (one path may
+    clip 255.0000000001 to 255 where the other truncates 254.9999999999 to 254)."""
     frac = rgb255 - np.floor(rgb255)
-    return ((frac < margin) | (frac > 1 - margin)) & (rgb255 > 0) & (rgb255 < 255)
+    edge = ((frac < margin) | (frac > 1 - margin)) & (rgb255 > 0) & (rgb255 < 255)
+    if unclipped is not None:
+        edge |= np.abs(unclipped - 255) < margin
+    return edge
 
 
-def assert_render_exact(got, want, rgb255, what):
-    """The uint8 render `got` equals `want` in every value outside render_edges(rgb255).  Prints and returns how many
-    values were excluded and how many of those differ."""
+def assert_render_exact(got, want, rgb255, what, unclipped=None):
+    """The uint8 render `got` equals `want` in every value outside render_edges(rgb255, unclipped=unclipped).  Prints
+    and returns how many values were excluded and how many of those differ."""
     assert got.shape == want.shape == rgb255.shape and got.dtype == want.dtype == np.uint8, (what, got.shape, want.shape)
-    edge = render_edges(rgb255)
+    edge = render_edges(rgb255, unclipped=unclipped)
     diff = got != want
     bad = np.argwhere(diff & ~edge)
     assert len(bad) == 0, (what, len(bad), [(tuple(i), int(got[tuple(i)]), int(want[tuple(i)])) for i in bad[:5]])

@@ -42,6 +42,17 @@ or PSNR under the global-hints conditions taken from each photo itself (none, sa
     python ideepcolor_b200.py --color_model glob.pth --global_hints --caffe --image_dir scans/ --out o/ --glob_ref ref.jpg
     python ideepcolor_b200.py --color_model glob.pth --global_hints --image_dir val/ --out o/ --glob_sweep [none,hist]
 
+Under torchrun (WORLD_SIZE > 1 in the environment) the folder mode is one shard of a job per process: rank r takes
+the contiguous slice parallel.shard_range(n, world, r) of the sorted photos on GPU LOCAL_RANK (--gpu is ignored),
+writes its own photos' <stem>.png and <stem>_suggestions.json, and rank 0 gathers every rank's rows and writes
+psnr.csv, reveal_psnr.csv or glob_psnr.csv and the mean rows, byte for byte what one process writes.  The checkpoint
+is read, and --calibrate / --save_act_ranges run, on rank 0 only; the other ranks receive the packed weights with one
+broadcast.  An error on any rank (a photo that fails to read, say) makes every rank exit with status 1 and its message.
+--dist_backend gloo lets ranks share one GPU (NCCL refuses two ranks on one device):
+
+    torchrun --nproc_per_node 8 ideepcolor_b200.py --color_model caffemodel.pth --image_dir val/ --out sweep/ \
+        --reveal_sweep 0,1,2,5,10,20,50 --batch 60
+
 hints.json: [{"loc": [row, col], "size": 3, "ab": [23, -69]}, {"loc": [100, 160], "rgb": [255, 255, 255]}, ...]
 (`loc` in load_size x load_size network coordinates, `size` = p of the notebook's put_point: a (2p+1)^2 patch.)
 """
@@ -92,6 +103,8 @@ def parse_args(argv=None):
                     help="with --global_hints: PSNR of every photo under global hints from its own statistics, one "
                          "column per condition of none,sat,hist,hist+sat (default all four), into <out>/glob_psnr.csv "
                          "(no images are written)")
+    ap.add_argument("--dist_backend", default="nccl", choices=("nccl", "gloo"),
+                    help="process-group backend of --image_dir under torchrun (gloo: ranks may share a GPU)")
     args = ap.parse_args(argv)
     given = {"global_hints": args.global_hints, "caffe": args.caffe, "glob_ref": bool(args.glob_ref),
              "glob_sweep": args.glob_sweep is not None, "hints_dir": bool(args.hints_dir), "caffe_dist": args.caffe_dist}
@@ -218,8 +231,10 @@ IMAGE_EXTS = (".jpg", ".jpeg", ".png", ".bmp", ".tif", ".tiff", ".webp")
 
 
 def colorize_dir(args):
-    """--image_dir: every photo of the folder (sorted by name) through PhotoColorizer -> OUT/<stem>.png (+ psnr.csv)."""
+    """--image_dir: every photo of the folder (sorted by name) through PhotoColorizer -> OUT/<stem>.png (+ psnr.csv);
+    this process's shard of them under torchrun (colorize_dir_sharded)."""
     import torch
+    from interactive_deep_colorization_b200 import parallel
     from interactive_deep_colorization_b200.photos import PhotoColorizer
     if not args.out:
         print("--image_dir needs --out")
@@ -233,16 +248,27 @@ def colorize_dir(args):
         print("photos share a name and would overwrite each other's result: %s" % ", ".join(clash))
         return 2
     paths = [os.path.join(args.image_dir, f) for f in names]
-    if not os.path.isdir(args.out):
-        os.makedirs(args.out)
-    hints = read_hints_dir(args.hints_dir, names) if args.hints_dir else None
-    sd = torch.load(args.color_model, map_location="cpu")
+    os.makedirs(args.out, exist_ok=True)
+    args.world, args.rank = parallel.world_rank()
+    sd = hints = error = None
+    try:
+        hints = read_hints_dir(args.hints_dir, names) if args.hints_dir else None
+        if args.rank == 0:        # the other ranks of a job receive the packed weights
+            sd = torch.load(args.color_model, map_location="cpu")
+    except Exception as e:
+        if args.world == 1:
+            raise
+        error = e
+    if args.world > 1:
+        parallel.agree(error, device=args.gpu)
     extra = {}
     if hints is not None and args.suggest > 0:
         extra = {"caffe_dist": True} if args.caffe_dist else {"suggest": True}
     pc = PhotoColorizer(sd, Xd=args.load_size, batch=args.batch, device=args.gpu, maskcent=args.pytorch_maskcent,
-                        calibrate=args.calibrate_source, global_hints=args.global_hints, caffe=args.caffe, **extra)
-    save_ranges(args, pc.act_ranges)
+                        calibrate=args.calibrate_source if args.rank == 0 else None, global_hints=args.global_hints,
+                        caffe=args.caffe, **extra)
+    if args.rank == 0:
+        save_ranges(args, pc.act_ranges)
     if hints is not None:
         return hinted_dir(args, pc, names, paths, hints)
     if args.reveal_levels is not None:
@@ -252,25 +278,91 @@ def colorize_dir(args):
     glob = None
     if args.glob_ref:         # histogram transfer: every photo with REF's histogram (DemoGlobalHistogramTransfer.ipynb)
         from interactive_deep_colorization_b200 import photos
-        ref = next(iter(pc.global_stats([args.glob_ref])))
+        # one copy of REF per rank, so that every rank's shard holds one; its statistics do not depend on the batch
+        ref = next(iter(pc.global_stats([args.glob_ref] * args.world)))
         glob = [photos.glob_vector(ref, "hist")] * len(paths)
     write_photos(args, pc, names, pc.colorize(paths, glob=glob, psnr=args.psnr))
-    print("colorized %d photos into <%s>" % (len(names), args.out))
+    if args.rank == 0:
+        print("colorized %d photos into <%s>" % (len(names), args.out))
     return 0
+
+
+class JobFailed(Exception):
+    """A rank of a torchrun job failed; every rank raises this with the same message from the final gather."""
+
+
+def final_gather(args, error, items):
+    """The last collective of a folder-mode job, which every rank reaches once, whether its shard succeeded or not:
+    its error text (None if none) and its items, in photo order -> every rank's items in rank order (which is photo
+    order) on rank 0, None on the others.  Raises JobFailed on every rank if any rank sent an error."""
+    import torch.distributed as dist
+    args.gathered = True
+    got = [None] * args.world
+    dist.all_gather_object(got, (error, items))
+    errors = [e for e, _ in got if e is not None]
+    if errors:
+        raise JobFailed("; ".join(errors))
+    return [x for _, part in got for x in part] if args.rank == 0 else None
+
+
+def merge_rows(args, items):
+    """This process's rows -> the rows of every photo on the process that writes the CSVs, None on the others."""
+    return items if args.world == 1 else final_gather(args, None, items)
+
+
+def my_names(pc, names):
+    """The names of the photos this process colours (PhotoColorizer.local_slice), in order."""
+    start, count = pc.local_slice(len(names))
+    return names[start:start + count]
+
+
+def colorize_dir_sharded(args):
+    """--image_dir under torchrun: the process group for the job's lifetime, and every failure carried into the final
+    gather (final_gather), so that all ranks exit with status 1 and the failing rank's message instead of waiting."""
+    import traceback
+    import torch
+    import torch.distributed as dist
+    local = int(os.environ.get("LOCAL_RANK", "0"))
+    if args.gpu != local:
+        print("note: --gpu %d is ignored under torchrun: this rank runs on GPU LOCAL_RANK = %d" % (args.gpu, local))
+    args.gpu = local
+    if args.dist_backend == "nccl":
+        torch.cuda.set_device(local)
+    dist.init_process_group(args.dist_backend)
+    args.gathered = False
+    try:
+        try:
+            return colorize_dir(args)
+        except JobFailed as e:
+            msg = str(e)
+        except Exception as e:
+            if args.gathered:
+                raise
+            traceback.print_exc()
+            msg = "rank %d: %s: %s" % (dist.get_rank(), type(e).__name__, e)
+            try:
+                final_gather(args, msg, [])
+            except JobFailed as f:        # with every rank's errors
+                msg = str(f)
+        print("the job failed: %s" % msg, file=sys.stderr)
+        return 1
+    finally:
+        dist.destroy_process_group()
 
 
 def write_photos(args, pc, names, results):
     """OUT/<stem>.png of each photo's PhotoResult (its full-resolution result) and, with --psnr, OUT/psnr.csv; then
-    closes pc."""
+    closes pc.  names: every photo's; results: those of this process's photos."""
     import cv2
     rows = []
-    for name, r in zip(names, results):
+    for name, r in zip(my_names(pc, names), results):
         stem = os.path.splitext(name)[0]
         cv2.imwrite(os.path.join(args.out, stem + ".png"), np.ascontiguousarray(r.fullres[:, :, ::-1]))
         if args.psnr:
             rows.append("%s,%.17g" % (name, r.psnr))
     pc.close()
-    if args.psnr:
+    rows = merge_rows(args, rows)
+    if args.psnr and rows is not None:
         with open(os.path.join(args.out, "psnr.csv"), "w") as f:
             f.write("image,psnr\n" + "".join(row + "\n" for row in rows))
 
@@ -285,7 +377,8 @@ def hinted_dir(args, pc, names, paths, hints):
         suggested = pc.suggest(paths, rects, locs, K=args.suggest, psnr=args.psnr)
 
         def results():
-            for name, hl, r in zip(names, hints, suggested):
+            start = pc.local_slice(len(names))[0]
+            for name, hl, r in zip(names[start:], hints[start:], suggested):
                 if hl:
                     write_suggestions(os.path.join(args.out, os.path.splitext(name)[0] + "_suggestions.json"), hl,
                                       r.centers, r.conf)
@@ -293,18 +386,24 @@ def hinted_dir(args, pc, names, paths, hints):
         write_photos(args, pc, names, results())
     else:
         write_photos(args, pc, names, pc.colorize(paths, hints=rects, psnr=args.psnr))
-    print("colorized %d photos with the hints of <%s> into <%s>" % (len(names), args.hints_dir, args.out))
+    if args.rank == 0:
+        print("colorized %d photos with the hints of <%s> into <%s>" % (len(names), args.hints_dir, args.out))
     return 0
 
 
 def write_sweep(args, pc, names, csv, labels, results, title, line):
     """A sweep's PSNR, one result per photo -> OUT/<csv> (a row per photo, a column per label, then the mean row), and
-    `title` and the mean per label (`line` % (label, mean)) on stdout; closes pc."""
-    rows, curves = [], []
-    for name, r in zip(names, results):
-        rows.append([name] + ["%.17g" % v for v in r.psnr])
-        curves.append(r.psnr)
+    `title` and the mean per label (`line` % (label, mean)) on stdout; closes pc.  names: every photo's; results: those
+    of this process's photos."""
+    rows = []
+    for name, r in zip(my_names(pc, names), results):
+        rows.append(([name] + ["%.17g" % v for v in r.psnr], r.psnr))
     pc.close()
+    rows = merge_rows(args, rows)
+    if rows is None:
+        return 0
+    curves = [c for _, c in rows]
+    rows = [row for row, _ in rows]
     mean = np.mean(curves, axis=0) if curves else np.full(len(labels), np.nan)
     rows.append(["mean"] + ["%.17g" % v for v in mean])
     with open(os.path.join(args.out, csv), "w") as f:
@@ -335,8 +434,13 @@ def glob_sweep_dir(args, pc, names, paths):
 
 def main(argv=None):
     args = parse_args(argv)
+    world = int(os.environ.get("WORLD_SIZE", "1"))
     if args.image_dir:
-        return colorize_dir(args)
+        return colorize_dir_sharded(args) if world > 1 else colorize_dir(args)
+    if world > 1:
+        print("--image_file colours one photo on one GPU: run it without torchrun (WORLD_SIZE = %d), or shard a folder "
+              "with --image_dir" % world)
+        return 2
     import cv2
     import torch
     from interactive_deep_colorization_b200 import colorize_image as CI

@@ -114,6 +114,8 @@ int idc_finalize_weights(idc_ctx* ctx);
 int idc_weights_arena(idc_ctx* ctx, void** dev_ptr, size_t* bytes);
 int idc_reserve_weights(idc_ctx* ctx);    /* allocate the arena without packing (receiver side) */
 int idc_adopt_weights(idc_ctx* ctx);      /* mark a received arena as final                     */
+/* The arena does not hold IDC_FLAG_CAFFE313's bin centres: load "caffe.pts_in_hull" [313,2] (idc_load_tensor) before
+ * idc_adopt_weights, which fails with IDC_ERR_KEY without it. */
 
 /* Replaces `self.net.forward(img_l_mc, input_ab_mc, input_mask_mult, mask_cent)`
  * (data/colorize_image.py:263 / :308), batched.

@@ -925,11 +925,6 @@ int idc_finalize_weights(idc_ctx* c) {
   std::vector<char> host(c->arena_bytes, 0);
   rc = pack_weights(c, host.data());
   if (rc != IDC_OK) return rc;
-  if (c->caffe313) {
-    const HostTensor* pts = find(c, "caffe.pts_in_hull");
-    if (!check_dims(pts, {313, 2})) return fail(c, IDC_ERR_KEY, "missing/bad caffe.pts_in_hull [313,2]");
-    CUDA_TRY(c, cudaMemcpy(c->pts313.get(), pts->data.data(), sizeof(float) * 626, cudaMemcpyHostToDevice));
-  }
   CUDA_TRY(c, cudaMemcpy(c->arena.get(), host.data(), c->arena_bytes, cudaMemcpyHostToDevice));
   return idc_adopt_weights(c);
 }
@@ -937,6 +932,12 @@ int idc_finalize_weights(idc_ctx* c) {
 int idc_adopt_weights(idc_ctx* c) {
   if (!c || !c->arena.get()) return fail(c, IDC_ERR_STATE, "no arena");
   CUDA_TRY(c, cudaSetDevice(c->dev));
+  // the 313 bin centres are not part of the arena: a context that received it loads caffe.pts_in_hull itself
+  if (c->caffe313) {
+    const HostTensor* pts = find(c, "caffe.pts_in_hull");
+    if (!check_dims(pts, {313, 2})) return fail(c, IDC_ERR_KEY, "missing/bad caffe.pts_in_hull [313,2]");
+    CUDA_TRY(c, cudaMemcpy(c->pts313.get(), pts->data.data(), sizeof(float) * 626, cudaMemcpyHostToDevice));
+  }
   // conv1_1 takes its weights as a kernel parameter: read them back from the (possibly received) arena
   CUDA_TRY(c, cudaMemcpy(c->h_w11.w, c->w11, sizeof(c->h_w11.w), cudaMemcpyDeviceToHost));
   CUDA_TRY(c, cudaMemcpy(c->h_w11.b, c->b11, sizeof(c->h_w11.b), cudaMemcpyDeviceToHost));

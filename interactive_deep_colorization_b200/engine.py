@@ -245,21 +245,24 @@ class LhnContext(object):
                 if b in mine:
                     _lib.check(self.h, self.lib.idc_set_act_range(self.h, b.encode(), v))
         for k, v in sd.items():
-            a = v.detach().cpu().numpy() if hasattr(v, "detach") else np.asarray(v)
-            if a.dtype == np.float32:
-                dt = _lib.F32
-            elif a.dtype == np.float64:
-                dt = _lib.F64
-            elif a.dtype == np.int64:
-                dt = _lib.I64
-            else:
-                a = a.astype(np.float32)
-                dt = _lib.F32
-            a = np.ascontiguousarray(a)
-            dims = (ctypes.c_int64 * max(a.ndim, 1))(*a.shape)
-            _lib.check(self.h, self.lib.idc_load_tensor(self.h, k.encode(), _np_ptr(a), dt, a.ndim, dims))
+            self._load_tensor(k, v)
         _lib.check(self.h, self.lib.idc_finalize_weights(self.h))
         self.ready = True
+
+    def _load_tensor(self, k, v):
+        a = v.detach().cpu().numpy() if hasattr(v, "detach") else np.asarray(v)
+        if a.dtype == np.float32:
+            dt = _lib.F32
+        elif a.dtype == np.float64:
+            dt = _lib.F64
+        elif a.dtype == np.int64:
+            dt = _lib.I64
+        else:
+            a = a.astype(np.float32)
+            dt = _lib.F32
+        a = np.ascontiguousarray(a)
+        dims = (ctypes.c_int64 * max(a.ndim, 1))(*a.shape)
+        _lib.check(self.h, self.lib.idc_load_tensor(self.h, k.encode(), _np_ptr(a), dt, a.ndim, dims))
 
     def weights_arena(self):
         p, n = ctypes.c_void_p(), ctypes.c_size_t()
@@ -270,6 +273,12 @@ class LhnContext(object):
         _lib.check(self.h, self.lib.idc_reserve_weights(self.h))
 
     def adopt_weights(self):
+        """Take the arena as received (reserve_weights, then a copy into weights_arena()).  The Caffe 313-bin head's
+        bin centres are not part of the arena: with caffe313 they are the package's pts_in_hull, the centres every
+        loader of the Caffe distribution model adds (ColorizeImageB200Caffe.prep_net, PhotoColorizer)."""
+        if self.flags & _lib.FLAG_CAFFE313:
+            from .prepost import pts_in_hull
+            self._load_tensor("caffe.pts_in_hull", pts_in_hull())
         _lib.check(self.h, self.lib.idc_adopt_weights(self.h))
         self.ready = True
 

@@ -1,11 +1,15 @@
 """Multi-GPU: one process per GPU, images sharded across ranks, ONE broadcast of the packed
 weight arena at init, no per-step collective (SURVEY.md 8e -- images are independent: the
 network has no cross-image state, BatchNorm runs in eval mode,
-/root/reference/data/colorize_image.py:232).
+/root/reference/data/colorize_image.py:232).  Before the broadcast the ranks agree (agree) that
+every one of them is ready for it, so a rank that fails makes all of them raise instead of wait.
+ShardedColorizer (device tensors) and photos.PhotoColorizer (photo batches and sweeps) both
+get their context from share_weights.
 
 Host logic here is backend-agnostic (`gloo` on CPU in the tests, `nccl` over NVLink on the box).
 """
-import numpy as np
+import contextlib
+
 import torch
 import torch.distributed as dist
 
@@ -32,6 +36,91 @@ def broadcast_blob(t, src=0):
     return t
 
 
+def world_rank():
+    """(world size, rank) of the default process group; (1, 0) when there is none."""
+    if dist.is_available() and dist.is_initialized():
+        return dist.get_world_size(), dist.get_rank()
+    return 1, 0
+
+
+def _object_device(device):
+    """NCCL's object collectives stage through the current CUDA device: make it this rank's for their duration."""
+    if dist.get_backend() == "nccl":
+        return torch.cuda.device(device)
+    return contextlib.nullcontext()
+
+
+def agree(error, fingerprint=None, payload=None, device=0):
+    """One all_gather_object of every rank's outcome so far, so that all ranks leave a set-up step together: either
+    every rank goes on, or every rank raises.  error: the exception this rank met (None if none); fingerprint: what must
+    be equal on every rank; payload: what rank 0 hands to every rank (-> the return value).
+    Raises on every rank: the lowest failing rank's error (that rank re-raises its own exception, the others a
+    ValueError with its text), else, when a rank's fingerprint differs from rank 0's, a ValueError naming both."""
+    world, rank = world_rank()
+    got = [None] * world
+    with _object_device(device):
+        dist.all_gather_object(got, (None if error is None else "%s: %s" % (type(error).__name__, error),
+                                     fingerprint, payload))
+    for r, (msg, _, _) in enumerate(got):
+        if msg is not None:
+            if r == rank:
+                raise error
+            raise ValueError("rank %d failed: %s" % (r, msg))
+    for r, (_, fp, _) in enumerate(got):
+        if fp != got[0][1]:
+            raise ValueError("rank %d was given %r, rank 0 %r: every rank of a job needs the same arguments"
+                             % (r, fp, got[0][1]))
+    return got[0][2]
+
+
+def share_weights(make_ctx, state_dict, act_ranges=None, device=0):
+    """A context with the job's weights on every rank.  Without a process group (or world size 1) make_ctx() loads
+    state_dict.  Otherwise rank 0 loads state_dict (act_ranges set its storage exponents, which the arena carries), the
+    other ranks reserve_weights(), receive the packed arena with ONE broadcast and adopt_weights(); state_dict is needed
+    on rank 0 only.  Whether every rank built its context is agreed first, so a rank that fails there makes every rank
+    raise instead of leaving the others in the broadcast.  Over gloo the arena goes through a host byte tensor, which
+    lets ranks share one GPU (NCCL refuses two ranks on one device)."""
+    world, rank = world_rank()
+    if world == 1:
+        ctx = make_ctx()
+        try:
+            ctx.load_state_dict(state_dict, act_ranges=act_ranges)
+        except BaseException:
+            ctx.close()
+            raise
+        return ctx
+    ctx, error = None, None
+    try:
+        ctx = make_ctx()
+        if rank == 0:
+            if state_dict is None:
+                raise ValueError("rank 0 needs the state_dict")
+            ctx.load_state_dict(state_dict, act_ranges=act_ranges)
+        else:
+            ctx.reserve_weights()
+    except Exception as e:
+        error = e
+    try:
+        agree(error, device=device)
+        ptr, nbytes = ctx.weights_arena()
+        blob = torch.as_tensor(_DevBlob(ptr, nbytes), device="cuda:%d" % device)
+        if dist.get_backend() == "gloo":
+            host = blob.cpu() if rank == 0 else torch.empty(nbytes, dtype=torch.uint8)
+            broadcast_blob(host, src=0)
+            if rank != 0:
+                blob.copy_(host)
+        else:
+            broadcast_blob(blob, src=0)
+        torch.cuda.synchronize(device)
+        if rank != 0:
+            ctx.adopt_weights()
+    except BaseException:
+        if ctx is not None:
+            ctx.close()
+        raise
+    return ctx
+
+
 def max_over_ranks(value, device=None):
     """Device-timed durations are reduced with MAX so a step is as slow as its slowest rank."""
     t = torch.tensor([float(value)], dtype=torch.float64, device=device)
@@ -54,8 +143,7 @@ class ShardedColorizer(object):
                  calibrate_maskcent=0.0, **ctx_kw):
         from . import engine
         from .engine import LhnContext
-        self.world = dist.get_world_size() if dist.is_initialized() else 1
-        self.rank = dist.get_rank() if dist.is_initialized() else 0
+        self.world, self.rank = world_rank()
         self.device = torch.cuda.current_device() if device is None else device
         ranges = None
         if self.rank == 0 and calibrate is not None:
@@ -67,23 +155,10 @@ class ShardedColorizer(object):
                 state_dict, engine.calibration_batch(photos, H, device=self.device,
                                                      global_hints=flags.get("global_hints", False)),
                 H, W, device=self.device, maskcent=float(calibrate_maskcent), **flags))
-        self.ctx = LhnContext(device=self.device, max_n=per_rank_batch, H=H, W=W, dist=dist_head, **ctx_kw)
-        if self.world == 1:
-            self.ctx.load_state_dict(state_dict, act_ranges=ranges)
-            return
-        if self.rank == 0:
-            if state_dict is None:
-                raise ValueError("rank 0 needs the state_dict")
-            self.ctx.load_state_dict(state_dict, act_ranges=ranges)
-        else:
-            self.ctx.reserve_weights()
-        ptr, nbytes = self.ctx.weights_arena()
-        blob = torch.as_tensor(_DevBlob(ptr, nbytes), device="cuda:%d" % self.device)
-        broadcast_blob(blob, src=0)                     # the only collective of the whole job
-        torch.cuda.synchronize(self.device)
-        if self.rank != 0:
-            self.ctx.adopt_weights()
-        self.arena_bytes = nbytes
+        self.ctx = share_weights(lambda: LhnContext(device=self.device, max_n=per_rank_batch, H=H, W=W,
+                                                    dist=dist_head, **ctx_kw), state_dict, ranges, self.device)
+        if self.world > 1:
+            self.arena_bytes = self.ctx.weights_arena()[1]
 
     def local_slice(self, n_total):
         return shard_range(n_total, self.world, self.rank)

@@ -311,11 +311,46 @@ class PhotoColorizer(object):
                 no distribution head).
     caffe_dist  with caffe: the context also carries the checkpoint's Caffe 313-bin distribution head (the caffe.* keys
                 of include/idc_b200.h), for `suggest`, as ColorizeImageB200CaffeDist loads it; the colour result still
-                comes from the regression head and is what caffe=True alone gives.  Not with global_hints."""
+                comes from the regression head and is what caffe=True alone gives.  Not with global_hints.
+
+    One shard of a job.  When torch.distributed is initialised with world size > 1 (one process per GPU, under
+    torchrun), every rank constructs a PhotoColorizer with the same arguments; state_dict and calibrate are needed on
+    rank 0 only, where the checkpoint is checked, calibrated and loaded, and the other ranks receive the packed weights
+    with one broadcast (parallel.share_weights; NCCL, or gloo for ranks that share a GPU).  Before that, every rank
+    learns rank 0's outcome and compares its arguments (Xd, batch, the flags and options, the device's SM count) with
+    rank 0's: if rank 0 failed, or any rank's arguments differ, every rank raises.  Every pass method then takes the
+    whole job's lists (photos, hints, glob, points), checks them whole, and processes this rank's contiguous slice
+    local_slice(len(photos)): its iterator yields result j for photo start + j.  The launch plan depends on batch and
+    the SM count, never on a pass's photos, so every result equals the single-process one bit for bit, whatever the
+    world size.  The process group belongs to the caller; close() releases this rank's buffers only."""
 
     def __init__(self, state_dict, Xd=256, batch=32, device=0, maskcent=False, global_hints=False, engine="wgmma",
                  max_batch_bytes=96 << 20, readahead=None, workers=4, calibrate=None, caffe=False, suggest=False,
                  caffe_dist=False):
+        from . import parallel
+        self.world, self.rank = parallel.world_rank()
+        error = fingerprint = None
+        try:
+            fingerprint = self._setup(Xd, batch, device, maskcent, global_hints, engine, caffe, suggest, caffe_dist)
+            if self.rank == 0:
+                state_dict = self._load(state_dict, calibrate)
+            else:
+                self.act_ranges = None
+        except Exception as e:
+            if self.world == 1:
+                raise
+            error = e
+        if self.world > 1:
+            # no rank may go on to the weights' broadcast (or raise) alone
+            self.act_ranges = parallel.agree(error, fingerprint, None if error else self.act_ranges, device=device)
+        self.max_batch_bytes = int(max_batch_bytes)
+        self.readahead = int(readahead) if readahead else 2 * self.batch
+        self.workers = int(workers)
+        self._backend = self._make_backend(state_dict)
+
+    def _setup(self, Xd, batch, device, maskcent, global_hints, engine, caffe, suggest, caffe_dist):
+        """The checks and settings of the arguments every rank is given -> what must be equal on every rank of a job
+        (with the device's SM count, which the launch plan depends on)."""
         if Xd < 8 or Xd % 8:
             raise ValueError("Xd must be a multiple of 8, got %d" % Xd)
         if not 1 <= batch <= _lib.MAX_PHOTOS:
@@ -331,14 +366,26 @@ class PhotoColorizer(object):
             raise ValueError("caffe_dist=True needs caffe=True: the 313-bin head belongs to the Caffe checkpoint")
         if caffe_dist and global_hints:
             raise ValueError("caffe_dist=True excludes global_hints=True: the global model has no 313-bin head")
-        if caffe_dist:
-            missing = [k for k in CAFFE313_KEYS if k not in state_dict]
-            if missing:
-                raise ValueError("caffe_dist=True needs the checkpoint's 313-bin head: it has no %r" % missing[0])
         self.Xd, self.batch, self.device = int(Xd), int(batch), int(device)
         self.maskcent, self.global_hints, self.engine = bool(maskcent), bool(global_hints), engine
         self.caffe, self.dist, self.caffe_dist = bool(caffe), bool(suggest), bool(caffe_dist)
         self.options = {"tanh_scale": 100} if self.caffe else None
+        if self.world == 1:
+            return None
+        import torch
+        # None without CUDA, where no device pass can run: only colorizers with a fake backend get that far
+        sms = torch.cuda.get_device_properties(self.device).multi_processor_count if torch.cuda.is_available() else None
+        return dict(Xd=self.Xd, batch=self.batch, maskcent=self.maskcent, global_hints=self.global_hints,
+                    engine=self.engine, caffe=self.caffe, suggest=self.dist, caffe_dist=self.caffe_dist,
+                    options=self.options, sms=sms)
+
+    def _load(self, state_dict, calibrate):
+        """The checks of the checkpoint and the calibration, rank 0's alone in a job of many -> the state_dict as the
+        context loads it; sets act_ranges."""
+        if self.caffe_dist:
+            missing = [k for k in CAFFE313_KEYS if k not in state_dict]
+            if missing:
+                raise ValueError("caffe_dist=True needs the checkpoint's 313-bin head: it has no %r" % missing[0])
         if self.caffe:
             from .colorize_image import caffe_scaled_state_dict
             state_dict = caffe_scaled_state_dict(state_dict)
@@ -346,11 +393,14 @@ class PhotoColorizer(object):
             import torch
             from .prepost import pts_in_hull
             state_dict["caffe.pts_in_hull"] = torch.from_numpy(pts_in_hull())
-        self.max_batch_bytes = int(max_batch_bytes)
-        self.readahead = int(readahead) if readahead else 2 * self.batch
-        self.workers = int(workers)
         self.act_ranges = self._calibrate(calibrate, state_dict)
-        self._backend = self._make_backend(state_dict)
+        return state_dict
+
+    def local_slice(self, n):
+        """(start, count): the photos of an n-photo job this rank processes, photos[start:start + count]
+        (parallel.shard_range; (0, n) on a single process)."""
+        from .parallel import shard_range
+        return shard_range(n, self.world, self.rank)
 
     def _calibrate(self, calibrate, state_dict):
         X, dev, glob = self.Xd, self.device, self.global_hints
@@ -486,8 +536,10 @@ class PhotoColorizer(object):
         return out
 
     def _batches(self, photos, per_pass, hints=None):
-        """The photos, decoded `readahead` ahead of the consumer, cut into device passes of at most per_pass photos,
-        max_batch_bytes source bytes and IDC_MAX_HINTS hints -> (indices, photo arrays) per pass, in input order."""
+        """This rank's photos (local_slice), decoded `readahead` ahead of the consumer, cut into device passes of at
+        most per_pass photos, max_batch_bytes source bytes and IDC_MAX_HINTS hints -> (indices into photos, photo
+        arrays) per pass, in input order."""
+        start, count = self.local_slice(len(photos))
         def load(i):
             p = photos[i]
             if isinstance(p, np.ndarray):
@@ -495,7 +547,7 @@ class PhotoColorizer(object):
             return i, check_photo(read_photo(p), "photo %d (%s)" % (i, p))
 
         def items():
-            for i, a in read_ahead(range(len(photos)), load, self.readahead, self.workers):
+            for i, a in read_ahead(range(start, start + count), load, self.readahead, self.workers):
                 yield a.nbytes, 0 if hints is None or hints[i] is None else hints[i].shape[0], (i, a)
 
         for b in cut_batches(items(), per_pass, self.max_batch_bytes):
@@ -644,7 +696,8 @@ _Batch = collections.namedtuple("_Batch", "slot serial n V info")
 
 
 class _DeviceBatches(object):
-    """Device side of PhotoColorizer: one LhnContext (max_n = batch) and two _Slots of batch buffers.  submit() packs
+    """Device side of PhotoColorizer: one LhnContext (max_n = batch; its weights loaded, or received from rank 0 in a
+    job of many ranks) and two _Slots of batch buffers.  submit() packs
     and enqueues a batch on slot k % 2 and returns; collect() waits for that batch's copies and returns its results.
     submit() first waits until the slot's previous batch is off the device, so a slot is never overwritten while a
     kernel or a copy still uses it, whether or not that batch was collected; collecting a batch whose slot has been
@@ -659,9 +712,10 @@ class _DeviceBatches(object):
         from . import prepost
         self.torch, self.lib = torch, _lib.load()
         self.X, self.batch, self.device, self.maskcent, self.caffe313 = X, batch, device, maskcent, caffe313
-        self.ctx = engine.LhnContext(device=device, max_n=batch, H=X, W=X, engine=engine_name, global_hints=global_hints,
-                                     options=options, dist=dist, caffe313=caffe313)
-        self.ctx.load_state_dict(state_dict, act_ranges=act_ranges)
+        from .parallel import share_weights
+        self.ctx = share_weights(lambda: engine.LhnContext(device=device, max_n=batch, H=X, W=X, engine=engine_name,
+                                                           global_hints=global_hints, options=options, dist=dist,
+                                                           caffe313=caffe313), state_dict, act_ranges, device)
         self.dev = torch.device("cuda:%d" % device)
         self.s_in, self.s_comp, self.s_out = (torch.cuda.Stream(self.dev) for _ in range(3))
         f32 = torch.float32

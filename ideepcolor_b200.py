@@ -32,7 +32,10 @@ PSNR against the number of hint points revealed from each photo's own colours (p
 <out>/reveal_psnr.csv with no images:
 
     python ideepcolor_b200.py --color_model caffemodel.pth --image_dir val/ --out sweep/ --reveal_sweep 0,1,2,5,10,20,50
-        [--reveal_seed 0] [--batch 60]
+        [--reveal_seed 0] [--batch 60] [--reveal_levin]
+
+--reveal_levin also writes <out>/reveal_psnr_levin.csv, the same sweep with the network replaced by the classical
+baseline, colorization by optimization (Levin et al. 2004) on the same revealed points (DESIGN.md §4b).
 
 With a global-hints checkpoint (--global_hints: the glob.* keys; --caffe: Caffe-scaled weights such as the global
 model's), every photo of the folder coloured with a reference photo's ab histogram (DemoGlobalHistogramTransfer.ipynb),
@@ -90,6 +93,9 @@ def parse_args(argv=None):
                     help="with --image_dir: PSNR of every photo against the number of hint points revealed from its own "
                          "colours, one column per level, into <out>/reveal_psnr.csv (no images are written)")
     ap.add_argument("--reveal_seed", type=int, default=None, help="seed of the revealed points (--reveal_sweep; default 0)")
+    ap.add_argument("--reveal_levin", action="store_true",
+                    help="with --reveal_sweep: also the classical baseline, colorization by optimization on the same "
+                         "revealed points, into <out>/reveal_psnr_levin.csv")
     ap.add_argument("--global_hints", action="store_true",
                     help="the checkpoint has the global-hints branch (glob.* keys; --image_dir)")
     ap.add_argument("--caffe", action="store_true",
@@ -151,6 +157,8 @@ def parse_args(argv=None):
             ap.error("--reveal_sweep: %s" % e)
     elif args.reveal_seed is not None:
         ap.error("--reveal_seed needs --reveal_sweep")
+    elif args.reveal_levin:
+        ap.error("--reveal_levin needs --reveal_sweep")
     if args.reveal_seed is None:
         args.reveal_seed = 0
     args.calibrate_source = None
@@ -395,13 +403,21 @@ def write_sweep(args, pc, names, csv, labels, results, title, line):
     """A sweep's PSNR, one result per photo -> OUT/<csv> (a row per photo, a column per label, then the mean row), and
     `title` and the mean per label (`line` % (label, mean)) on stdout; closes pc.  names: every photo's; results: those
     of this process's photos."""
-    rows = []
-    for name, r in zip(my_names(pc, names), results):
-        rows.append(([name] + ["%.17g" % v for v in r.psnr], r.psnr))
+    rows = sweep_rows(pc, names, results)
     pc.close()
     rows = merge_rows(args, rows)
-    if rows is None:
-        return 0
+    if rows is not None:
+        write_sweep_csv(args, csv, labels, rows, title, line)
+    return 0
+
+
+def sweep_rows(pc, names, results):
+    """A sweep's results for this process's photos -> its rows ([name, PSNR text...], psnr curve)."""
+    return [([name] + ["%.17g" % v for v in r.psnr], r.psnr) for name, r in zip(my_names(pc, names), results)]
+
+
+def write_sweep_csv(args, csv, labels, rows, title, line):
+    """Every photo's sweep rows -> OUT/<csv> and the mean curve on stdout (write_sweep)."""
     curves = [c for _, c in rows]
     rows = [row for row, _ in rows]
     mean = np.mean(curves, axis=0) if curves else np.full(len(labels), np.nan)
@@ -411,17 +427,28 @@ def write_sweep(args, pc, names, csv, labels, results, title, line):
     print(title)
     for c, v in zip(labels, mean):
         print(line % (c, v))
-    return 0
 
 
 def reveal_dir(args, pc, names, paths):
     """--reveal_sweep: PhotoColorizer.reveal_sweep over the folder -> OUT/reveal_psnr.csv, and the mean curve on
-    stdout."""
+    stdout; with --reveal_levin first the Levin baseline's sweep -> OUT/reveal_psnr_levin.csv."""
     levels = args.reveal_levels
-    return write_sweep(args, pc, names, "reveal_psnr.csv", levels,
-                       pc.reveal_sweep(paths, levels=levels, seed=args.reveal_seed),
-                       "reveal sweep of %d photos (seed %d), mean PSNR per number of revealed points:"
-                       % (len(names), args.reveal_seed), "  %4d  %.3f dB")
+    title = ("reveal sweep of %d photos (seed %d), mean PSNR per number of revealed points:"
+             % (len(names), args.reveal_seed))
+    if not args.reveal_levin:
+        return write_sweep(args, pc, names, "reveal_psnr.csv", levels,
+                           pc.reveal_sweep(paths, levels=levels, seed=args.reveal_seed), title, "  %4d  %.3f dB")
+    # both sweeps' rows travel in one gather, the job's last collective
+    rows = [(0, r) for r in sweep_rows(pc, names, pc.reveal_sweep(paths, levels=levels, seed=args.reveal_seed))]
+    rows += [(1, r) for r in sweep_rows(pc, names, pc.reveal_sweep(paths, levels=levels, seed=args.reveal_seed,
+                                                                    method="levin"))]
+    pc.close()
+    rows = merge_rows(args, rows)
+    if rows is not None:
+        write_sweep_csv(args, "reveal_psnr.csv", levels, [r for k, r in rows if k == 0], title, "  %4d  %.3f dB")
+        write_sweep_csv(args, "reveal_psnr_levin.csv", levels, [r for k, r in rows if k == 1],
+                        "Levin baseline (colorization by optimization) on the same points:", "  %4d  %.3f dB")
+    return 0
 
 
 def glob_sweep_dir(args, pc, names, paths):

@@ -397,6 +397,42 @@ int idc_hint_fill_mean(int device, int n_blocks, int levels, int X, const double
 int idc_global_stats_batch(int device, int n, int h, int w, const uint8_t* rgb, const float* pts313, float* out,
                            void* stream);
 
+/* Colorization by optimization (Levin, Lischinski & Weiss, SIGGRAPH 2004) on a reveal sweep's hint planes: the
+ * classical baseline of PhotoColorizer.reveal_sweep(method="levin"); the rule is DESIGN.md §4b's.  DEVICE pointers,
+ * asynchronous on `stream`.
+ * idc_levin_weights: lab [n,3,h,w] float64 (idc_rgb2lab_f64) -> wts [n,8,h,w] float64.  With Y = L / 100 and N(p) the
+ *   3 x 3 window around p without p, clipped to the image: s = max(0.6 * var(Y over N(p) and p), -min_q (Y(q) - Y(p))^2
+ *   / ln 0.01, 2e-6), w_pq = exp(-(Y(q) - Y(p))^2 / s) normalised to sum 1 over N(p).  Plane k holds neighbour
+ *   (y + dy, x + dx) with (dy, dx) the k-th of (-1,-1) (-1,0) (-1,1) (0,-1) (0,1) (1,-1) (1,0) (1,1); 0 outside the
+ *   image.  Each operation rounded on its own.  IDC_ERR_ARG, before any device call, for n outside [1, 65535], h or w
+ *   outside [2, IDC_MAX_PHOTO_X] and a NULL pointer. */
+int idc_levin_weights(int device, int n, int h, int w, const double* lab, double* wts, void* stream);
+/* idc_levin_solve: for each image i of n and each channel c of ab, the u with u_p = ab_hint[i,c,p] where mask[i,0,p] > 0
+ *   and u_p - sum_q w_pq u_q = 0 elsewhere, w being photo i / levels of wts -> out_ab [n,2,h,w] float32 (the hints as
+ *   they are on hinted pixels).  FP64 BiCGSTAB from u = 0 on the system reduced to the free pixels, one CTA per image,
+ *   the iterations on the device.  A channel stops when its true relative residual ||b - A u|| / ||b|| (b = the hinted
+ *   columns moved to the right) is at most tol, or after max_iter iterations; iters [n,2] int32 and relres [n,2]
+ *   float64 receive each channel's iteration count and the true relative residual it stopped at (0 for b = 0: an image
+ *   without hints, or whose hints no free pixel depends on, gets u = 0 exactly).  Free pixels that depend on no hint
+ *   through non-zero weights get 0 (DESIGN.md §4b).  relres > tol after the call means "not converged".  Every sum in a
+ *   fixed order: an image's result is the same bit for bit whatever n, its position and the other images.  ab_hint
+ *   [n,2,h,w] and mask [n,1,h,w] float32 as idc_hint_raster writes them.  workspace: idc_levin_workspace_bytes(n, h, w)
+ *   bytes of DEVICE scratch, 8-byte aligned, owned by the caller; nothing is allocated.  IDC_ERR_ARG, before any device
+ *   call (idc_levin_check runs the same checks, in this order): n outside [1, 65535], h or w outside
+ *   [2, IDC_MAX_PHOTO_X], levels outside [1, n], a NULL wts, ab_hint, mask, out_ab, iters, relres or workspace, tol not
+ *   in (0, 1), max_iter outside [1, IDC_LEVIN_MAX_ITER], a workspace not 8-byte aligned, and workspace_bytes below
+ *   idc_levin_workspace_bytes(n, h, w).
+ * idc_levin_workspace_bytes: the workspace idc_levin_solve needs for n images of h x w; 0 for sizes it rejects.
+ * idc_lab2rgb_u8_mc: the render of idc_forward's out_rgb on caller planes, L = (double)L_mc + 50 with L_mc [n,1,h,w]
+ *   (idc_forward's mean-centred L input) and ab [n,2,h,w] float32 -> rgb [n,h,w,3] uint8: the network's own ab gives
+ *   its out_rgb bit for bit.  IDC_ERR_ARG for n, h or w below 1 and a NULL pointer. */
+#define IDC_LEVIN_MAX_ITER 10000000
+int idc_levin_solve(int device, int n, int levels, int h, int w, const double* wts, const float* ab_hint,
+                    const float* mask, double tol, int max_iter, float* out_ab, int32_t* iters, double* relres,
+                    void* workspace, size_t workspace_bytes, void* stream);
+size_t idc_levin_workspace_bytes(int n, int h, int w);
+int idc_lab2rgb_u8_mc(int device, int n, int h, int w, const float* L_mc, const float* ab, uint8_t* rgb, void* stream);
+
 /* ---- introspection / test hooks (used by tests/, never by the product path) ---- */
 /* The host argument checks of idc_ab_reccs_batch, the same code, for a context with (has_head != 0) or without the
  * 529-bin head whose last forward carried n_img images of h x w (n_img = 0: no forward yet) -> the code
@@ -406,6 +442,11 @@ int idc_ab_reccs_batch_check(int has_head, int n_img, int h, int w, int q, const
 /* The same for idc_caffe313_reccs_batch: has_head = the context has IDC_FLAG_CAFFE313; queries on the h x w grid. */
 int idc_caffe313_reccs_batch_check(int has_head, int n_img, int h, int w, int q, const int32_t* queries, float S, int K,
                                    int max_iter, int n_init, char* msg, size_t msg_bytes);
+/* The host argument checks of idc_levin_solve, the same code -> the code idc_levin_solve returns for these arguments;
+ * msg (may be NULL) receives the reason.  The pointers are only tested for NULL and alignment.  Touches no device. */
+int idc_levin_check(int n, int levels, int h, int w, const double* wts, const float* ab_hint, const float* mask,
+                    double tol, int max_iter, const float* out_ab, const int32_t* iters, const double* relres,
+                    const void* workspace, size_t workspace_bytes, char* msg, size_t msg_bytes);
 /* wgmma engine: the exponent S with which activation `name` is stored (FP16 hi/lo planes of value * 2^S), chosen per
  * buffer from the weights by idc_finalize_weights (DESIGN.md §3); 0 on the SIMT engine.  IDC_ERR_KEY for an unknown
  * name, IDC_ERR_STATE before the weights are packed. */

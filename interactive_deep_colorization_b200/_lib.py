@@ -30,6 +30,7 @@ MAX_PHOTOS = 128                      # IDC_MAX_PHOTOS
 MAX_PHOTO_SIDE = 1 << 24               # IDC_MAX_PHOTO_SIDE
 MAX_PHOTO_X = 16384                   # IDC_MAX_PHOTO_X
 MAX_RECCS_QUERIES = 65535             # IDC_MAX_RECCS_QUERIES
+LEVIN_MAX_ITER = 10000000             # IDC_LEVIN_MAX_ITER
 HINT_HDR_BYTES = 16                   # header {count, 0, 0, 0} of an idc_hint_raster block
 # idc_photo: a photo of a packed batch, its first pixel and its size
 PHOTO_DTYPE = np.dtype([("off", "<i8"), ("h", "<i4"), ("w", "<i4")])
@@ -90,6 +91,13 @@ SYMBOLS = [
     ("idc_rgb_sse", _c.c_int, [_c.c_int, _c.c_int, _c.c_int, _c.c_int, _P, _P, _P, _P]),
     ("idc_hint_fill_mean", _c.c_int, [_c.c_int, _c.c_int, _c.c_int, _c.c_int, _P, _P, _c.c_size_t, _P]),
     ("idc_global_stats_batch", _c.c_int, [_c.c_int, _c.c_int, _c.c_int, _c.c_int, _P, _P, _P, _P]),
+    ("idc_levin_weights", _c.c_int, [_c.c_int, _c.c_int, _c.c_int, _c.c_int, _P, _P, _P]),
+    ("idc_levin_solve", _c.c_int, [_c.c_int, _c.c_int, _c.c_int, _c.c_int, _c.c_int, _P, _P, _P, _c.c_double, _c.c_int,
+                                   _P, _P, _P, _P, _c.c_size_t, _P]),
+    ("idc_levin_workspace_bytes", _c.c_size_t, [_c.c_int, _c.c_int, _c.c_int]),
+    ("idc_levin_check", _c.c_int, [_c.c_int, _c.c_int, _c.c_int, _c.c_int, _P, _P, _P, _c.c_double, _c.c_int, _P, _P,
+                                   _P, _P, _c.c_size_t, _P, _c.c_size_t]),
+    ("idc_lab2rgb_u8_mc", _c.c_int, [_c.c_int, _c.c_int, _c.c_int, _c.c_int, _P, _P, _P, _P]),
     ("idc_get_activation", _c.c_int, [_P, _c.c_char_p, _P, _c.c_size_t, _c.POINTER(_c.c_int),
                                       _c.POINTER(_c.c_int), _c.POINTER(_c.c_int)]),
     ("idc_set_activation", _c.c_int, [_P, _c.c_char_p, _c.c_int, _P]),

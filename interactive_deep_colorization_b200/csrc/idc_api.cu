@@ -1699,6 +1699,75 @@ int idc_rgb_sse(int device, int n, int h, int w, const uint8_t* a, const uint8_t
   return launch_rgb_sse(n, (size_t)h * w * 3, a, b, sse, (cudaStream_t)stream) == cudaSuccess ? IDC_OK : IDC_ERR_CUDA;
 }
 
+int idc_lab2rgb_u8_mc(int device, int n, int h, int w, const float* L_mc, const float* ab, uint8_t* rgb, void* stream) {
+  if (n < 1 || h < 1 || w < 1 || !L_mc || !ab || !rgb) return IDC_ERR_ARG;
+  if (cudaSetDevice(device) != cudaSuccess) return IDC_ERR_CUDA;
+  return launch_lab2rgb(nullptr, n, h, w, L_mc, 50.0f, ab, rgb, (cudaStream_t)stream) == cudaSuccess ? IDC_OK
+                                                                                                    : IDC_ERR_CUDA;
+}
+
+static bool levin_size_ok(int n, int h, int w) {
+  return n >= 1 && n <= 65535 && h >= 2 && w >= 2 && h <= IDC_MAX_PHOTO_X && w <= IDC_MAX_PHOTO_X;
+}
+
+size_t idc_levin_workspace_bytes(int n, int h, int w) {
+  return levin_size_ok(n, h, w) ? levin_workspace_bytes(n, h, w) : 0;
+}
+
+int idc_levin_weights(int device, int n, int h, int w, const double* lab, double* wts, void* stream) {
+  if (!levin_size_ok(n, h, w) || !lab || !wts) return IDC_ERR_ARG;
+  if (cudaSetDevice(device) != cudaSuccess) return IDC_ERR_CUDA;
+  return launch_levin_weights(n, h, w, lab, wts, (cudaStream_t)stream) == cudaSuccess ? IDC_OK : IDC_ERR_CUDA;
+}
+
+// the argument checks of idc_levin_solve, in the order include/idc_b200.h lists them
+static int levin_check(int n, int levels, int h, int w, const void* wts, const void* ab_hint, const void* mask,
+                       double tol, int max_iter, const void* out_ab, const void* iters, const void* relres,
+                       const void* workspace, size_t workspace_bytes, char* msg, size_t cap) {
+  if (!levin_size_ok(n, h, w))
+    return snprintf(msg, cap, "idc_levin_solve: n = %d, h = %d, w = %d: need n in [1, 65535], h and w in [2, %d]", n, h,
+                    w, IDC_MAX_PHOTO_X), IDC_ERR_ARG;
+  if (levels < 1 || levels > n)
+    return snprintf(msg, cap, "idc_levin_solve: levels = %d outside [1, n = %d]", levels, n), IDC_ERR_ARG;
+  const struct { const void* p; const char* name; } ptrs[] = {{wts, "wts"}, {ab_hint, "ab_hint"}, {mask, "mask"},
+      {out_ab, "out_ab"}, {iters, "iters"}, {relres, "relres"}, {workspace, "workspace"}};
+  for (const auto& e : ptrs)
+    if (!e.p) return snprintf(msg, cap, "idc_levin_solve: NULL %s", e.name), IDC_ERR_ARG;
+  if (!std::isfinite(tol) || !(tol > 0.0) || !(tol < 1.0))
+    return snprintf(msg, cap, "idc_levin_solve: tol = %g outside (0, 1)", tol), IDC_ERR_ARG;
+  if (max_iter < 1 || max_iter > IDC_LEVIN_MAX_ITER)
+    return snprintf(msg, cap, "idc_levin_solve: max_iter = %d outside [1, %d]", max_iter, IDC_LEVIN_MAX_ITER),
+           IDC_ERR_ARG;
+  if ((uintptr_t)workspace % 8)
+    return snprintf(msg, cap, "idc_levin_solve: workspace not 8-byte aligned"), IDC_ERR_ARG;
+  const size_t need = levin_workspace_bytes(n, h, w);
+  if (workspace_bytes < need)
+    return snprintf(msg, cap, "idc_levin_solve: workspace of %zu bytes, need %zu", workspace_bytes, need), IDC_ERR_ARG;
+  return IDC_OK;
+}
+
+int idc_levin_check(int n, int levels, int h, int w, const double* wts, const float* ab_hint, const float* mask,
+                    double tol, int max_iter, const float* out_ab, const int32_t* iters, const double* relres,
+                    const void* workspace, size_t workspace_bytes, char* msg, size_t msg_bytes) {
+  char buf[256];
+  const int rc = levin_check(n, levels, h, w, wts, ab_hint, mask, tol, max_iter, out_ab, iters, relres, workspace,
+                             workspace_bytes, buf, sizeof(buf));
+  if (rc != IDC_OK && msg && msg_bytes) snprintf(msg, msg_bytes, "%s", buf);
+  return rc;
+}
+
+int idc_levin_solve(int device, int n, int levels, int h, int w, const double* wts, const float* ab_hint,
+                    const float* mask, double tol, int max_iter, float* out_ab, int32_t* iters, double* relres,
+                    void* workspace, size_t workspace_bytes, void* stream) {
+  char msg[256];
+  if (levin_check(n, levels, h, w, wts, ab_hint, mask, tol, max_iter, out_ab, iters, relres, workspace,
+                  workspace_bytes, msg, sizeof(msg)) != IDC_OK)
+    return IDC_ERR_ARG;
+  if (cudaSetDevice(device) != cudaSuccess) return IDC_ERR_CUDA;
+  return launch_levin_solve(n, levels, h, w, wts, ab_hint, mask, tol, max_iter, out_ab, iters, relres, workspace,
+                            (cudaStream_t)stream) == cudaSuccess ? IDC_OK : IDC_ERR_CUDA;
+}
+
 int idc_act_exponent(idc_ctx* c, const char* name, int* exp_out) {
   if (!c || !name || !exp_out) return IDC_ERR_ARG;
   auto it = c->buf_index.find(name);

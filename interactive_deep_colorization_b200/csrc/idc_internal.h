@@ -351,6 +351,12 @@ cudaError_t launch_hint_fill_mean(int n_blocks, int levels, int X, const double*
 // n in [1, 65535], h and w multiples of 4 in [4, IDC_MAX_PHOTO_X], checked by the caller
 cudaError_t launch_global_stats_batch(int n, int h, int w, const uint8_t* rgb, const float* pts, float* out,
                                       cudaStream_t st);
+// colorization by optimization (idc_levin.cu); arguments checked by the caller (levin_check in idc_api.cu)
+size_t levin_workspace_bytes(int n, int h, int w);
+cudaError_t launch_levin_weights(int n, int h, int w, const double* lab, double* wts, cudaStream_t st);
+cudaError_t launch_levin_solve(int n, int levels, int h, int w, const double* wts, const float* ab_hint,
+                               const float* mask, double tol, int max_iter, float* out_ab, int32_t* iters,
+                               double* relres, void* workspace, cudaStream_t st);
 cudaError_t launch_global_mlp(Ctx* c, int n, const float* glob, cudaStream_t st);
 cudaError_t launch_act_to_nchw(Ctx* c, const ActBuf& b, int n, float* out, cudaStream_t st);
 cudaError_t launch_nchw_to_act(Ctx* c, const ActBuf& b, int n, const float* in, cudaStream_t st);

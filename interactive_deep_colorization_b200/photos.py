@@ -30,6 +30,12 @@ conditions of GLOBAL_CONDITIONS, every condition of a photo in the same device p
 The two sweeps are one pass from the repeat of L and img_rgb on; they differ only in how they make the forward's ab /
 mask planes and glob rows.
 
+`PhotoColorizer.reveal_sweep(method="levin")` is the classical baseline of the reveal curve, colorization by
+optimization (Levin et al. 2004; DESIGN.md §4b) on exactly the hint planes, Lab and PSNR rule the network sweep uses:
+
+    H2D -> ... -> idc_hint_raster per image (as above) -> L and img_rgb repeated once per level -> idc_levin_weights
+    (once per photo) -> idc_levin_solve (every level of every photo) -> idc_lab2rgb_u8_mc -> idc_rgb_sse -> D2H
+
 `PhotoColorizer.suggest` (a colorizer made with suggest=True, whose context carries the 529-bin distribution head)
 colours every photo with its hints as `colorize(hints=...)` does and also answers the GUI palette's question, the K
 colour suggestions get_ab_reccs(h, w, K) gives, at each photo's query points, on the distribution of that photo's own
@@ -78,6 +84,11 @@ GlobalSweepResult.__doc__ = """One photo of a global-hints sweep, over the C con
 
 XFULLRES_MAX = 10000          # the wrapper's Xfullres_max (ColorizeImageBase): larger photos are resized on the host
 REVEAL_LEVELS = (0, 1, 2, 5, 10, 20, 50, 100, 200, 500)
+REVEAL_METHODS = ("network", "levin")
+# idc_levin_solve's stopping rule for reveal_sweep(method="levin"): the true relative residual, and the iteration budget
+# (DESIGN.md §4b, from tools/levin_profile.py's measured counts with margin)
+LEVIN_TOL = 1e-10
+LEVIN_MAX_ITER = 20000
 # The paper's global-hints evaluation: no hints, the photo's own saturation, its own histogram, both.
 GLOBAL_CONDITIONS = ("none", "sat", "hist", "hist+sat")
 # Which entries of a [316] statistics row each condition keeps (the others are 0): the histogram with its indicator
@@ -466,25 +477,47 @@ class PhotoColorizer(object):
             raise ValueError("photo %d: a point lies outside the %d x %d network grid" % (i, self.Xd, self.Xd))
         return p.astype(np.int64)
 
-    def reveal_sweep(self, photos, levels=REVEAL_LEVELS, seed=0):
+    def reveal_sweep(self, photos, levels=REVEAL_LEVELS, seed=0, method="network", levin_tol=LEVIN_TOL,
+                     levin_max_iter=LEVIN_MAX_ITER):
         """PSNR against the number of revealed hint points: for every photo and every level m, the network-size result
         with the first m points of reveal_points(Xd, max(levels), seed, i) (i = the photo's position in `photos`) as
         hints, each painted with the photo's mean ground-truth ab under it (idc_hint_fill_mean, the Lab of the
         network-size photo).  A device pass carries batch // len(levels) photos, each as len(levels) consecutive forward
         images; nothing is rendered at full resolution.
+        method "levin": the same hint planes propagated by colorization by optimization (Levin et al. 2004, DESIGN.md
+        §4b) instead of the network: ab is the solve's result (the hints on hinted pixels), rgb its render with the
+        photo's L as output_rgb renders the network's ab, psnr by the same rule.  Each image and channel is solved to a
+        true relative residual of levin_tol within levin_max_iter iterations; one that is not raises RuntimeError naming
+        the photo and the level.
         photos: as colorize.  levels: distinct integers in [0, IDC_MAX_HINTS], at most `batch` of them.
-        -> iterator of RevealResult, in input order.  Bad levels or photos raise ValueError here, before any device
-        work (paths as in colorize)."""
+        -> iterator of RevealResult, in input order.  Bad levels, photos or options raise ValueError here, before any
+        device work (paths as in colorize)."""
         levels = check_levels(levels, self.batch)
         if self.Xd < 9:
             raise ValueError("reveal_sweep needs Xd >= 9 for a 9 x 9 patch, got %d" % self.Xd)
+        if method not in REVEAL_METHODS:
+            raise ValueError("method must be one of %s, got %r" % (REVEAL_METHODS, method))
+        levin = None
+        if method == "levin":
+            levin_tol = float(levin_tol)
+            if not 0.0 < levin_tol < 1.0:
+                raise ValueError("levin_tol must be in (0, 1), got %r" % levin_tol)
+            if isinstance(levin_max_iter, (bool, np.bool_)) or not isinstance(levin_max_iter, (int, np.integer)) \
+                    or not 1 <= levin_max_iter <= _lib.LEVIN_MAX_ITER:
+                raise ValueError("levin_max_iter must be an integer in [1, %d], got %r"
+                                 % (_lib.LEVIN_MAX_ITER, levin_max_iter))
+            levin = (levin_tol, int(levin_max_iter))
         self._check_photos(photos)
         seed = int(seed)
         M = max(levels)
-        return self._pipeline(self._batches(photos, self.batch // len(levels)),
-                              lambda idx, imgs: self._backend.submit_reveal(
-                                  imgs, [reveal_points(self.Xd, M, seed, i) for i in idx], levels),
-                              self._backend.collect_reveal)
+
+        def submit(idx, imgs):
+            points = [reveal_points(self.Xd, M, seed, i) for i in idx]
+            if levin is None:
+                return self._backend.submit_reveal(imgs, points, levels)
+            return self._backend.submit_reveal(imgs, points, levels, levin=levin + (idx,))
+
+        return self._pipeline(self._batches(photos, self.batch // len(levels)), submit, self._backend.collect_reveal)
 
     def global_stats(self, photos):
         """The global-hints statistics of every photo: the float32 [316] row [313-bin ab histogram, 1, s_avg, 1] of the
@@ -682,6 +715,8 @@ class _Slot(object):
         self.cen = _Twin(b, (2,), f32)                    # suggest: queries x K centres and their masses
         self.conf = _Twin(b, (), f32)
         self.blocks = _Twin(b, (), u8)                    # reveal sweeps: one hint block per forward image
+        self.iters = _Twin(b, (2,), torch.int32)          # Levin reveal sweeps: per image and channel
+        self.relres = _Twin(b, (2,), torch.float64)
         self.ev_in, self.ev_comp, self.ev_out = (torch.cuda.Event() for _ in range(3))
 
     def free(self):
@@ -727,6 +762,10 @@ class _DeviceBatches(object):
         self.rgb_photo = _Twin(self, (X, X, 3), torch.uint8, hosts=0)
         self.pts313 = _Twin(self, (2,), f32, 313, hosts=0, init=prepost.pts_in_hull()).dev    # the 313 ab bin centres
         self.zero = _Twin(self, (), f32, 1, hosts=0, init=np.zeros(1, np.float32)).dev[0]
+        # Levin reveal sweeps: each photo's weights and the solver's workspace, made on the first such sweep
+        self.levin_wts = _Twin(self, (8, X, X), torch.float64, hosts=0)
+        self.levin_ws = _Twin(self, (), torch.uint8, hosts=0)
+        self.levin_log = None                   # a list to append each collected photo's iters [V,2] to (tools)
         self.keep = {}                          # conditions -> [C,316] bool: the entries each keeps (_GLOB_KEEP)
         self.max_bytes = max_bytes
         self.slots = [_Slot(self) for _ in range(2)]
@@ -858,23 +897,33 @@ class _DeviceBatches(object):
         return [SuggestResult(r, cen[e - c:e].astype(np.float64), conf[e - c:e].astype(np.float64))
                 for r, c, e in zip(out, counts, ends)]
 
-    def _submit_sweep(self, photos, V, fill):
+    def _submit_sweep(self, photos, V, fill, levin=None):
         """One device pass of a sweep: photo i of the batch is forward images i*V .. i*V+V-1 (V variants: the levels or
         the conditions), each with the photo's prepared L and img_rgb.  fill(s, m, table, nbytes) uploads the batch,
         preps its m photos into L_photo / rgb_photo and makes the forward's ab / mask planes on the compute stream; it
-        returns the forward's glob rows (or None) and the (buffer, rows) it adds to the D2H of ab, rgb and SSE."""
+        returns the forward's glob rows (or None) and the (buffer, rows) it adds to the D2H of ab, rgb and SSE.
+        levin: None, or (tol, max_iter): the Levin solve on those planes in place of the forward (_levin)."""
         torch, lib, X = self.torch, self.lib, self.X
         m = len(photos)
         N = m * V
         self.L_photo.grow(self.batch)
         self.rgb_photo.grow(self.batch)
         s, table, nbytes = self._next_slot(photos)
+        if levin is not None:                  # allocated outside the compute stream, like every other buffer
+            self.levin_wts.grow(self.batch)
+            self.levin_ws.grow(self.lib.idc_levin_workspace_bytes(self.batch, X, X))
+            s.iters.grow(self.batch)
+            s.relres.grow(self.batch)
         glob, extra = fill(s, m, table, nbytes)
         with torch.cuda.stream(self.s_comp):
             self.L_mc[:N].view(m, V, 1, X, X).copy_(self.L_photo.dev[:m, None].expand(m, V, 1, X, X))
             s.img_rgb.dev[:N].view(m, V, X, X, 3).copy_(self.rgb_photo.dev[:m, None].expand(m, V, X, X, 3))
-            self.ctx.forward_device(self.L_mc[:N], self.ab_in[:N], self.mask[:N], self.maskcent, glob=glob,
-                                    want_rgb=True, out_ab=s.ab.dev[:N], out_rgb=s.rgb.dev[:N])
+            if levin is None:
+                self.ctx.forward_device(self.L_mc[:N], self.ab_in[:N], self.mask[:N], self.maskcent, glob=glob,
+                                        want_rgb=True, out_ab=s.ab.dev[:N], out_rgb=s.rgb.dev[:N])
+            else:
+                self._levin(s, m, V, *levin)
+                extra = list(extra) + [(s.iters, N), (s.relres, N)]
             _lib.check(None, lib.idc_rgb_sse(self.device, N, X, X, s.img_rgb.dev.data_ptr(), s.rgb.dev.data_ptr(),
                                              s.sse.dev.data_ptr(), self.s_comp.cuda_stream))
         self._download(s, (s.ab, N), (s.rgb, N), (s.sse, N), *extra)
@@ -890,9 +939,24 @@ class _DeviceBatches(object):
             out.append((np.array([_psnr(e, self.X) for e in sse[k]], np.float64), ab[k].copy(), rgb[k].copy()))
         return out
 
-    def submit_reveal(self, photos, points, levels):
+    def _levin(self, s, m, V, tol, max_iter):
+        """On the compute stream, for the m photos whose Lab fill left in lab and their m * V images' ab_in / mask and
+        L_mc: idc_levin_weights (once per photo) -> idc_levin_solve into the slot's ab, iters and relres ->
+        idc_lab2rgb_u8_mc into the slot's rgb."""
+        lib, X, N, sh = self.lib, self.X, m * V, self.s_comp.cuda_stream
+        ws_bytes = self.levin_ws.rows
+        wts = self.levin_wts.dev.data_ptr()
+        _lib.check(None, lib.idc_levin_weights(self.device, m, X, X, self.lab.data_ptr(), wts, sh))
+        _lib.check(None, lib.idc_levin_solve(self.device, N, V, X, X, wts, self.ab_in.data_ptr(), self.mask.data_ptr(),
+                                             tol, max_iter, s.ab.dev.data_ptr(), s.iters.dev.data_ptr(),
+                                             s.relres.dev.data_ptr(), self.levin_ws.dev.data_ptr(), ws_bytes, sh))
+        _lib.check(None, lib.idc_lab2rgb_u8_mc(self.device, N, X, X, self.L_mc.data_ptr(), s.ab.dev.data_ptr(),
+                                               s.rgb.dev.data_ptr(), sh))
+
+    def submit_reveal(self, photos, points, levels, levin=None):
         """One device pass of a reveal sweep: image i*L+j of the sweep (L = len(levels)) has the first levels[j] rows of
-        points[i] as hints, coloured with the mean ground-truth ab under each (idc_hint_fill_mean)."""
+        points[i] as hints, coloured with the mean ground-truth ab under each (idc_hint_fill_mean).  levin: None (the
+        network), or (tol, max_iter, indices of the photos in the sweep) for the Levin baseline on the same planes."""
         lib, X, L = self.lib, self.X, len(levels)
         # the points as hint rectangles; their colours are filled on the device
         pts = np.stack(points)
@@ -914,10 +978,26 @@ class _DeviceBatches(object):
                                                      self.ab_in[b].data_ptr(), self.mask[b].data_ptr(), sh))
             return None, []
 
-        return self._submit_sweep(photos, L, fill)._replace(info=points)
+        token = self._submit_sweep(photos, L, fill, None if levin is None else levin[:2])
+        return token._replace(info=(points, None if levin is None else (levin[0], levin[2], levels)))
 
     def collect_reveal(self, token):
-        return [RevealResult(p, ab, rgb, pts) for (p, ab, rgb), pts in zip(self._collect_sweep(token), token.info)]
+        points, levin = token.info
+        out = [RevealResult(p, ab, rgb, pts) for (p, ab, rgb), pts in zip(self._collect_sweep(token), points)]
+        if levin is not None:
+            tol, idx, levels = levin
+            V = len(levels)
+            iters = token.slot.iters.h_out.numpy()[:token.n * V].reshape(token.n, V, 2)
+            relres = token.slot.relres.h_out.numpy()[:token.n * V].reshape(token.n, V, 2)
+            for i in range(token.n):
+                for j in range(V):
+                    if not relres[i, j].max() <= tol:         # NaN included
+                        raise RuntimeError("reveal_sweep(method='levin'): photo %d, level %d did not converge: relative "
+                                           "residual %.3g > %.3g after %d iterations" % (
+                                               idx[i], levels[j], relres[i, j].max(), tol, iters[i, j].max()))
+            if self.levin_log is not None:
+                self.levin_log.extend(iters[i].copy() for i in range(token.n))
+        return out
 
     def submit_stats(self, photos):
         """One device pass of global_stats: prep -> idc_global_stats_batch -> D2H of the [n,316] rows."""

@@ -1,8 +1,10 @@
 """Float64 numpy statement of the Levin baseline (DESIGN.md §4b), the oracle of idc_levin_weights / idc_levin_solve:
 the weight rule (vectorised, each operation in the order the kernel rounds it), the reachability rule (a breadth-first
 search over non-zero weights from the hinted pixels) and a direct sparse solve on the pixels that reach a hint, with 0
-on the rest."""
+on the rest; the solver's right-hand side and true relative residual rounded as the kernel rounds them, and the layout
+of its workspace."""
 import collections
+import math
 
 import numpy as np
 import scipy.sparse as sp
@@ -122,6 +124,63 @@ def solve(w, ab_hint, mask):
         b = Wrh @ ab_hint[c, hinted.reshape(-1)]
         u[c, ridx] = sla.spsolve(A, b)
     return u.reshape(2, h, wd)
+
+
+def rhs(w, ab_hint, mask):
+    """b [2,h,w] float64 of the system reduced to the free pixels: b_p = sum over hinted neighbours q of w_pq c_q on
+    free p, 0 on hinted p.  Summed over k in neighbour order with each product and sum rounded on its own, from the
+    float32 hint, as levin_rhs in idc_levin.cu does, so it is the solver's b bit for bit."""
+    _, h, wd = w.shape
+    hinted = np.asarray(mask).reshape(h, wd) > 0
+    c = np.asarray(ab_hint, np.float32).reshape(2, h, wd).astype(np.float64)
+    b = np.zeros((2, h, wd))
+    for k, (dy, dx) in enumerate(OFFSETS):
+        hq, inside = _shift(hinted, dy, dx)
+        for ch in range(2):
+            cq, _ = _shift(c[ch], dy, dx)
+            b[ch] = np.where(inside & hq, b[ch] + w[k] * cq, b[ch])
+    b[:, hinted] = 0.0
+    return b
+
+
+def _apply(w, x, hinted):
+    """(A x)_p = x_p - sum_q w_pq x_q on free p (0 on hinted p), with x taken as 0 on hinted pixels: levin_apply's
+    order and roundings."""
+    x = np.where(hinted, 0.0, x)
+    acc = np.zeros_like(x)
+    for k, (dy, dx) in enumerate(OFFSETS):
+        xq, inside = _shift(x, dy, dx)
+        acc = np.where(inside, acc + w[k] * xq, acc)
+    return np.where(hinted, 0.0, x - acc)
+
+
+def residual(w, ab_hint, mask, u):
+    """The true relative residual ||b - A u||_2 / ||b||_2 of each channel -> float64 [2]; u [2,h,w], its hinted entries
+    ignored; 0 for a channel whose b is 0.  Each element b_p - (A u)_p is rounded as the solver's true-residual check
+    rounds it, and the squares are summed exactly (math.fsum), so only the order of the solver's final sum differs."""
+    _, h, wd = w.shape
+    hinted = np.asarray(mask).reshape(h, wd) > 0
+    b = rhs(w, ab_hint, mask)
+    out = np.zeros(2)
+    for ch in range(2):
+        r = b[ch] - _apply(w, np.asarray(u[ch], np.float64), hinted)
+        nb = math.fsum((b[ch] * b[ch]).ravel())
+        if nb > 0:
+            out[ch] = math.sqrt(math.fsum((r * r).ravel())) / math.sqrt(nb)
+    return out
+
+
+# The solver workspace's vectors per image and channel, in levin_solve_kernel's order (idc_levin.cu)
+WS_VECS = ("u", "r", "rhat", "p", "v", "t")
+
+
+def workspace(ws, h, w, image, channel, vec="u"):
+    """One FP64 vector [h,w] of idc_levin_solve's workspace (a host copy, any dtype: it is viewed as float64): by
+    default the solution u.  The layout is levin_solve_kernel's (idc_levin.cu): vector v of channel c of image i
+    starts at double ((i * 2 + c) * 6 + v) * h * w, v in WS_VECS order; r holds s in place during an iteration."""
+    d = np.ascontiguousarray(ws).reshape(-1).view(np.float64)
+    o = ((image * 2 + channel) * len(WS_VECS) + WS_VECS.index(vec)) * h * w
+    return d[o:o + h * w].reshape(h, w)
 
 
 def matrix_rows(w, hinted):

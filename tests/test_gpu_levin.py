@@ -30,13 +30,14 @@ def _st():
     return torch.cuda.current_stream().cuda_stream
 
 
-def _edges_photo(X):
-    """Flat regions with hard edges between them, and one ramp."""
-    a = np.zeros((X, X, 3), np.uint8)
-    a[:, :X // 2] = (20, 40, 200)
-    a[:, X // 2:] = (240, 230, 30)
-    a[X // 2:, :X // 3] = (128, 128, 128)
-    a[:X // 3, X // 2:, 0] = np.linspace(120, 250, X - X // 2).astype(np.uint8)
+def _edges_photo(H, W=None):
+    """Flat regions with hard edges between them, and one ramp: H x W (H x H by default)."""
+    W = H if W is None else W
+    a = np.zeros((H, W, 3), np.uint8)
+    a[:, :W // 2] = (20, 40, 200)
+    a[:, W // 2:] = (240, 230, 30)
+    a[H // 2:, :W // 3] = (128, 128, 128)
+    a[:H // 3, W // 2:, 0] = np.linspace(120, 250, W - W // 2).astype(np.uint8)
     return a
 
 
@@ -94,7 +95,7 @@ def test_weights_equal_the_oracle(X):
         bad = ~tiny & (np.abs(got[i] - want) > 1e-13 * np.abs(want))
         assert not bad.any(), (i, np.argwhere(bad)[:5])
         assert ((got[i] == 0) == (want == 0)).mean() > 0.999
-    assert (got[-1] == 0).any()                          # the hard edges make weights underflow to 0
+    assert (got[-1] == 0).any()                          # neighbours outside the image weigh 0
 
 
 REPORT = []

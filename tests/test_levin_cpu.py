@@ -1,11 +1,13 @@
 """CPU: the Levin baseline of reveal sweeps -- its float64 oracle (tests/levin_ref.py: the weight rule, its floors, the
-reachability rule and the degenerate cases), the argument checks of idc_levin_solve (idc_levin_check and the device
+reachability rule and the degenerate cases, the solver's right-hand side, true residual and workspace layout), the
+argument checks of idc_levin_solve (idc_levin_check and the device
 entry points, IDC_ERR_ARG before any device call), the method's argument checks and the command line."""
 import ctypes
 import os
 
 import numpy as np
 import pytest
+import scipy.sparse as sp
 
 import ideepcolor_b200 as cli
 from interactive_deep_colorization_b200 import _lib, photos
@@ -136,6 +138,92 @@ def test_level_zero_is_zero():
     w = levin_ref.weights(_smooth(10, 12, 4))
     u = levin_ref.solve(w, np.full((2, 10, 12), 9.0, np.float32), np.zeros((10, 12), np.float32))
     assert (u == 0).all()
+
+
+def _hints(L, frac, seed):
+    """A mask of about frac of the pixels and hint planes with a colour on EVERY pixel (free ones too: not hints)."""
+    rs = np.random.RandomState(seed)
+    mask = (rs.rand(*L.shape) < frac).astype(np.float32)
+    ab = (rs.rand(2, *L.shape) * 200 - 100).astype(np.float32)
+    return ab, mask
+
+
+@pytest.mark.parametrize("L", [_smooth(17, 23, 5), _edges(20, 26), _smooth(2, 9, 6)])
+def test_rhs_is_the_hinted_columns_summed_in_neighbour_order(L):
+    w = levin_ref.weights(L)
+    ab, mask = _hints(L, 0.3, 7)
+    hinted = mask > 0
+    b = levin_ref.rhs(w, ab, mask)
+    assert (b[:, hinted] == 0).all()
+    # bit for bit: a scalar loop over k in neighbour order, each product and sum rounded on its own
+    h, wd = L.shape
+    for y in range(h):
+        for x in range(wd):
+            if hinted[y, x]:
+                continue
+            for c in range(2):
+                acc = 0.0
+                for k, (dy, dx) in enumerate(levin_ref.OFFSETS):
+                    yy, xx = y + dy, x + dx
+                    if 0 <= yy < h and 0 <= xx < wd and hinted[yy, xx]:
+                        acc = acc + float(w[k, y, x]) * float(ab[c, yy, xx])
+                assert b[c, y, x] == acc, (c, y, x)
+    # and W_fh c_h of the sparse matrix solve() builds, to rounding
+    rows, cols, vals = levin_ref._edges(w)
+    W = sp.csr_matrix((vals, (rows, cols)), shape=(L.size, L.size))
+    for c in range(2):
+        want = W[:, hinted.ravel()] @ ab[c].ravel()[hinted.ravel()].astype(np.float64)
+        want[hinted.ravel()] = 0
+        assert np.abs(b[c].ravel() - want).max() <= 1e-13 * max(np.abs(want).max(), 1)
+
+
+def test_residual_is_the_true_relative_residual():
+    L = _smooth(19, 21, 8)
+    w = levin_ref.weights(L)
+    ab, mask = _hints(L, 0.05, 9)
+    hinted = mask > 0
+    b = levin_ref.rhs(w, ab, mask)
+    # u = 0: r = b exactly
+    assert levin_ref.residual(w, ab, mask, np.zeros((2,) + L.shape)).tolist() == [1.0, 1.0]
+    # the direct solve: a residual at rounding level
+    u = levin_ref.solve(w, ab, mask)
+    assert (levin_ref.residual(w, ab, mask, u) <= 1e-13).all()
+    # a perturbed u: against the sparse matrix of matrix_rows, to rounding; the hinted entries of u do not count
+    rs = np.random.RandomState(10)
+    v = u + rs.randn(*u.shape) * 1e-3
+    v[:, hinted] = 1e30
+    A = levin_ref.matrix_rows(w, hinted)
+    free = ~hinted.ravel()
+    got = levin_ref.residual(w, ab, mask, v)
+    for c in range(2):
+        x = np.where(hinted, 0.0, v[c]).ravel()
+        r = (b[c].ravel() - A @ x)[free]
+        want = np.linalg.norm(r) / np.linalg.norm(b[c])
+        assert abs(got[c] - want) <= 1e-12 * want
+    # a channel whose b is 0 (every hint 0 in a): 0
+    ab0 = ab.copy()
+    ab0[0][hinted] = 0
+    assert levin_ref.residual(w, ab0, mask, v)[0] == 0.0
+
+
+def test_workspace_reads_each_vector_at_its_offset():
+    n, h, w, V = 3, 4, 5, len(levin_ref.WS_VECS)
+    hw = h * w
+    # a synthetic buffer: the double at ((i * 2 + c) * 6 + v) * hw + p holds i * 1e4 + c * 1e3 + v * 1e2 + p
+    ws = np.zeros(n * 2 * V * hw)
+    for i in range(n):
+        for c in range(2):
+            for v in range(V):
+                o = ((i * 2 + c) * V + v) * hw
+                ws[o:o + hw] = i * 1e4 + c * 1e3 + v * 1e2 + np.arange(hw)
+    raw = ws.view(np.uint8)                       # a byte copy, as a device workspace comes back
+    for i in range(n):
+        for c in range(2):
+            for v, name in enumerate(levin_ref.WS_VECS):
+                want = (i * 1e4 + c * 1e3 + v * 1e2 + np.arange(hw)).reshape(h, w)
+                assert np.array_equal(levin_ref.workspace(raw, h, w, i, c, name), want), (i, c, name)
+            assert np.array_equal(levin_ref.workspace(ws, h, w, i, c), levin_ref.workspace(raw, h, w, i, c, "u"))
+    assert _lib.load().idc_levin_workspace_bytes(n, h, w) == ws.nbytes     # the C ABI sizes exactly this layout
 
 
 def test_levin_abi_argument_checks():

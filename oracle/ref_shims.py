@@ -3,8 +3,9 @@
 The reference wrapper needs matplotlib and scikit-image, both absent here
 (data/colorize_image.py:3-4).  We inject a stub ``matplotlib`` and a ``skimage.color``
 backed by oracle/color_ref.py into sys.modules, then import the reference modules as
-they are.  Where no checkout exists, callers must check
-``reference_available()`` and skip.
+they are.  Where neither a checkout nor the staged copy exists, ``reference_available()``
+is False: bench.py's CPU arm then times the oracle port, and the live-reference tests
+(tests/live_ref.py) fail rather than skip.
 
 Test infrastructure only -- see oracle/__init__.py.
 """
@@ -40,9 +41,10 @@ def full_reference_available():
 
 def stage_reference(src="/root/reference"):
     """Build step (called by __graft_entry__.build()): copy the reference's own network + wrapper files,
-    byte for byte, into the git-ignored oracle/_ref/ so that a machine without the checkout can
-    time the UNMODIFIED reference CPU path in `bench.py --impl reference`.  Nothing staged is product or test source:
-    oracle/_ref/ is listed in .gitignore (never committed) and only bench.py's CPU arm reads it."""
+    byte for byte, into the git-ignored oracle/_ref/ so that a machine without the checkout can run the
+    UNMODIFIED reference: `bench.py --impl reference` times its CPU path, and the live-reference tests
+    (tests/live_ref.py, tests/test_live_reference_cpu.py, tests/test_gpu_live_reference.py) compare the port
+    with it.  Nothing staged is product or test source: oracle/_ref/ is listed in .gitignore (never committed)."""
     import shutil
     if not os.path.isfile(os.path.join(src, "models", "pytorch", "model.py")):
         return False

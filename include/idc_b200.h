@@ -194,9 +194,9 @@ int idc_fetch_dist(idc_ctx* ctx, int img, int y4, int x4, float* out_host);
  * BEFORE the forward which pixel (img, y4, x4) of the (h/4 x w/4) distribution grid the user clicked and how many colour
  * suggestions K (0 = none) the GUI will ask for.  The next idc_forward_host(_q) with n <= 4 and resident mode on then
  * also gathers that pixel's 529-bin pmf and clusters it (idc_ab_reccs with the default 8 restarts / 100 iterations /
- * PyTorch gamut grid) on the dist head's side branch of the click graph -- off the critical path -- and brings the 8 KB
- * answer back with the same graph launch: idc_fetch_dist / idc_ab_reccs for the same pixel (and K) then return from
- * pinned host memory without touching the device.  The coordinates live in mapped host memory and are read when the
+ * PyTorch gamut grid) on the dist head's side branch of the click graph -- off the critical path -- and brings the
+ * pmf and the picked suggestions (2.6 KB) back with the same graph launch: idc_fetch_dist / idc_ab_reccs for the same
+ * pixel (and K) then return from pinned host memory without touching the device.  The coordinates live in mapped host memory and are read when the
  * graph runs, so moving the click never re-captures the graph.  y4 < 0 switches the mode off (one re-capture). */
 int idc_set_click(idc_ctx* ctx, int img, int y4, int x4, int K);
 
@@ -208,7 +208,9 @@ int idc_set_click(idc_ctx* ctx, int img, int y4, int x4, int K);
  * or max_iter); n_init restarts run side by side (restart v seeds from the bin of weight-rank v) and the one
  * with the lowest inertia wins (sklearn's n_init; 1 <= n_init <= 16).  pts_host: [529][2] ab coordinates of the bins, or NULL for the PyTorch wrapper's grid
  * (bin i = (g[i % 23], g[i / 23]), g = -110..110 step 10, :283).  Outputs (host): centers [K][2], conf [K]
- * (cluster mass, descending; may be NULL), iters_out (Lloyd iterations used; may be NULL).  1 <= K <= 32. */
+ * (cluster mass, descending; may be NULL), iters_out (Lloyd iterations used; may be NULL).  1 <= K <= 32.  The best
+ * restart is picked on the device.  Runs on the legacy default stream in the context scratch of idc_ab_reccs_batch:
+ * a batched call still running on another stream must be waited for first. */
 int idc_ab_reccs(idc_ctx* ctx, int img, int y4, int x4, int K, int max_iter, int n_init, const float* pts_host,
                  float* centers_host, float* conf_host, int* iters_out);
 /* Same clustering for a caller-supplied pmf (host, 529 floats, need not be normalised); no ctx needed. */

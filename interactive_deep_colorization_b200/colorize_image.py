@@ -680,13 +680,8 @@ class ColorizeImageB200Dist(_DistPlots, ColorizeImageB200):
         if not self.dist_ab_set:
             print('Need to set prediction first')
             return 0
-        if method == 'gpu':
-            if not self.materialize_full:                    # the pixel's pmf never leaves the device
-                centers, conf, _ = self._dist_ctx.ab_reccs(0, int(h) // 4, int(w) // 4, K=K, pts=self.pts_in_hull)
-            else:
-                from .prepost import ab_reccs_pmf_gpu
-                centers, conf, _ = ab_reccs_pmf_gpu(np.asarray(self.dist_ab[:, h, w]), K=K, pts=self.pts_in_hull,
-                                                    device=self._dist_ctx.device)
+        if method == 'gpu':                                  # the distribution of the last forward is still on the device
+            centers, conf, _ = self._dist_ctx.ab_reccs(0, int(h) // 4, int(w) // 4, K=K, pts=self.pts_in_hull)
             centers, conf = centers.astype(np.float64), conf.astype(np.float64)
             return (centers, conf) if return_conf else centers
         if method != 'sampled':
@@ -952,22 +947,19 @@ class ColorizeImageB200CaffeDist(_DistPlots, ColorizeImageB200Caffe):
 
     def get_ab_reccs(self, h, w, K=5, N=25000, return_conf=False, method='gpu'):
         """reference :515-547 on the 313 in-gamut bins.  method='gpu': weighted k-means on the device (the N -> infinity
-        limit, as ColorizeImageB200Dist); method='sampled': the reference's np.random + sklearn procedure."""
+        limit, as ColorizeImageB200Dist; idc_caffe313_reccs_batch on this one pixel); method='sampled': the reference's
+        np.random + sklearn procedure."""
         if not self.dist_ab_set:
             print('Need to set prediction first')
             return 0
-        pmf = np.asarray(self.dist_ab[:, int(h), int(w)], dtype=np.float64)
         if method == 'gpu':
-            from .prepost import ab_reccs_pmf_gpu
-            p529, q529 = np.zeros(529, np.float32), np.zeros((529, 2), np.float32)     # the kernel clusters 529 slots;
-            p529[:313], q529[:313] = pmf, self.pts_in_hull                              # zero-weight padding is inert
-            centers, conf, _ = ab_reccs_pmf_gpu(p529, K=K, pts=q529, device=self._ctx.device)
-            centers, conf = centers.astype(np.float64), conf.astype(np.float64)
+            centers, conf, _ = self._ctx.caffe313_reccs_batch([(0, int(h), int(w))], K, S=self.S)
+            centers, conf = centers[0].cpu().numpy().astype(np.float64), conf[0].cpu().numpy().astype(np.float64)
             return (centers, conf) if return_conf else centers
         if method != 'sampled':
             raise ValueError("method must be 'gpu' or 'sampled'")
         from sklearn.cluster import KMeans
-        cmf = np.cumsum(pmf)
+        cmf = np.cumsum(np.asarray(self.dist_ab[:, int(h), int(w)], dtype=np.float64))
         cmf /= cmf[-1]
         samples = self.pts_in_hull[np.digitize(np.random.uniform(low=0, high=1.0, size=N), bins=cmf), :]
         km = KMeans(n_clusters=K).fit(samples)

@@ -648,19 +648,23 @@ struct HostCopy {
 // the copy list, in issue order: the inputs, then the outputs
 enum { kCpHints, kCpL, kCpAb, kCpMask, kCpGlob, kCpOutAb, kCpRgb, kCpAbq, kCpDist, kNumCopies };
 
+// The picked suggestions of one pixel (idc_ab_reccs, the announced click) as they sit on the device and come back:
+// the first K entries of each array hold the answer
+struct alignas(8) ReccsAnswer { float centers[2 * 32], mass[32]; int32_t iters; };
+
 // idc_set_click: layout of the click answer block (device d_clickout, pinned host h_clickout)
 constexpr int kClickInit = 8, kClickMaxIter = 100;                       // the defaults of LhnContext.ab_reccs
-constexpr size_t kClickHdr = 32, kClickPmf = 544 * sizeof(float);
-constexpr size_t kClickRes = (size_t)kClickInit * (3 * 32 + 2) * sizeof(double);
-constexpr size_t kClickCopy = kClickHdr + kClickPmf + kClickRes;         // what travels back per click
-constexpr size_t kClickBytes = kClickCopy + 529 * 2 * sizeof(float);     // + the default gamut grid (device only)
+constexpr size_t kClickHdr = 32, kClickPmf = 544 * sizeof(float), kClickAns = kClickHdr + kClickPmf;
+constexpr size_t kClickCopy = kClickAns + sizeof(ReccsAnswer);           // what travels back per click
+constexpr size_t kClickRes = (size_t)kClickInit * kReccsRes * sizeof(double);
+constexpr size_t kClickBytes = kClickCopy + kClickRes + 529 * 2 * sizeof(float);   // + every restart, the default grid
 
 cudaError_t new_stream(Stream& s) { return cudaStreamCreateWithFlags(s.put(), cudaStreamNonBlocking); }
 cudaError_t new_event(Event& e) { return cudaEventCreateWithFlags(e.put(), cudaEventDisableTiming); }
 
 // After the class conv of a small-batch forward: the clicked pixel's pmf straight from its 529 logits (same per-row
-// softmax routine as the full map, so the same bits), K-means on it (K from the click header), the block to pinned host
-// memory.  Runs next to the full-map softmax on a branch of the dist head's side branch.
+// softmax routine as the full map, so the same bits), the suggestions for it (K from the click header), the header, pmf
+// and picked answer to pinned host memory.  Runs next to the full-map softmax on a branch of the dist head's side branch.
 bool click_tail_on(Ctx* c, int n) { return c->click_mode && c->click && n <= 4; }
 
 cudaError_t click_tail(Ctx* c, int n, cudaStream_t st) {
@@ -668,12 +672,14 @@ cudaError_t click_tail(Ctx* c, int n, cudaStream_t st) {
   char* out = c->click->d_clickout.get();
   int* hdr = reinterpret_cast<int*>(out);
   float* pmf = reinterpret_cast<float*>(out + kClickHdr);
-  double* res = reinterpret_cast<double*>(out + kClickHdr + kClickPmf);
-  const float* pts = reinterpret_cast<const float*>(out + kClickCopy);
+  ReccsAnswer* ans = reinterpret_cast<ReccsAnswer*>(out + kClickAns);
+  double* res = reinterpret_cast<double*>(out + kClickCopy);
+  const float* pts = reinterpret_cast<const float*>(out + kClickCopy + kClickRes);
   cudaError_t e = launch_click_pmf(c, c->click->d_click, n, hdr, pmf, st);
   if (e != cudaSuccess) return e;
-  if ((e = launch_ab_reccs(pmf, 1, pts, 0, kClickMaxIter, kClickInit, res, st, hdr)) != cudaSuccess) return e;
-  c->launch_count += 2;
+  e = launch_reccs(pmf, 1, 1, pts, 0, kClickMaxIter, kClickInit, res, ans->centers, ans->mass, &ans->iters, st, hdr);
+  if (e != cudaSuccess) return e;
+  c->launch_count += 3;
   return cudaMemcpyAsync(c->click->h_clickout.get(), out, kClickCopy, cudaMemcpyDeviceToHost, st);
 }
 
@@ -1314,9 +1320,9 @@ int idc_set_click(idc_ctx* c, int img, int y4, int x4, int K) {
     CUDA_TRY(c, cudaMemset(g->d_clickout.get(), 0, kClickBytes));
     CUDA_TRY(c, cudaMallocHost(g->h_clickout.put(), kClickCopy));
     memset(g->h_clickout.get(), 0, kClickCopy);
-    float pts[529 * 2];   // the PyTorch wrapper's gamut grid (data/colorize_image.py:283): bin i = (g[i % 23], g[i / 23])
-    for (int i = 0; i < 529; ++i) { pts[2 * i] = -110.f + 10.f * (i % 23); pts[2 * i + 1] = -110.f + 10.f * (i / 23); }
-    CUDA_TRY(c, cudaMemcpy(g->d_clickout.get() + kClickCopy, pts, sizeof(pts), cudaMemcpyHostToDevice));
+    float pts[529 * 2];
+    reccs_points(nullptr, pts);
+    CUDA_TRY(c, cudaMemcpy(g->d_clickout.get() + kClickCopy + kClickRes, pts, sizeof(pts), cudaMemcpyHostToDevice));
     c->click = std::move(g);
   }
   volatile int* h = c->click->h_click.get();
@@ -1349,40 +1355,52 @@ int idc_fetch_dist(idc_ctx* c, int img, int y4, int x4, float* out) {
   return IDC_OK;
 }
 
-// shared by idc_ab_reccs / idc_ab_reccs_pmf.  scratch (doubles): [kReccsMaxInit][3*32+2] results, then the 529x2
-// gamut points as floats.
-constexpr size_t kReccsScratchBytes = (size_t)kReccsMaxInit * kReccsRes * sizeof(double) + 529 * 2 * sizeof(float);
-
 static bool reccs_args_ok(int K, int max_iter, int n_init) {
   return K >= 1 && K <= 32 && max_iter >= 1 && n_init >= 1 && n_init <= kReccsMaxInit;
 }
 
-// the restart reccs_best picks, as float32 outputs
-static void reccs_pick(const double* res, int K, int n_init, float* centers_host, float* conf_host, int* iters_out) {
-  const int stride = 3 * K + 2;
-  const double* r = res + (size_t)reccs_best(res, K, n_init) * stride;
-  for (int i = 0; i < 2 * K; ++i) centers_host[i] = (float)r[i];
-  if (conf_host) for (int k = 0; k < K; ++k) conf_host[k] = (float)r[2 * K + k];
-  if (iters_out) *iters_out = (int)r[3 * K];
+static bool reccs_default_points(const float* pts_host) {
+  float g[529 * 2];
+  reccs_points(nullptr, g);
+  return !pts_host || std::equal(g, g + 529 * 2, pts_host);
 }
 
-static cudaError_t reccs_run(const float* pmf_dev, size_t bin_stride, double* scratch, int K, int max_iter, int n_init,
-                             const float* pts_host, float* centers_host, float* conf_host, int* iters_out) {
+static void reccs_answer(const ReccsAnswer& a, int K, float* centers_host, float* conf_host, int* iters_out) {
+  memcpy(centers_host, a.centers, 2 * K * sizeof(float));
+  if (conf_host) memcpy(conf_host, a.mass, K * sizeof(float));
+  if (iters_out) *iters_out = a.iters;
+}
+
+// idc_ab_reccs / idc_ab_reccs_pmf: launch_reccs on one pmf on the device (bins bin_stride floats apart), in suggestion
+// scratch for one query, on the legacy default stream.  The answer takes the scratch's pmf slot, which a pmf already on
+// the device leaves free, and comes back in one copy.
+static cudaError_t reccs_pixel(char* scratch, const float* pmf_dev, size_t bin_stride, int K, int max_iter, int n_init,
+                               const float* pts_host, float* centers_host, float* conf_host, int* iters_out) {
+  const ReccsScratch s(scratch, 1);
+  ReccsAnswer* ans = reinterpret_cast<ReccsAnswer*>(s.pmf);
   float pts[529 * 2];
-  if (pts_host) {
-    memcpy(pts, pts_host, sizeof(pts));
-  } else {   // the PyTorch wrapper's gamut grid (data/colorize_image.py:283, quirk q3): bin i = (g[i % 23], g[i / 23])
-    for (int i = 0; i < 529; ++i) { pts[2 * i] = -110.f + 10.f * (i % 23); pts[2 * i + 1] = -110.f + 10.f * (i / 23); }
+  reccs_points(pts_host, pts);
+  cudaError_t e = cudaMemcpy(s.pts, pts, sizeof(pts), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess)
+    e = launch_reccs(pmf_dev, bin_stride, 1, s.pts, K, max_iter, n_init, s.res, ans->centers, ans->mass, &ans->iters, 0);
+  ReccsAnswer a;
+  if (e == cudaSuccess) e = cudaMemcpy(&a, ans, sizeof(a), cudaMemcpyDeviceToHost);
+  if (e == cudaSuccess) reccs_answer(a, K, centers_host, conf_host, iters_out);
+  return e;
+}
+
+// The context's suggestion scratch, room for q queries.  Grows stream-ordered: neither the release nor the allocation
+// waits for the device.
+static cudaError_t reccs_batch_scratch(Ctx* c, int q, cudaStream_t st) {
+  if (q <= c->reccs_batch_q) return cudaSuccess;
+  if (c->d_reccs_batch.get()) {
+    const cudaError_t e = cudaFreeAsync(c->d_reccs_batch.release(), st);
+    if (e != cudaSuccess) return e;
   }
-  float* pts_dev = reinterpret_cast<float*>(scratch + (size_t)kReccsMaxInit * kReccsRes);
-  cudaError_t e = cudaMemcpy(pts_dev, pts, sizeof(pts), cudaMemcpyHostToDevice);
-  if (e != cudaSuccess) return e;
-  if ((e = launch_ab_reccs(pmf_dev, bin_stride, pts_dev, K, max_iter, n_init, scratch, 0)) != cudaSuccess) return e;
-  const int stride = 3 * K + 2;
-  double res[kReccsMaxInit * kReccsRes];
-  if ((e = cudaMemcpy(res, scratch, (size_t)n_init * stride * sizeof(double), cudaMemcpyDeviceToHost)) != cudaSuccess) return e;
-  reccs_pick(res, K, n_init, centers_host, conf_host, iters_out);
-  return cudaSuccess;
+  c->reccs_batch_q = 0;
+  const cudaError_t e = cudaMallocAsync(reinterpret_cast<void**>(c->d_reccs_batch.put()), reccs_batch_scratch_bytes(q), st);
+  if (e == cudaSuccess) c->reccs_batch_q = q;
+  return e;
 }
 
 int idc_ab_reccs(idc_ctx* c, int img, int y4, int x4, int K, int max_iter, int n_init, const float* pts_host,
@@ -1396,26 +1414,18 @@ int idc_ab_reccs(idc_ctx* c, int img, int y4, int x4, int K, int max_iter, int n
   if (y4 < 0 || y4 >= H4 || x4 < 0 || x4 >= W4) return fail(c, IDC_ERR_ARG, "pixel (%d,%d) outside the %dx%d grid", y4, x4, H4, W4);
   const size_t HW = (size_t)c->H * c->W, HW4 = (size_t)H4 * W4;
   // idc_set_click with the same pixel and K, default restarts / iterations / gamut grid: the click graph already
-  // clustered this pmf on its side branch and the results are in pinned host memory
+  // answered for this pmf on its side branch and the answer is in pinned host memory
   const char* clickout = c->click ? c->click->h_clickout.get() : nullptr;
   if (click_answers(c, img, y4, x4) && reinterpret_cast<const int*>(clickout)[3] == K && max_iter == kClickMaxIter &&
-      n_init == kClickInit) {
-    bool default_pts = pts_host == nullptr;
-    if (!default_pts) {
-      default_pts = true;
-      for (int i = 0; i < 529 && default_pts; ++i)
-        default_pts = pts_host[2 * i] == -110.f + 10.f * (i % 23) && pts_host[2 * i + 1] == -110.f + 10.f * (i / 23);
-    }
-    if (default_pts) {
-      reccs_pick(reinterpret_cast<const double*>(clickout + kClickHdr + kClickPmf), K, n_init, centers_host, conf_host,
-                 iters_out);
-      return IDC_OK;
-    }
+      n_init == kClickInit && reccs_default_points(pts_host)) {
+    reccs_answer(*reinterpret_cast<const ReccsAnswer*>(clickout + kClickAns), K, centers_host, conf_host, iters_out);
+    return IDC_OK;
   }
   const float* d = c->stage->d_out.get() + (size_t)c->max_n * 2 * HW + (size_t)img * 529 * HW4 + (size_t)y4 * W4 + x4;
   CUDA_TRY(c, cudaSetDevice(c->dev));
-  if (!c->d_reccs.get()) CUDA_TRY(c, cudaMalloc(c->d_reccs.put(), kReccsScratchBytes));
-  CUDA_TRY(c, reccs_run(d, HW4, c->d_reccs.get(), K, max_iter, n_init, pts_host, centers_host, conf_host, iters_out));
+  CUDA_TRY(c, reccs_batch_scratch(c, 1, 0));
+  CUDA_TRY(c, reccs_pixel(c->d_reccs_batch.get(), d, HW4, K, max_iter, n_init, pts_host, centers_host, conf_host,
+                          iters_out));
   return IDC_OK;
 }
 
@@ -1423,13 +1433,13 @@ int idc_ab_reccs_pmf(int device, const float* pmf_host, int K, int max_iter, int
                      float* centers_host, float* conf_host, int* iters_out) {
   if (!pmf_host || !centers_host || !reccs_args_ok(K, max_iter, n_init)) return IDC_ERR_ARG;
   if (cudaSetDevice(device) != cudaSuccess) return IDC_ERR_CUDA;
+  const size_t scratch = reccs_batch_scratch_bytes(1);
   DevMem<char> buf;
-  if (cudaMalloc(buf.put(), kReccsScratchBytes + 529 * sizeof(float)) != cudaSuccess) return IDC_ERR_CUDA;
-  float* pmf_dev = reinterpret_cast<float*>(buf.get() + kReccsScratchBytes);
+  if (cudaMalloc(buf.put(), scratch + 529 * sizeof(float)) != cudaSuccess) return IDC_ERR_CUDA;
+  float* pmf_dev = reinterpret_cast<float*>(buf.get() + scratch);
   cudaError_t e = cudaMemcpy(pmf_dev, pmf_host, 529 * sizeof(float), cudaMemcpyHostToDevice);
   if (e == cudaSuccess)
-    e = reccs_run(pmf_dev, 1, reinterpret_cast<double*>(buf.get()), K, max_iter, n_init, pts_host, centers_host, conf_host,
-                  iters_out);
+    e = reccs_pixel(buf.get(), pmf_dev, 1, K, max_iter, n_init, pts_host, centers_host, conf_host, iters_out);
   return e == cudaSuccess ? IDC_OK : IDC_ERR_CUDA;
 }
 
@@ -1473,20 +1483,6 @@ static int caffe313_reccs_check(bool head, int n_img, int h, int w, int q, const
   if (rc == IDC_OK && !std::isfinite(S))
     return snprintf(msg, cap, "%s: S = %g is not finite", kReccsHead313.fn, (double)S), IDC_ERR_ARG;
   return rc;
-}
-
-// The context's batched-suggestion scratch, room for q queries.  Grows stream-ordered: neither the release nor the
-// allocation waits for the device.
-static cudaError_t reccs_batch_scratch(Ctx* c, int q, cudaStream_t st) {
-  if (q <= c->reccs_batch_q) return cudaSuccess;
-  if (c->d_reccs_batch.get()) {
-    const cudaError_t e = cudaFreeAsync(c->d_reccs_batch.release(), st);
-    if (e != cudaSuccess) return e;
-  }
-  c->reccs_batch_q = 0;
-  const cudaError_t e = cudaMallocAsync(reinterpret_cast<void**>(c->d_reccs_batch.put()), reccs_batch_scratch_bytes(q), st);
-  if (e == cudaSuccess) c->reccs_batch_q = q;
-  return e;
 }
 
 int idc_ab_reccs_batch(idc_ctx* c, int q, const int32_t* queries_host, int K, int max_iter, int n_init,

@@ -190,7 +190,7 @@ struct HintBlock { HostMem<char> h_hints; DevMem<char> d_hints; };
 // idc_set_click: the clicked pixel's pmf + K colour suggestions ride on a side branch of the click graph
 struct ClickBlock {
   HostMem<int> h_click; int* d_click = nullptr;   // {img, y4, x4, K, seq} in mapped host memory, read when the graph runs
-  DevMem<char> d_clickout; HostMem<char> h_clickout;   // [8-int header | 544 floats pmf | n_init x (3K+2) doubles]
+  DevMem<char> d_clickout; HostMem<char> h_clickout;   // [8-int header | 544 floats pmf | the picked suggestions]
 };
 // dist head off the critical path: class + softmax run on s_side next to decoder levels 9-10; the announced click's
 // pmf + suggestions run on s_click, next to the full-map softmax
@@ -264,8 +264,7 @@ struct Ctx {
   bool chain = false;           // the previous operation on the forward's stream was a kernel of this forward (PDL)
   bool gadd_active = false;     // a global-hints vector was supplied to this forward
   int last_n = 0;
-  DevMem<double> d_reccs;       // idc_ab_reccs scratch (results of every restart, then the 529x2 gamut points)
-  DevMem<char> d_reccs_batch;   // idc_ab_reccs_batch scratch: gamut points, [Q][529] pmfs, every restart of every query
+  DevMem<char> d_reccs_batch;   // colour-suggestion scratch (ReccsScratch) of idc_ab_reccs and the batched calls
   int reccs_batch_q = 0;        // the query count it holds room for
   DevMem<float> d_negent;       // idc_dist_negentropy result, (H/4)*(W/4) floats
   DevMem<float> d_dist313;      // idc_caffe313_dist_pixel result, 320 floats
@@ -310,20 +309,39 @@ cudaError_t launch_decode313(Ctx* c, int n, float T, float* out_ab, cudaStream_t
 cudaError_t launch_dist313_pixel(Ctx* c, int img, int y, int x, float S, float* out313_dev, cudaStream_t st);
 cudaError_t launch_dist313_map(Ctx* c, int n, float S, float* out_dev, cudaStream_t st);
 cudaError_t launch_negentropy(int n, int bins, int hw, const float* dist, float* out, cudaStream_t st);
-// n_query > 1: pmf holds n_query pmfs of 529 bins back to back (bin_stride 1) and out_dev n_query * n_init rows
-cudaError_t launch_ab_reccs(const float* pmf, size_t bin_stride, const float* pts_dev, int K, int max_iter,
-                            int n_init, double* out_dev, cudaStream_t st, const int* dyn = nullptr, int n_query = 1);
 cudaError_t launch_click_pmf(Ctx* c, const int* click_dev, int n_img, int* out_hdr, float* out_pmf, cudaStream_t st);
-// idc_ab_reccs_batch on the device: queries [q][3] (img, y4, x4, HOST memory, checked by the caller), pts [529][2]
-// (HOST memory); scratch = kReccsBatchPtsBytes, then reccs_batch_pmf_bytes(q), then q * kReccsMaxInit * kReccsRes
-// doubles.  The pmfs go to pmf_out when given (else to the scratch).  Stream-ordered: the queries and points reach the
-// device as kernel parameters.
+// Colour suggestions for q pmfs on the device, the one path of every entry point.  Row i of pmf starts at pmf + i * 529,
+// its bins bin_stride floats apart; pts_dev [529][2]; res q * n_init * (3K+2) doubles for every restart.  Writes each
+// row's picked restart: centers [q][K][2], conf [q][K] (may be null), iters [q] (may be null).  dyn (the click header
+// of click_pmf_kernel): K = dyn[3], and nothing is written unless dyn[7] is set and 1 <= K <= 32.
+cudaError_t launch_reccs(const float* pmf, size_t bin_stride, int q, const float* pts_dev, int K, int max_iter,
+                         int n_init, double* res, float* centers, float* conf, int32_t* iters, cudaStream_t st,
+                         const int* dyn = nullptr);
+// The k-means points: the caller's [529][2] pts, or (pts null) the PyTorch wrapper's gamut grid
+// (data/colorize_image.py:283, quirk q3): bin i = (g[i % 23], g[i / 23]), g = -110, -100, ..., 110.
+inline void reccs_points(const float* pts, float* out) {
+  for (int i = 0; i < 529; ++i) {
+    out[2 * i] = pts ? pts[2 * i] : -110.f + 10.f * (i % 23);
+    out[2 * i + 1] = pts ? pts[2 * i + 1] : -110.f + 10.f * (i / 23);
+  }
+}
+// The suggestion scratch for q queries (reccs_batch_scratch_bytes(q)): the k-means points, the [q][529] pmfs, then
+// kReccsMaxInit rows of kReccsRes doubles per query for every restart.
 constexpr int kReccsMaxInit = 16, kReccsRes = 3 * 32 + 2;   // restarts per query, doubles per restart (at K = 32)
 constexpr size_t kReccsBatchPtsBytes = 4352;                 // 529 x 2 floats, rounded up to 256 bytes
 inline size_t reccs_batch_pmf_bytes(int q) { return ((size_t)q * 529 * sizeof(float) + 255) / 256 * 256; }
 inline size_t reccs_batch_scratch_bytes(int q) {
   return kReccsBatchPtsBytes + reccs_batch_pmf_bytes(q) + (size_t)q * kReccsMaxInit * kReccsRes * sizeof(double);
 }
+struct ReccsScratch {
+  float* pts; float* pmf; double* res;
+  ReccsScratch(char* s, int q)
+      : pts(reinterpret_cast<float*>(s)), pmf(reinterpret_cast<float*>(s + kReccsBatchPtsBytes)),
+        res(reinterpret_cast<double*>(s + kReccsBatchPtsBytes + reccs_batch_pmf_bytes(q))) {}
+};
+// idc_ab_reccs_batch on the device: queries [q][3] (img, y4, x4, HOST memory, checked by the caller), pts [529][2]
+// (HOST memory, or null), scratch a ReccsScratch for q.  The pmfs go to pmf_out when given (else to the scratch).
+// Stream-ordered: the queries and points reach the device as kernel parameters.
 cudaError_t launch_reccs_batch(Ctx* c, int q, const int32_t* queries, const float* pts, int K, int max_iter, int n_init,
                                char* scratch, float* centers, float* conf, int32_t* iters, float* pmf_out,
                                cudaStream_t st);
@@ -547,29 +565,6 @@ __device__ __forceinline__ double zoom_sample(const double* __restrict__ p, int 
   s = __dadd_rn(s, __dmul_rn(__dmul_rn(v01, ty.w0), tx.w1));
   s = __dadd_rn(s, __dmul_rn(__dmul_rn(v10, ty.w1), tx.w0));
   return __dadd_rn(s, __dmul_rn(__dmul_rn(v11, ty.w1), tx.w1));
-}
-
-// Colour suggestions: which of n_init k-means restarts wins.  res = n_init rows of 3K+2 doubles ([K][2] centres, [K]
-// mass, iterations, inertia).  Lowest inertia; restarts within 1e-9 (relative) of it count as ties -> lowest index.
-// The one definition of the rule, for the host pick of idc_ab_reccs and reccs_pick_kernel: on the device the threshold
-// is rounded step by step as on the host (no FMA), so both pick the same restart.  The walk stops at the last restart:
-// a negative inertia (negative weights, i.e. a caller's pmf with negative entries) puts the threshold below the
-// minimum, and an unbounded walk would read past the rows.
-__host__ __device__ __forceinline__ int reccs_best(const double* res, int K, int n_init) {
-  const int stride = 3 * K + 2;
-  double best = res[stride - 1];
-  for (int v = 1; v < n_init; ++v) {
-    const double e = res[v * stride + stride - 1];
-    if (e < best) best = e;
-  }
-#ifdef __CUDA_ARCH__
-  const double thr = __dadd_rn(__dmul_rn(best, 1.0 + 1e-9), 1e-300);
-#else
-  const double thr = best * (1.0 + 1e-9) + 1e-300;
-#endif
-  int pick = 0;
-  while (pick + 1 < n_init && res[pick * stride + stride - 1] > thr) ++pick;
-  return pick;
 }
 
 __device__ __forceinline__ void pdl_prologue_done() {   // small kernels: let the successor start, then wait for the predecessor

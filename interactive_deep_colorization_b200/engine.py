@@ -418,6 +418,14 @@ class LhnContext(object):
                                                  ctypes.byref(iters)))
         return centers, conf, iters.value
 
+    def _reccs_outputs(self, q, K):
+        """The default outputs of the batched suggestion calls: centres [q,K,2] float32, mass [q,K] float32, Lloyd
+        iterations [q] int32, on this context's device."""
+        import torch
+        dev, k = torch.device("cuda:%d" % self.device), max(int(K), 0)
+        return (torch.empty((q, k, 2), dtype=torch.float32, device=dev), torch.empty((q, k), dtype=torch.float32, device=dev),
+                torch.empty((q,), dtype=torch.int32, device=dev))
+
     def ab_reccs_batch(self, queries, K=5, max_iter=100, n_init=8, pts=None, out=None, out_pmf=None):
         """Colour suggestions at many pixels of the last forward's images in one device pass (idc_ab_reccs_batch):
         queries int [Q,3] rows (img, y4, x4) -> (centres [Q,K,2] float32, mass [Q,K] float32, Lloyd iterations [Q]
@@ -430,13 +438,8 @@ class LhnContext(object):
         p = None if pts is None else np.ascontiguousarray(pts, np.float32)
         if p is not None and p.shape != (529, 2):
             raise ValueError("pts: need [529, 2] ab coordinates, got %s" % (p.shape,))
-        dev = torch.device("cuda:%d" % self.device)
-        if out is None:
-            n, k = q.shape[0], max(int(K), 0)
-            out = (torch.empty((n, k, 2), dtype=torch.float32, device=dev), torch.empty((n, k), dtype=torch.float32, device=dev),
-                   torch.empty((n,), dtype=torch.int32, device=dev))
-        centers, conf, iters = out
-        st = torch.cuda.current_stream(dev).cuda_stream
+        centers, conf, iters = out if out is not None else self._reccs_outputs(q.shape[0], K)
+        st = torch.cuda.current_stream(self.device).cuda_stream
         _lib.check(self.h, self.lib.idc_ab_reccs_batch(self.h, int(q.shape[0]), _np_ptr(q), int(K), int(max_iter),
                                                        int(n_init), None if p is None else _np_ptr(p), centers.data_ptr(),
                                                        None if conf is None else conf.data_ptr(),
@@ -478,13 +481,8 @@ class LhnContext(object):
         float32 CUDA tensor [Q,529] that receives each query's padded pmf."""
         import torch
         q = np.ascontiguousarray(queries, np.int32).reshape(-1, 3)
-        dev = torch.device("cuda:%d" % self.device)
-        if out is None:
-            n, k = q.shape[0], max(int(K), 0)
-            out = (torch.empty((n, k, 2), dtype=torch.float32, device=dev), torch.empty((n, k), dtype=torch.float32, device=dev),
-                   torch.empty((n,), dtype=torch.int32, device=dev))
-        centers, conf, iters = out
-        st = torch.cuda.current_stream(dev).cuda_stream
+        centers, conf, iters = out if out is not None else self._reccs_outputs(q.shape[0], K)
+        st = torch.cuda.current_stream(self.device).cuda_stream
         _lib.check(self.h, self.lib.idc_caffe313_reccs_batch(self.h, int(q.shape[0]), _np_ptr(q), float(S), int(K),
                                                              int(max_iter), int(n_init), centers.data_ptr(),
                                                              None if conf is None else conf.data_ptr(),

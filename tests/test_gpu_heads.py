@@ -225,9 +225,9 @@ def test_click_graph_256(nets):
     against the FP64 interval; the fused head's ab as well.
 
     The C ABI does not say whether fetch_dist(0, y4, x4) was answered from the click tail's block or from the resident
-    plane: the launch count shows that the forward ran the click tail (click_pmf_kernel and the k-means, two launches
-    more than the same forward without an announced click), and test_gpu_click pins the answered pixel to the device
-    path bit for bit."""
+    plane: the launch count shows that the forward ran the click tail (click_pmf_kernel, the k-means and the restart
+    pick, three launches more than the same forward without an announced click), and test_gpu_click pins the answered
+    pixel to the device path bit for bit."""
     sd = nets[0]["synth"]
     y4, x4 = 37, 21
     ctx = util.make_ctx(sd, 256, 256, max_n=1, dist=True)
@@ -240,7 +240,7 @@ def test_click_graph_256(nets):
         ctx.set_click(0, y4, x4, K=9)
         ab = ctx.forward_host(*batch, 0.5)["ab"].copy()
         print("click_256: %d launches with the announced click, %d without" % (ctx.last_launch_count(), plain))
-        assert ctx.last_launch_count() == plain + 2
+        assert ctx.last_launch_count() == plain + 3
         check_ab("click_256", sd, ctx, ab, 1, "wgmma", False, 110.0)
         ref = head_ref.dist_head(sd, ctx.get_activation("conv8_3", 1).cpu())
         check_dist("click_256", ctx.fetch_dist(0)[None], ref, "fetch_dist plane")

@@ -73,7 +73,7 @@ def test_resident_distribution_path_and_wrapper(synth_sd):
     assert R.weighted_inertia(pmf, cd.pts_in_hull, centers) <= 1.01 * R.weighted_inertia(pmf, cd.pts_in_hull, ref)
     # a pixel whose 4x4 cell is shared returns the same suggestions (nearest x4 upsample)
     assert np.array_equal(cd.get_ab_reccs(131, 129, K=9), centers)
-    # materialised host distribution takes the ctx-less entry point and agrees
+    # the wrapper that materialises the host distribution agrees
     cm = CI.ColorizeImageB200Dist(Xd=256, maskcent=True, materialize_full=True)
     cm.prep_net(state_dict=synth_sd)
     cm.set_image(g["img_rgb"])
